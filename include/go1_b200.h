@@ -1,5 +1,5 @@
 /*
- * go1_b200.h — C-ABI of libgo1b200.so: the B200-native replacement for the hot path of
+ * go1_b200.h — C-ABI of libgo1b200.so: the H100-native (sm_90a) replacement for the hot path of
  * Improbable-AI/walk-these-ways (LeggedRobot.step() + the ppo_cse learner).
  *
  * Conventions (SURVEY.md §8b):
@@ -293,12 +293,9 @@ int go1_ppo_normalize_advantages(float* advantages, const double* stats, int64_t
  * Row strides let a layer read/write column slices of wider buffers, so cat(obs_history, latent)
  * (actor_critic.py:115) is never materialised.  accumulate: add into C instead of overwriting
  * (bias/act are applied after the accumulation).  act: 0 none, 1 ELU(alpha=1).
- * impl: 0 = fp32 CUDA cores (exact-fp32 path), 1 = tcgen05 TF32 tensor cores with fp32 accumulation. */
+ * impl: 0 = fp32 CUDA cores (exact-fp32 path), 1 = wgmma TF32 tensor cores with fp32 accumulation. */
 int go1_gemm(int transA, int transB, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
              float* C, int ldc, const float* bias, int act, int accumulate, int impl, void* stream);
-/* impl=1 tile selection (default 1): products with K >= 1024, N >= 256 and enough tiles run as cta_group::2 256 x 256 tile pairs
- * (128 x 256 single-CTA tiles when M < 256); 0 forces the 128 x 128 persistent kernel everywhere (a tuning / bisecting switch). */
-void go1_gemm_tf32_set_wide(int on);
 /* Same product with the full fused epilogue, applied in this order to each output element v = sum_k a*b:
  *   v += C_old (accumulate);  v += sum_e extra[m][e] * w_extra[n][e]  (num_extra <= 4: the 2 trailing input columns of
  *   the actor/critic first layer, i.e. cat(obs_history, latent) without the cat);  v += bias[n];
@@ -320,11 +317,11 @@ typedef struct Go1GemmEpilogue {
 } Go1GemmEpilogue;
 int go1_gemm_ex(int transA, int transB, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
                 float* C, int ldc, const Go1GemmEpilogue* ep, int impl, void* stream);
-/* nprob (<= 4) tcgen05 products of the SAME shape and operand strides in one grid: C[p] (+)= op(A[p]) op(B[p]) (impl 1 only, no fused
+/* nprob (<= 4) wgmma products of the SAME shape and operand strides in one grid: C[p] (+)= op(A[p]) op(B[p]) (impl 1 only, no fused
  * epilogue operands).  Used for the equal-shape split-K wgrads of the three MLPs (nn.Linear weight gradients, actor_critic.py:38-77). */
 int go1_gemm_grouped(int transA, int transB, int M, int N, int K, int nprob, const float* const* A, int lda, const float* const* B, int ldb,
                      float* const* C, int ldc, int accumulate, void* stream);
-/* The layers BEHIND a first layer of one of ActorCritic's MLPs in one launch (impl 1, tcgen05; actor_critic.py:38-77, 113-144):
+/* The layers BEHIND a first layer of one of ActorCritic's MLPs in one launch (impl 1, wgmma; actor_critic.py:38-77, 113-144):
  *   y2 = ELU(x W2^T + b2) [M][N2];   y3 = ELU(y2 W3^T + b3) [M][N3]  (N3 = 0: skipped);   out = y_last Wh^T + bh [M][nh], nh <= 16.
  * x is the first layer's activated output (K1 columns, row stride ldx); W* are torch nn.Linear weights [out][in], contiguous; y2 / y3 are
  * kept for the backward pass.  Supported tails: K1-N2-N3 = 512-256-128 (actor / critic bodies of scripts/train.py) and 256-128-0
@@ -342,14 +339,14 @@ int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int nprob, int M, 
 /* Backward of the same bodies, first half, for up to two problems in one grid (nn.Linear / nn.ELU autograd of actor_critic.py:38-77):
  *   dz3 = (dout Wh) * ELU'(y3) [M][N3];  dz2 = (dz3 W3) * ELU'(y2) [M][N2];  gb3 += colsum(dz3);  gb2 += colsum(dz2)   (N3 = 128, N2 = 256, nh <= 12)
  * dout is the gradient of the head's output [M][nh], Wh [nh][N3] and W3 [N3][N2] the nn.Linear weights, y3 / y2 the saved activations;
- * dz3 never leaves the SM between the CUDA-core product and the tcgen05 product.  gb3 / gb2 are accumulated with atomics. */
+ * dz3 never leaves the SM between the CUDA-core product and the wgmma product.  gb3 / gb2 are accumulated with atomics. */
 typedef struct Go1TailBwdProblem {
     const float* dout; int32_t lddout, nh; const float* Wh; const float* y3; int32_t ldy3; const float* W3; const float* y2; int32_t ldy2;
     float* dz3; int32_t lddz3; float* dz2; int32_t lddz2; float* gb3; float* gb2;
 } Go1TailBwdProblem;
 int go1_mlp_tail_backward_grouped(const Go1TailBwdProblem* probs, int nprob, int M, int N3, int N2, void* stream);
 
-/* Per-launch timing of the impl-1 (tcgen05) products for the roofline report: on = 1 starts collecting (CUDA events on the launch
+/* Per-launch timing of the impl-1 (wgmma) products for the roofline report: on = 1 starts collecting (CUDA events on the launch
  * stream around every call that is not being graph-captured), on = 0 stops and returns the summed kernel time, flops and count. */
 int go1_gemm_timing(int on, double* total_ms, double* total_flop, long long* launches);
 /* number of kernels replayed through CUDA graphs, added to go1_kernel_launch_count() by the caller that replays them */

@@ -54,7 +54,7 @@ def test_bench_reference_arm_prints_the_contract_line():
     assert line["impl"] == "reference" and line["metric"] == "env_steps_per_s" and line["unit"] == "env-steps/s" and line["higher_is_better"] is True
     assert line["value"] > 0 and line["cpu_baseline"]["kind"] == "port" and line["cpu_baseline"]["cores"] >= 1
     assert line["e2e"] == {"value": line["value"], "unit": line["unit"], "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
-    # the same workload definition as the B200 arm prints (the bounded sample is named separately), fixed thread count <= 32
+    # the same workload definition as the GPU arm prints (the bounded sample is named separately), fixed thread count <= 32
     assert line["config"]["name"] == "flat" and line["config"]["envs_per_gpu"] == 4096 and line["scaling"] == "weak" and line["warmup"] == 1
     assert "8 envs x 24-step rollout" in line["sample"] and line["cpu_baseline"]["cores"] <= 32
     # other ranks of a torchrun launch do no work and print nothing

@@ -1,5 +1,5 @@
 """Sim-to-sim acceptance (SURVEY.md §8c(7), the scripts/play.py:89-139 scenario): the policy shipped with the reference
-(runs/.../ac_weights_last.pt, stored here as fp16: tests/golden/pretrained_policy_fp16.npz), trained in Isaac Gym, is
+(runs/.../ac_weights_last.pt, stored here as fp16 in slices below 1 MB: tests/golden/pretrained_policy_fp16.part*.npz), trained in Isaac Gym, is
 rolled out in THIS simulator with a 1.5 m/s, 3 Hz trot command for 250 steps.  It must walk forward without falling —
 the only end-to-end check available for the new rigid-body step (PhysX parity is unpinned)."""
 import os
@@ -33,15 +33,36 @@ def _play_env(n):
     return HistoryWrapper(VelocityTrackingEasyEnv(sim_device="cuda:0", headless=True, cfg=Cfg))
 
 
+def _load_policy():
+    """name -> float32 array, reassembled from the flattened slices `name@offset` (+ `name@shape`) of the part files."""
+    import glob
+    flat, shape = {}, {}
+    for fn in sorted(glob.glob(os.path.join(HERE, "golden", "pretrained_policy_fp16.part*.npz"))):
+        z = np.load(fn)
+        for key in z.files:
+            name, tag = key.rsplit("@", 1)
+            if tag == "shape":
+                shape[name] = tuple(int(v) for v in z[key])
+            else:
+                flat.setdefault(name, {})[int(tag)] = z[key]
+    out = {}
+    for name, chunks in flat.items():
+        a = np.concatenate([chunks[o] for o in sorted(chunks)]).astype(np.float32)
+        assert a.size == int(np.prod(shape[name])), name
+        out[name] = a.reshape(shape[name])
+    return out
+
+
 def test_shipped_policy_trots_forward_in_this_simulator():
     from go1_gym_learn.ppo_cse import ActorCritic
     n = 32
     env = _play_env(n)
-    w = np.load(os.path.join(HERE, "golden", "pretrained_policy_fp16.npz"))
+    w = _load_policy()
+    assert len(w) == 15
     ac = ActorCritic(env.num_obs, env.num_privileged_obs, env.num_obs_history, env.num_actions).to("cuda:0")
     sd = ac.state_dict()
-    for k in w.files:
-        sd[k] = torch.from_numpy(w[k].astype(np.float32))
+    for k in w:
+        sd[k] = torch.from_numpy(w[k])
     ac.load_state_dict(sd)
     obs = env.reset()
     vx, resets = [], 0

@@ -133,7 +133,7 @@ def test_clip_adam_matches_torch_optim():
 @pytest.mark.parametrize("impl", [0, 1])
 def test_full_ppo_cycle_matches_reference_golden(impl):
     """BASELINE config 1: act x24 -> process_env_step -> compute_returns -> update (5 epochs x 4 minibatches + adaptation
-    steps) on the reference's own vectors.  impl 0: fp32 CUDA-core GEMMs (tolerances ~1e-4); impl 1: tcgen05 TF32 GEMMs
+    steps) on the reference's own vectors.  impl 0: fp32 CUDA-core GEMMs (tolerances ~1e-4); impl 1: wgmma TF32 GEMMs
     (10-bit mantissa products: tolerances x250 on the rollout quantities, x25 on the losses, stated as `k` / `kl`)."""
     from ppo_golden_util import seeded_weights, sample_tensor
     from go1_gym_learn.ppo_cse import ActorCritic
@@ -182,13 +182,13 @@ def test_full_ppo_cycle_matches_reference_golden(impl):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# tcgen05 TF32 tensor-core GEMM (impl=1).  TF32 keeps 10 mantissa bits: |err| <= ~2^-10 * sum|a||b| per product, so the
+# TF32 tensor-core GEMM (impl=1; wgmma).  TF32 keeps 10 mantissa bits: |err| <= ~2^-10 * sum|a||b| per product, so the
 # tolerance is stated relative to the fp64 reference of |A| |B|^T (torch 1.10, the reference's version, also ran its
 # matmuls in TF32 by default on Ampere+).
 # ----------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("M,N,K", [(128, 128, 32), (128, 64, 64), (4096, 256, 2100), (300, 200, 70), (4, 512, 2100), (1000, 1280, 2100),
                                    (8000, 1280, 1056), (24576, 256, 1024),
-                                   (3584, 1280, 1056), (24576, 1280, 1024), (3500, 1100, 2100),   # 128 x 256 tiles / cta_group::2 pairs (wide heuristic)
+                                   (3584, 1280, 1056), (24576, 1280, 1024), (3500, 1100, 2100),   # many tiles per CTA, long K
                                    (24576, 128, 256), (256, 128, 24576), (2100, 1280, 4096)])
 def test_gemm_tcgen05_tf32(M, N, K):
     torch.manual_seed(M * 7 + N * 3 + K)
@@ -212,7 +212,7 @@ def test_gemm_tcgen05_tf32(M, N, K):
     assert ((C2.double() - want).abs() <= bound + 1e-5).all()
 
 
-# Staged epilogue of the BN <= 128 kernels: 32 x 32 output blocks leave through shared memory + one TMA store per warp, the ELU' operand
+# Staged epilogue: 32 x 32 output blocks leave through shared memory + one TMA store per warp, the ELU' operand
 # arrives through TMA loads (taken when C / dact_y are 16-byte aligned with row strides that are multiples of 4 floats, no accumulate, no split-K).
 # Ragged M and N exercise the TMA clipping; the guard columns behind N and guard rows behind M must stay untouched.
 @pytest.mark.parametrize("tb", [1, 0])
@@ -481,8 +481,8 @@ def test_fused_backward_epilogues_match_separate_kernels(M):
 
 @pytest.mark.parametrize("M", [4, 100, 4096, 24576 + 37])
 def test_fused_mlp_tail_forward_matches_layer_by_layer(M):
-    """go1_mlp_tail_forward (layers behind the first one in ONE tcgen05 launch, activations kept on the SM) against the
-    layer-by-layer tcgen05 path and an fp64 torch evaluation of the same modules: all three MLPs, every saved activation."""
+    """go1_mlp_tail_forward (layers behind the first one in ONE tensor-core launch, activations kept on the SM) against the
+    layer-by-layer tensor-core path and an fp64 torch evaluation of the same modules: all three MLPs, every saved activation."""
     from go1_gym_learn.ppo_cse import ActorCritic
     from go1_gym_learn.ppo_cse.actor_critic import AC_Args
     AC_Args.gemm_impl = 1

@@ -669,8 +669,8 @@ extern "C" int go1_launch_curriculum_pack(const Go1SimBuffers* b, const Go1Curri
     return (int)cudaGetLastError();
 }
 
-// The category-parallel grouped path is ON by default (bit-exact against the host twin in all four curriculum modes on a B200:
-// tests/test_curriculum_gpu.py::test_grouped_path_matches_host_twin; iteration 49.6 -> 48.8 ms); GO1_CUR_GROUPED=0 or
+// The category-parallel grouped path is ON by default (bit-exact against the host twin in all four curriculum modes:
+// tests/test_curriculum_gpu.py::test_grouped_path_matches_host_twin); GO1_CUR_GROUPED=0 or
 // go1_curriculum_set_grouped(0) select the category-by-category path.
 static int g_cur_grouped = -1;
 extern "C" void go1_curriculum_set_grouped(int on) { g_cur_grouped = on ? 1 : 0; }

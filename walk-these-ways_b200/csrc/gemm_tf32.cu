@@ -1,21 +1,20 @@
-// gemm_tf32.cu — hand-written tcgen05 TF32 GEMM for sm_100a (the dense layers of ppo_cse's ActorCritic).
+// gemm_tf32.cu — hand-written wgmma TF32 GEMM for sm_90a (the dense layers of ppo_cse's ActorCritic).
 //
 //   C[M][N] (+)= A[M][K] * B[N][K]^T (+ bias[n]) (ELU)          fp32 in HBM, TF32 multiply, fp32 accumulate
 //
-// The forward products read both operands K-major (A = activations row-major, B = torch.nn.Linear weight [out][in]);
-// dgrad (B = W as [K][N]) and wgrad (A = dz as [K][M], B = activations as [K][N]) read MN-major operands straight from
-// HBM: the TMA boxes become [32 k-rows][32 mn-floats] and the UMMA descriptors / instruction descriptor switch to the
-// MN-major canonical layout, so no transposed copies exist anywhere.  Structure (persistent CTAs, one per SM, 576 threads,
-// walking 128 x BN output tiles; gemm_tf32_2cta pairs two CTAs on 256 x 256 tiles):
-//   warp 0      TMA producer: cp.async.bulk.tensor 2D loads of 128x32 (A) and BNx32 (B) fp32 boxes, 128B swizzle,
-//               ring of 3-8 stages guarded by full/empty mbarriers
-//   warp 1      TMEM allocator + single-thread tcgen05.mma.cta_group::1.kind::tf32 issuer (M=128, N=BN, K=8 per
-//               instruction, 4 per k-block), tcgen05.commit to release smem stages and to publish the accumulator
-//   warps 2-17  epilogue (TMEM lane quarter x column group): tcgen05.ld 32x32b -> registers -> bias / ELU / ELU' / column sums /
-//               trailing-input terms -> swizzled shared memory -> one TMA store per warp and 32 x 32 block (staged epilogue),
-//               red.global.add.v4 when split-K partitions the reduction
-// Accumulators live in TMEM, double-buffered (2 x BN fp32 columns x 128 lanes): the epilogue of tile i overlaps the main loop of
-// tile i+1.  mlp_tail_fwd_kernel chains two such products and a CUDA-core head for the layers behind a first layer.
+// The forward products read both operands K-major (A = activations row-major, B = torch.nn.Linear weight [out][in]).
+// dgrad (B = W as [K][N]) and wgrad (A = dz as [K][M], B = activations as [K][N]) have MN-major operands, and TF32 wgmma
+// multiplies K-major shared-memory tiles only: their TMA boxes ([32 k-rows][tile width], unswizzled) are transposed by the
+// consumer warps from shared memory to shared memory (into the 128B-swizzled K-major form, double-buffered so that the
+// transposition of k-block i + 1 overlaps the tensor-core work on k-block i); no transposed copy exists in HBM.
+// Structure (persistent CTAs, one per SM, 384 threads, walking 128 x BN output tiles):
+//   warps 0-7   two consumer warpgroups, 64 rows x BN columns each: wgmma.mma_async m64nBNk8 (4 per k-block) with the accumulator
+//               in registers, then the epilogue: accumulator -> swizzled shared memory -> one 32 x 32 block per warp at a time,
+//               a row per lane -> bias / ELU / ELU' / column sums / trailing-input terms -> the same block -> one TMA store
+//               (staged epilogue), red.global.add.v4 when split-K partitions the reduction
+//   warp 8      TMA producer: cp.async.bulk.tensor 2D loads of the A and B boxes of a k-block into a ring of 3-8 stages guarded by
+//               full / empty mbarriers; it runs ahead into the next tile while the consumers are in their epilogue
+// mlp_tail_fwd_kernel chains two such products and a CUDA-core head for the layers behind a first layer.
 #include <cuda_runtime.h>
 #include <cuda.h>
 #include <stdint.h>
@@ -24,6 +23,7 @@
 #include <unordered_map>
 #include <stdlib.h>
 #include "../../include/go1_b200.h"
+#include "wgmma_tf32.cuh"
 
 extern int go1_set_error(const char* m);
 void go1_count_launch(int n);
@@ -31,7 +31,7 @@ void go1_count_launch(int n);
 namespace {
 
 constexpr int BM = 128, BK = 32;          // BK fp32 = 128 bytes = one swizzle-128B row
-constexpr int UMMA_K = 8;                 // tf32: 32 bytes per instruction along K
+constexpr int NCONS = 8, EPI_G = 2;       // consumer warps; column groups of the epilogue (warp = (32-row block, column group))
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -61,48 +61,38 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* ba
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-// K-major, 128B-swizzled operand tile: 8-row groups 1024 B apart (SBO), rows 128 B apart inside a group
-__device__ __forceinline__ uint64_t make_desc(const void* smem) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_u32(smem) >> 4) & 0x3FFF);        // start address
-    d |= (uint64_t)1 << 16;                                  // leading byte offset (unused for swizzled K-major) = 1
-    d |= (uint64_t)(1024 >> 4) << 32;                        // stride byte offset
-    d |= (uint64_t)1 << 46;                                  // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                                  // SWIZZLE_128B
-    return d;
+// named barriers of the consumer warps (the producer warp never joins them): 1 = both warpgroups, 2 / 3 = one warpgroup
+__device__ __forceinline__ void cons_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+__device__ __forceinline__ void wg_sync(int wgi) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wgi) : "memory"); }
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// MN-major operand box as TMA delivers it, raw[32 k][W mn], -> the K-major tile wgmma reads: dst[mn][32 k], 128-byte rows whose
+// 16-byte chunks are XOR-swizzled by row % 8.  All 256 consumer threads; a warp reads 32 consecutive mn of one k (conflict-free)
+// and writes 32 rows x 16 bytes that cover every bank group four times (the minimum for 512 bytes).
+template <int W>
+__device__ __forceinline__ void transpose_tile(const float* __restrict__ raw, uint8_t* dst, const int ctid) {
+#pragma unroll
+    for (int it = 0; it < W * 8 / 256; it++) {
+        const int idx = ctid + 256 * it;
+        const int mn = idx % W, kq = idx / W;
+        const float* r = raw + (size_t)(4 * kq) * W + mn;
+        *reinterpret_cast<float4*>(dst + mn * 128 + ((kq ^ (mn & 7)) << 4)) = make_float4(r[0], r[W], r[2 * W], r[3 * W]);
+    }
 }
-// MN-major TF32 operand tile.  32-bit MN-major operands have exactly one legal shared-memory layout on tcgen05: 128-byte
-// swizzle with 32-byte atoms (descriptor layout type 1, SWIZZLE_128B_BASE32B; TMA CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B) --
-// the ordinary 16-byte-atom SWIZZLE_128B descriptor is accepted but multiplies by zero (measured, tools/gemm_bench.py
-// history in DESIGN.md).  The TMA box is [32 k-rows][32 mn-floats] = 4 KB: rows of 128 B, the swizzle pattern repeats
-// every 4 k-rows (512 B = SBO), one instruction (K = 8) consumes 8 rows = 1024 B, and the 32-wide MN blocks of the
-// tile sit 4 KB apart (LBO).  Canonical layout ((8,n),(4,k)):((1,LBO),(8,SBO)) in 16-byte units.
-__device__ __forceinline__ uint64_t make_desc_mn(const void* smem) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_u32(smem) >> 4) & 0x3FFF);
-    d |= (uint64_t)(4096 >> 4) << 16;                        // leading byte offset: next 32-float MN block
-    d |= (uint64_t)(512 >> 4) << 32;                         // stride byte offset: next 4 k-rows
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)1 << 61;                                  // SWIZZLE_128B_BASE32B
-    return d;
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                 "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                   "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-                   "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-                   "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+
+// Accumulator fragment of a 64 x (8 NJ) warpgroup tile -> shared memory as [32-column chunk][64 rows][128 bytes], swizzled like a
+// TMA box: every 32 x 32 block of it is 4 KB that a TMA store can send and that the tensor core can read as a K-major k-block.
+// f(v, column) is applied to every value on the way; column = first column of the pair.
+template <int NJ, typename F>
+__device__ __forceinline__ void store_fragment(const float (&acc)[4 * NJ], uint8_t* tile, const int col_base, const int w, const int lane, F f) {
+    const int rb = 16 * w + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < NJ; j++) {
+        const int col = col_base + 8 * j + 2 * (lane & 3);
+        uint8_t* p = tile + (size_t)(col >> 5) * (64 * 128) + rb * 128 + ((((col & 31) >> 2) ^ (rb & 7)) << 4) + (lane & 1) * 8;
+        *reinterpret_cast<float2*>(p) = f(make_float2(acc[4 * j], acc[4 * j + 1]), col, 0);
+        *reinterpret_cast<float2*>(p + 8 * 128) = f(make_float2(acc[4 * j + 2], acc[4 * j + 3]), col, 1);
+    }
 }
 
 // ELU(v) = v > 0 ? v : expm1(v), branch-free: a degree-7 Taylor polynomial on (-0.35, 0] (truncation error < 2e-8 relative) and
@@ -137,11 +127,10 @@ constexpr int GEMM_MAXP = 4;
 struct GemmMaps { CUtensorMap a[GEMM_MAXP], b[GEMM_MAXP]; };
 
 // Per-warp shared-memory staging of the staged epilogue.  A row-per-lane float4 store touches 32 different 128-byte lines per
-// instruction (8 x the LSU wavefronts of a coalesced store); measured, that -- not the tensor core -- bounded every short-K product
-// (dgrad 24576 x 512 x 256: 37 us with nothing fused, 56 us with the ELU' operand, against 19 us of HBM time).  Staged: the warp's
+// instruction (8 x the LSU wavefronts of a coalesced store), which bounds every short-K product.  Staged: the warp's
 // 32 x 32 block is written to shared memory (128B-swizzled: conflict-free 16-byte accesses) and ONE thread hands it to the TMA unit.
 struct EpiStage {
-    uint8_t* out;            // 4 KB, 1024-byte aligned, or nullptr: direct global stores
+    uint8_t* out;            // 4 KB, 1024-byte aligned: the block the values came from, or nullptr: direct global stores
     const CUtensorMap* mapC;
     const uint8_t* aux;      // 4 KB block of the ELU' operand, fetched by TMA and already waited for, or nullptr
 };
@@ -330,70 +319,44 @@ __device__ __forceinline__ bool epilogue_prefetch(const GemmArgs& g, const int r
     return true;
 }
 
-// One accumulator tile (128 lanes x BN columns at tmem_d) drained by the epilogue warps: NEPI = 4 G warps, warp = (TMEM lane quarter
-// q = warp id % 4, column group grp): group grp takes the 32-column chunks grp, grp + G, ...  With G = 4 sixteen warps work on a tile:
-// the epilogue (activation, column sums, row-per-lane global traffic) is latency bound per warp, so its throughput scales with warps.
-template <int BN, int G>
-__device__ __forceinline__ void epilogue_tile(const GemmArgs& g, const uint32_t tmem_d, const int q, const int grp, const int row, const int n0,
-                                              const bool split, const int lane, const float4 (&ypre)[8], const bool have_pre) {
-#pragma unroll 1
-    for (int c = grp; c < BN / 32; c += G) {
-        uint32_t r[32];
-        tmem_ld32(tmem_d + ((uint32_t)(32 * q) << 16) + (uint32_t)(32 * c), r);
-        const EpiStage nostage = {nullptr, nullptr, nullptr};
-        epilogue_chunk(g, g.C, r, row, n0 + 32 * c, split, lane, ypre, have_pre && c == grp, nostage);
-    }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
-// Persistent variant: grid = min(#tiles, 2 x #SMs); every CTA walks tiles t = blockIdx.x + i * gridDim.x (n fastest, so the
-// CTAs of one wave share A tiles through L2).  The accumulator is double-buffered in TMEM (2 x BN columns): while the
-// epilogue warps drain tile i from buffer i&1, the MMA warp already accumulates tile i+1 into the other buffer, and the
-// per-CTA set-up (TMEM allocation, barrier init, tensormap prefetch) is paid once instead of once per tile.
+// Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x + i * gridDim.x (n fastest, so the CTAs of
+// one wave share A tiles through L2).  Shared memory: [ring: stages x (A | B)][X: 64 KB][ELU' operand staging 8 x 4 KB][barriers].
+// X serves the main loop as the double-buffered transposed tiles of MN-major operands (A 2 x 16 KB, B 2 x 16 KB) and the epilogue
+// as the accumulator / output staging (32 KB per warpgroup).
 // ---------------------------------------------------------------------------------------------------------------
-template <int BN, int G, bool STAGED>
-__global__ void __launch_bounds__(64 + 128 * G, 1) gemm_tf32_persistent(const __grid_constant__ GemmMaps gm,
-                                                                        const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
-                                                                        const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
-    constexpr int NEPI = 4 * G;                  // epilogue warps
-    constexpr int STAGE_BYTES = (BM + BN) * BK * 4;
+constexpr int X_BYTES = 65536;
+template <int BN, bool STAGED>
+__global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __grid_constant__ GemmMaps gm,
+                                                                      const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
+                                                                      const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
+    constexpr int G = EPI_G;
+    constexpr int A_BYTES = BM * BK * 4, STAGE_BYTES = (BM + BN) * BK * 4;
     constexpr int MAX_STAGES = 8;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    // carve: [ring: stages x (A | B)][out staging NEPI x 4 KB][ELU' operand staging NEPI x 4 KB][barriers]   (staging only if STAGED)
     uint8_t* base = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t* ring = base;
-    uint8_t* stage_out = base + (size_t)stages * STAGE_BYTES;
-    uint8_t* stage_aux = stage_out + (STAGED ? NEPI * 4096 : 0);
-    uint64_t* full = (uint64_t*)(stage_aux + ((STAGED && g.tma_aux) ? NEPI * 4096 : 0));
+    uint8_t* xreg = base + (size_t)stages * STAGE_BYTES;
+    uint8_t* stage_aux = xreg + X_BYTES;
+    uint64_t* full = (uint64_t*)(stage_aux + ((STAGED && g.tma_aux) ? NCONS * 4096 : 0));
     uint64_t* empty = full + MAX_STAGES;
-    uint64_t* tmem_full = empty + MAX_STAGES;    // [2]
-    uint64_t* tmem_empty = tmem_full + 2;        // [2]
-    uint64_t* aux_bar = tmem_empty + 2;          // [NEPI]
-    uint32_t* tmem_slot = (uint32_t*)(aux_bar + NEPI);
+    uint64_t* aux_bar = empty + MAX_STAGES;      // [NCONS]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int num_kb_total = (g.K + BK - 1) / BK;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int p = 0; p < g.nprob; p++) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&gm.a[p]) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&gm.b[p]) : "memory");
         }
         if (STAGED && g.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"(&mapC) : "memory");
         if (STAGED && g.tma_aux) asm volatile("prefetch.tensormap [%0];" ::"l"(&mapY) : "memory");
-        for (int s = 0; s < stages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; b++) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], 128 * G); }
-        for (int w = 0; w < NEPI; w++) mbar_init(&aux_bar[w], 1);
+        for (int s = 0; s < stages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], NCONS); }
+        for (int w = 0; w < NCONS; w++) mbar_init(&aux_bar[w], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)(2 * BN)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
     // tile -> (m0, n0, k-block range); grouped launches: tile t of problem t / tiles_per_prob
     auto tile_coords = [&](int t, int& m0, int& n0, int& kb0, int& nkb) {
@@ -403,7 +366,8 @@ __global__ void __launch_bounds__(64 + 128 * G, 1) gemm_tf32_persistent(const __
         m0 = tm * BM; n0 = tn * BN; kb0 = z * g.kb_per_split; nkb = min(g.kb_per_split, num_kb_total - kb0);
     };
 
-    if (warp == 0) {
+    if (warp == NCONS) {
+        // ===== TMA producer =====
         if (elect_one()) {
             int s = 0, ph = 0;      // ring position of this CTA's k-block stream
             for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
@@ -414,120 +378,109 @@ __global__ void __launch_bounds__(64 + 128 * G, 1) gemm_tf32_persistent(const __
                 for (int i = 0; i < nkb; i++) {
                     mbar_wait(&empty[s], ph ^ 1);
                     mbar_expect_tx(&full[s], STAGE_BYTES);
-                    float* a = (float*)(ring + (size_t)s * STAGE_BYTES);
-                    float* b = a + BM * BK;
-                    if (g.amn) {
-#pragma unroll
-                        for (int x = 0; x < BM / 32; x++) tma_load_2d(mapA, &full[s], a + x * 32 * BK, m0 + 32 * x, (kb0 + i) * BK);
-                    } else tma_load_2d(mapA, &full[s], a, (kb0 + i) * BK, m0);
-                    if (g.bmn) {
-#pragma unroll
-                        for (int x = 0; x < BN / 32; x++) tma_load_2d(mapB, &full[s], b + x * 32 * BK, n0 + 32 * x, (kb0 + i) * BK);
-                    } else tma_load_2d(mapB, &full[s], b, (kb0 + i) * BK, n0);
+                    uint8_t* a = ring + (size_t)s * STAGE_BYTES;
+                    uint8_t* b = a + A_BYTES;
+                    if (g.amn) tma_load_2d(mapA, &full[s], a, m0, (kb0 + i) * BK);        // box [32 k-rows][128 m]
+                    else tma_load_2d(mapA, &full[s], a, (kb0 + i) * BK, m0);              // box [128 m-rows][32 k]
+                    if (g.bmn) tma_load_2d(mapB, &full[s], b, n0, (kb0 + i) * BK);
+                    else tma_load_2d(mapB, &full[s], b, (kb0 + i) * BK, n0);
                     if (++s == stages) { s = 0; ph ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        // bits 15 / 16: A / B operand is MN-major
-        const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(g.amn ? 1 : 0) << 15) | ((uint32_t)(g.bmn ? 1 : 0) << 16) |
-                               ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        const uint32_t ka = g.amn ? (1024 >> 4) : 2, kb = g.bmn ? (1024 >> 4) : 2;     // per-instruction K advance of the descriptors
-        int s = 0, ph = 0, j = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, j++) {
-            int m0, n0, kb0, nkb; tile_coords(t, m0, n0, kb0, nkb);
-            const int buf = j & 1;
-            mbar_wait(&tmem_empty[buf], ((j >> 1) & 1) ^ 1);          // epilogue has drained this accumulator buffer
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t tmem_d = tmem_base + (uint32_t)(buf * BN);
-            for (int i = 0; i < nkb; i++) {
-                mbar_wait(&full[s], ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (elect_one()) {
-                    const float* a = (const float*)(ring + (size_t)s * STAGE_BYTES);
-                    const float* b = a + BM * BK;
-                    const uint64_t da = g.amn ? make_desc_mn(a) : make_desc(a);
-                    const uint64_t db = g.bmn ? make_desc_mn(b) : make_desc(b);
-#pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; k++) umma_tf32(tmem_d, da + ka * k, db + kb * k, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                    umma_commit(&empty[s]);
-                    if (i == nkb - 1) umma_commit(&tmem_full[buf]);
-                }
-                __syncwarp();
-                if (++s == stages) { s = 0; ph ^= 1; }
-            }
+        return;
+    }
+    if (warp > NCONS) return;
+
+    // ===== consumers: warpgroup wgi owns rows [64 wgi, 64 wgi + 64) of the tile =====
+    const int wgi = warp >> 2, w = warp & 3, ctid = threadIdx.x;
+    const int q = 2 * wgi + (w & 1), grp = w >> 1;      // epilogue: 32-row block q of the tile, column group grp
+    const bool tr = g.amn || g.bmn;
+    const bool split = g.kb_per_split < num_kb_total;
+    const bool st_out = STAGED && g.tma_store, st_aux = STAGED && g.tma_aux;
+    uint8_t* xwg = xreg + wgi * (X_BYTES / 2);          // this warpgroup's accumulator staging: [chunk][64 rows][128 B]
+    uint8_t* my_aux = stage_aux + warp * 4096;
+    uint64_t* my_bar = &aux_bar[warp];
+    // ELU' operand blocks run one chunk ahead of the epilogue: cursor (pt, pc) = the next chunk of this warp whose block has not been requested yet
+    int pt = blockIdx.x, pc = grp - G;
+    auto next_chunk = [&]() -> bool {
+        for (;;) {
+            pc += G;
+            if (pc >= BN / 32) { pt += gridDim.x; pc = grp; }
+            if (pt >= total_tiles) return false;
+            if (pc < BN / 32 && (pt % tiles_n) * BN + 32 * pc < g.N) return true;
         }
-    } else {
-        // ===== epilogue: NEPI warps; warp = (TMEM lane quarter q = warp id % 4, column group grp); group grp takes chunks grp, grp + G, ...
-        const int ew = warp - 2, q = warp & 3, grp = ew >> 2;
-        const bool split = g.kb_per_split < num_kb_total;
-        const bool st_out = STAGED && g.tma_store, st_aux = STAGED && g.tma_aux;
-        uint8_t* my_out = stage_out + ew * 4096;
-        uint8_t* my_aux = stage_aux + ew * 4096;
-        uint64_t* my_bar = &aux_bar[ew];
-        EpiStage es;
-        es.out = st_out ? my_out : nullptr; es.mapC = &mapC; es.aux = st_aux ? my_aux : nullptr;
-        // ELU' operand blocks run one chunk ahead of the epilogue: cursor (pt, pc) = the next chunk of this warp whose block has not been requested yet
-        int pt = blockIdx.x, pc = grp - G;
-        auto next_chunk = [&]() -> bool {
-            for (;;) {
-                pc += G;
-                if (pc >= BN / 32) { pt += gridDim.x; pc = grp; }
-                if (pt >= total_tiles) return false;
-                if ((pt % tiles_n) * BN + 32 * pc < g.N) return true;
+    };
+    auto request_aux = [&]() {
+        if (next_chunk() && lane == 0) {
+            int m0, n0, kb0, nkb; tile_coords(pt, m0, n0, kb0, nkb);
+            mbar_expect_tx(my_bar, 4096);
+            tma_load_2d(&mapY, my_bar, my_aux, n0 + 32 * pc, m0 + 32 * q);
+        }
+    };
+    if (st_aux) request_aux();
+    uint32_t aux_phase = 0;
+    int s = 0, ph = 0;
+    float acc[BN / 2];
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+        int m0, n0, kb0, nkb; tile_coords(t, m0, n0, kb0, nkb);
+        // X is about to be rewritten: the TMA stores of the previous tile have read it
+        if (st_out && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        cons_sync();
+        int prev = -1;
+        for (int i = 0; i < nkb; i++) {
+            mbar_wait(&full[s], ph);
+            const uint8_t* a = ring + (size_t)s * STAGE_BYTES;
+            const uint8_t* b = a + A_BYTES;
+            if (tr) {
+                if (g.amn) { uint8_t* ta = xreg + (i & 1) * A_BYTES; transpose_tile<BM>((const float*)a, ta, ctid); a = ta; }
+                if (g.bmn) { uint8_t* tb = xreg + 2 * A_BYTES + (i & 1) * A_BYTES; transpose_tile<BN>((const float*)b, tb, ctid); b = tb; }
+                if (prev >= 0) {        // k-block i - 1 is done: its stage returns to the producer, and its transposed tiles may be rewritten next round
+                    wg::wait<0>();
+                    if (lane == 0) mbar_arrive(&empty[prev]);
+                }
+                fence_async_smem();     // generic-proxy writes -> visible to the tensor core (async proxy)
+                cons_sync();
             }
-        };
-        auto request_aux = [&]() {
-            if (next_chunk() && lane == 0) {
-                int m0, n0, kb0, nkb; tile_coords(pt, m0, n0, kb0, nkb);
-                mbar_expect_tx(my_bar, 4096);
-                tma_load_2d(&mapY, my_bar, my_aux, n0 + 32 * pc, m0 + 32 * q);
+            wg::fence();
+            wg::mma_kblock<BN>(acc, a + (size_t)wgi * 64 * 128, b, i > 0);
+            wg::commit();
+            if (!tr && prev >= 0) {
+                wg::wait<1>();
+                if (lane == 0) mbar_arrive(&empty[prev]);
             }
-        };
-        if (st_aux) request_aux();
-        uint32_t aux_phase = 0;
-        int j = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x, j++) {
-            int m0, n0, kb0, nkb; tile_coords(t, m0, n0, kb0, nkb);
-            const int buf = j & 1;
-            const int row = m0 + 32 * q + lane;
-            float* const Cbase = g.nprob > 1 ? g.Cg[t / g.tiles_per_prob] : g.C;
-            float4 ypre[8];
-            const bool have_pre = !st_aux && (grp < BN / 32) && epilogue_prefetch(g, row, n0 + 32 * grp, split, ypre);
-            mbar_wait(&tmem_full[buf], (j >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t tmem_d = tmem_base + (uint32_t)(buf * BN);
-            bool released = false;
+            prev = s;
+            if (++s == stages) { s = 0; ph ^= 1; }
+        }
+        wg::wait<0>();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+        if (tr) cons_sync();            // both warpgroups are done with the transposed tiles that the staging overlays
+
+        const int row = m0 + 32 * q + lane;
+        float* const Cbase = g.nprob > 1 ? g.Cg[t / g.tiles_per_prob] : g.C;
+        float4 ypre[8];
+        const bool have_pre = !st_aux && (grp < BN / 32) && epilogue_prefetch(g, row, n0 + 32 * grp, split, ypre);
+        store_fragment<BN / 8>(acc, xwg, 0, w, lane, [](float2 v, int, int) { return v; });
+        wg_sync(wgi);
 #pragma unroll 1
-            for (int c = grp; c < BN / 32; c += G) {
-                if (n0 + 32 * c >= g.N) break;                           // warp-uniform
-                uint32_t r[32];
-                tmem_ld32(tmem_d + ((uint32_t)(32 * q) << 16) + (uint32_t)(32 * c), r);
-                if (c + G >= BN / 32 || n0 + 32 * (c + G) >= g.N) {      // last chunk of this warp in the tile: the accumulator is in registers, hand the buffer back now
-                    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                    mbar_arrive(&tmem_empty[buf]);
-                    released = true;
-                }
-                if (st_out) {                                            // the previous block must have left the staging buffer
-                    if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                    __syncwarp();
-                }
-                if (st_aux) { mbar_wait(my_bar, aux_phase); aux_phase ^= 1; }
-                epilogue_chunk(g, Cbase, r, row, n0 + 32 * c, split, lane, ypre, have_pre && c == grp, es);
-                if (st_aux) { __syncwarp(); request_aux(); }             // every lane has read the operand block: fetch the next one into it
+        for (int c = grp; c < BN / 32; c += G) {
+            if (n0 + 32 * c >= g.N) break;                           // warp-uniform
+            uint8_t* blk = xwg + (size_t)c * (64 * 128) + (w & 1) * 4096;
+            uint32_t r[32];
+            const uint8_t* srow = blk + lane * 128;
+#pragma unroll
+            for (int j = 0; j < 8; j++) {
+                const uint4 x = *reinterpret_cast<const uint4*>(srow + ((j ^ (lane & 7)) << 4));
+                r[4 * j] = x.x; r[4 * j + 1] = x.y; r[4 * j + 2] = x.z; r[4 * j + 3] = x.w;
             }
-            if (!released) {
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive(&tmem_empty[buf]);
-            }
+            EpiStage es;
+            es.out = st_out ? blk : nullptr; es.mapC = &mapC; es.aux = st_aux ? my_aux : nullptr;
+            if (st_aux) { mbar_wait(my_bar, aux_phase); aux_phase ^= 1; }
+            epilogue_chunk(g, Cbase, r, row, n0 + 32 * c, split, lane, ypre, have_pre && c == grp, es);
+            if (st_aux) { __syncwarp(); request_aux(); }             // every lane has read the operand block: fetch the next one into it
         }
-        if (st_out && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // all stores of this warp have completed
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * BN)) : "memory");
-    }
+    if (st_out && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // all stores of this warp have completed
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -535,27 +488,38 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 EncodeTiledFn g_encode = nullptr;
 std::once_flag g_once;
 
-int make_map_uncached(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int box_rows, CUtensorMapSwizzle swz);
+int sm_count() {
+    static int sms = 0;
+    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
+    return sms;
+}
+
+int make_map_uncached(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int box_rows, int box_cols, CUtensorMapSwizzle swz);
 // Encoding a tensor map costs about a microsecond of host time and the learner issues the same few hundred (pointer, shape) combinations
 // every update: keep them.
-struct MapKey { const float* ptr; int rows, cols, ld, box_rows, swz; bool operator==(const MapKey& o) const { return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && swz == o.swz; } };
-struct MapKeyHash { size_t operator()(const MapKey& k) const { size_t h = (size_t)k.ptr; h = h * 1000003u ^ (size_t)k.rows; h = h * 1000003u ^ (size_t)k.cols; h = h * 1000003u ^ (size_t)k.ld; h = h * 1000003u ^ (size_t)(k.box_rows * 8 + k.swz); return h; } };
+struct MapKey { const float* ptr; int rows, cols, ld, box_rows, box_cols, swz; bool operator==(const MapKey& o) const { return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && box_cols == o.box_cols && swz == o.swz; } };
+struct MapKeyHash { size_t operator()(const MapKey& k) const { size_t h = (size_t)k.ptr; h = h * 1000003u ^ (size_t)k.rows; h = h * 1000003u ^ (size_t)k.cols; h = h * 1000003u ^ (size_t)k.ld; h = h * 1000003u ^ (size_t)(k.box_rows * 8 + k.swz); h = h * 1000003u ^ (size_t)k.box_cols; return h; } };
 std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_map_cache;
 std::mutex g_map_mutex;
-int make_map(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int box_rows, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
-    const MapKey key{ptr, rows, cols, ld, box_rows, (int)swz};
+// rows x cols fp32 matrix with row stride ld; box = box_rows x box_cols.  K-major operand tiles and 32 x 32 output blocks: 32-float (128-byte)
+// box rows, 128B-swizzled.  MN-major operand boxes ([32 k-rows][tile width]): unswizzled, transposed on the SM.
+int make_map(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int box_rows, int box_cols = BK, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
+    const MapKey key{ptr, rows, cols, ld, box_rows, box_cols, (int)swz};
     {
         std::lock_guard<std::mutex> lk(g_map_mutex);
         auto it = g_map_cache.find(key);
         if (it != g_map_cache.end()) { *map = it->second; return 0; }
     }
-    if (int e = make_map_uncached(map, ptr, rows, cols, ld, box_rows, swz)) return e;
+    if (int e = make_map_uncached(map, ptr, rows, cols, ld, box_rows, box_cols, swz)) return e;
     std::lock_guard<std::mutex> lk(g_map_mutex);
     if (g_map_cache.size() > 8192) g_map_cache.clear();
     g_map_cache.emplace(key, *map);
     return 0;
 }
-int make_map_uncached(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int box_rows, CUtensorMapSwizzle swz) {
+int make_map_mn(CUtensorMap* map, const float* ptr, int k_rows, int mn_cols, int ld, int width) {
+    return make_map(map, ptr, k_rows, mn_cols, ld, BK, width, CU_TENSOR_MAP_SWIZZLE_NONE);
+}
+int make_map_uncached(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int box_rows, int box_cols, CUtensorMapSwizzle swz) {
     std::call_once(g_once, [] {
         void* fn = nullptr;
         cudaDriverEntryPointQueryResult q;
@@ -564,7 +528,7 @@ int make_map_uncached(CUtensorMap* map, const float* ptr, int rows, int cols, in
     if (!g_encode) return go1_set_error("cuTensorMapEncodeTiled unavailable");
     cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
     cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
-    cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
+    cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = g_encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                           swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -587,11 +551,11 @@ __global__ void bias_act_strided(float* C, int ldc, const float* bias, int M, in
     *c = v;
 }
 
-template <int BN, int G, bool STAGED>
-int launch_persistent(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st) {
-    constexpr int NEPI = 4 * G, STAGE_BYTES = (BM + BN) * BK * 4;
-    const size_t staging = STAGED ? (size_t)NEPI * 4096 * (g.tma_aux ? 2 : 1) : 0;
-    const size_t fixed = staging + (2 * 8 + 4 + NEPI) * 8 + 16 + 1024;
+template <int BN, bool STAGED>
+int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st) {
+    constexpr int STAGE_BYTES = (BM + BN) * BK * 4;
+    const size_t staging = X_BYTES + ((STAGED && g.tma_aux) ? (size_t)NCONS * 4096 : 0);
+    const size_t fixed = staging + (2 * 8 + NCONS) * 8 + 16 + 1024;
     const size_t budget = 227 * 1024;
     int stages = (int)((budget - fixed) / STAGE_BYTES);
     if (stages > 8) stages = 8;
@@ -599,281 +563,106 @@ int launch_persistent(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorM
     const size_t smem = (size_t)stages * STAGE_BYTES + fixed;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tf32_persistent<BN, G, STAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget);
+        cudaError_t e = cudaFuncSetAttribute(gemm_tf32_wgmma<BN, STAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget);
         if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
         configured = true;
     }
     const int tiles_m = (g.M + BM - 1) / BM, tiles_n = (g.N + BN - 1) / BN;
     g.tiles_per_prob = tiles_m * tiles_n * splits;
     const int total = g.tiles_per_prob * (g.nprob > 1 ? g.nprob : 1);
-    static int sms = 0;
-    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
+    const int sms = sm_count();
     const int grid = total < sms ? total : sms;          // one CTA per SM (the ring and the staging fill its shared memory)
-    gemm_tf32_persistent<BN, G, STAGED><<<grid, 64 + 128 * G, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages);
+    gemm_tf32_wgmma<BN, STAGED><<<grid, 32 * NCONS + 128, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages);
     go1_count_launch(1);
     return 0;
 }
-
-// ---------------------------------------------------------------------------------------------------------------
-// cta_group::2 variant (default for the shapes the wide heuristic selects; GO1_TF32_2CTA=0 falls back to the single-CTA 128 x 256
-// kernel).  A cluster of two CTAs owns a 256 x 256 output tile: CTA r holds rows [128r, 128r+128) of A and columns [128r, 128r+128) of B in ITS shared memory (32 KB per
-// k-block for a 128 x 256 accumulator per CTA = 0.5x the L2->SM bytes per flop of the 128 x 128 tiling), the leader CTA (rank 0)
-// issues tcgen05.mma.cta_group::2 (M = 256, N = 256) which reads both CTAs' operand slices and writes each CTA's half of the
-// accumulator into that CTA's TMEM.  Protocol: both producers load into their own smem and signal the LEADER's full barrier
-// (cp.async.bulk.tensor...cta_group::2, peer bit of the barrier address cleared); the leader's tcgen05.commit multicasts to the
-// empty / tmem_full barriers of both CTAs; both CTAs' epilogue threads release a TMEM buffer on the leader's tmem_empty barrier.
-// ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* map, uint64_t* leader_bar, void* dst, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(leader_bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void umma_tf32_2sm(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-                 ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {      // arrives on `bar` (same offset) in both CTAs of the pair
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-    asm volatile("{\n\t.reg .b32 ra;\n\tmapa.shared::cluster.u32 ra, %0, 0;\n\tmbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
-                 ::"r"(smem_u32(bar)) : "memory");
-}
-
-template <int STAGES, int G>
-__global__ void __launch_bounds__(64 + 128 * G, 1) gemm_tf32_2cta(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapB, const GemmArgs g,
-                                                          const int tiles_m2, const int tiles_n, const int total_tiles) {
-    constexpr int BN = 256, HB = 128;              // cluster tile 256 x 256; each CTA stages 128 rows of A and 128 columns of B
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* base = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    float* sA = (float*)base;
-    float* sB = (float*)(base + (size_t)STAGES * BM * BK * 4);
-    uint64_t* full = (uint64_t*)(base + (size_t)STAGES * (BM + HB) * BK * 4);
-    uint64_t* empty = full + STAGES;
-    uint64_t* tmem_full = empty + STAGES;        // [2]
-    uint64_t* tmem_empty = tmem_full + 2;        // [2] (the leader's are used)
-    uint32_t* tmem_slot = (uint32_t*)(tmem_empty + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_rank();
-    const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
-    const int num_kb_total = (g.K + BK - 1) / BK;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&mapA) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&mapB) : "memory");
-        for (int s = 0; s < STAGES; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int b = 0; b < 2; b++) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], 2 * 128 * G); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {     // both CTAs of the pair allocate together (same warp id, same slot address)
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"((uint32_t)(2 * BN)) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();                          // the peer's barriers exist before anything signals them
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
-
-    auto tile_coords = [&](int t, int& m0, int& n0, int& kb0, int& nkb) {
-        const int tn = t % tiles_n; t /= tiles_n;
-        const int tm = t % tiles_m2; const int z = t / tiles_m2;
-        m0 = (2 * tm + (int)rank) * BM; n0 = tn * BN; kb0 = z * g.kb_per_split; nkb = min(g.kb_per_split, num_kb_total - kb0);
-    };
-
-    if (warp == 0) {
-        if (elect_one()) {
-            int it = 0;
-            for (int t = cluster_id; t < total_tiles; t += num_clusters) {
-                int m0, n0, kb0, nkb; tile_coords(t, m0, n0, kb0, nkb);
-                const int nb0 = n0 + (int)rank * HB;                     // this CTA's half of the B tile
-                for (int i = 0; i < nkb; i++, it++) {
-                    const int s = it % STAGES, ph = (it / STAGES) & 1;
-                    mbar_wait(&empty[s], ph ^ 1);
-                    if (rank == 0) mbar_expect_tx(&full[s], 2 * (BM + HB) * BK * 4);      // bytes of BOTH CTAs land on the leader's barrier
-                    float* a = sA + (size_t)s * BM * BK;
-                    float* b = sB + (size_t)s * HB * BK;
-                    if (g.amn) {
-#pragma unroll
-                        for (int x = 0; x < BM / 32; x++) tma_load_2d_2sm(&mapA, &full[s], a + x * 32 * BK, m0 + 32 * x, (kb0 + i) * BK);
-                    } else tma_load_2d_2sm(&mapA, &full[s], a, (kb0 + i) * BK, m0);
-                    if (g.bmn) {
-#pragma unroll
-                        for (int x = 0; x < HB / 32; x++) tma_load_2d_2sm(&mapB, &full[s], b + x * 32 * BK, nb0 + 32 * x, (kb0 + i) * BK);
-                    } else tma_load_2d_2sm(&mapB, &full[s], b, (kb0 + i) * BK, nb0);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (rank == 0) {         // the leader issues the pair's MMAs
-            const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(g.amn ? 1 : 0) << 15) | ((uint32_t)(g.bmn ? 1 : 0) << 16) |
-                                   ((uint32_t)(BN >> 3) << 17) | ((uint32_t)((2 * BM) >> 4) << 24);
-            const uint32_t ka = g.amn ? (1024 >> 4) : 2, kb = g.bmn ? (1024 >> 4) : 2;
-            int it = 0, j = 0;
-            for (int t = cluster_id; t < total_tiles; t += num_clusters, j++) {
-                int m0, n0, kb0, nkb; tile_coords(t, m0, n0, kb0, nkb);
-                const int buf = j & 1;
-                mbar_wait(&tmem_empty[buf], ((j >> 1) & 1) ^ 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t tmem_d = tmem_base + (uint32_t)(buf * BN);
-                for (int i = 0; i < nkb; i++, it++) {
-                    const int s = it % STAGES, ph = (it / STAGES) & 1;
-                    mbar_wait(&full[s], ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    if (elect_one()) {
-                        const uint64_t da = g.amn ? make_desc_mn(sA + (size_t)s * BM * BK) : make_desc(sA + (size_t)s * BM * BK);
-                        const uint64_t db = g.bmn ? make_desc_mn(sB + (size_t)s * HB * BK) : make_desc(sB + (size_t)s * HB * BK);
-#pragma unroll
-                        for (int k = 0; k < BK / UMMA_K; k++) umma_tf32_2sm(tmem_d, da + ka * k, db + kb * k, idesc, (i > 0 || k > 0) ? 1u : 0u);
-                        umma_commit_2sm(&empty[s]);
-                        if (i == nkb - 1) umma_commit_2sm(&tmem_full[buf]);
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-    } else {
-        const int q = warp & 3, grp = (warp - 2) >> 2;
-        const bool split = g.kb_per_split < num_kb_total;
-        int j = 0;
-        for (int t = cluster_id; t < total_tiles; t += num_clusters, j++) {
-            int m0, n0, kb0, nkb; tile_coords(t, m0, n0, kb0, nkb);
-            const int buf = j & 1;
-            const int row = m0 + 32 * q + lane;
-            float4 ypre[8];
-            const bool have_pre = epilogue_prefetch(g, row, n0 + 32 * grp, split, ypre);
-            mbar_wait(&tmem_full[buf], (j >> 1) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            epilogue_tile<BN, G>(g, tmem_base + (uint32_t)(buf * BN), q, grp, row, n0, split, lane, ypre, have_pre);
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive_leader(&tmem_empty[buf]);
-        }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    cluster_sync_all();                          // nobody leaves while the pair may still touch its shared memory / barriers / TMEM
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(2 * BN)) : "memory");
-    }
-}
-
-template <int STAGES, int G>
-int launch_2cta(const CUtensorMap& ma, const CUtensorMap& mb, const GemmArgs& g, int splits, cudaStream_t st) {
-    const size_t smem = (size_t)STAGES * (BM + 128) * BK * 4 + (2 * STAGES + 4) * 8 + 16 + 1024;
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tf32_2cta<STAGES, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
-        configured = true;
-    }
-    const int tiles_m2 = (g.M + 2 * BM - 1) / (2 * BM), tiles_n = (g.N + 255) / 256, total = tiles_m2 * tiles_n * splits;
-    static int sms = 0;
-    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
-    const int clusters = total < sms / 2 ? total : sms / 2;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * clusters); cfg.blockDim = dim3(64 + 128 * G); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_tf32_2cta<STAGES, G>, ma, mb, g, tiles_m2, tiles_n, total);
-    if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
-    go1_count_launch(1);
-    return 0;
-}
-
 
 // ---------------------------------------------------------------------------------------------------------------
 // Fused MLP tail, forward: the layers behind a first layer of ActorCritic's MLPs (actor_critic.py:38-77) in ONE launch,
 //     y2 = ELU(x W2^T + b2)   [M][N2]        x = the first layer's activated output, K1 wide (a column slice of the fused first-layer product)
 //     y3 = ELU(y2 W3^T + b3)  [M][N3]        (N3 = 0: two-layer tail, the head reads y2)
 //     out = y_last Wh^T + bh  [M][nh]        nh <= 12 (12 action means / 1 value / 2 latents): CUDA cores, from registers
-// for up to two problems of the same shape (actor and critic bodies) in one grid.  One CTA (576 threads) owns a 128-row block:
-//   warp 0   TMA producer: ring 1 streams x and W2 k-blocks, ring 2 the W3 k-blocks
-//   warp 1   tcgen05 issuer: product 1 -> TMEM columns [0, N2); product 2 -> TMEM columns [256, 256 + N3), its A operand is the y2 tile
-//            the epilogue warps laid out in shared memory (K-major, 128B-swizzled, overlaying ring 1)
-//   warps 2-17  epilogue, warp = (TMEM lane quarter, column group): bias + ELU on the accumulator chunks; y2 goes to shared memory once
-//            and from there BOTH to the tensor core (product 2) and to global memory (one TMA store per warp and 32 x 32 block: the
-//            backward pass needs y2); y3 is stored from registers; the head's partial dot products of the four column groups meet
-//            in shared memory.
-// Product 1 of tile t+1 (operand loads included: the L2 -> SM stream of x and W2 bounds the kernel) overlaps the second epilogue of tile t.
-// Barriers, all flipping once per tile: acc1_full (commit of product 1), y2_ready (512 epilogue threads: the y2 tile is in ring 1 and
-// accumulator 1 has been read), acc2_full (commit of product 2), r1_free (commit of product 2: the tensor core is done with ring 1),
-// y2_stored (16 lanes: the TMA stores have read ring 1).  The producer refills ring 1 after r1_free and y2_stored.
+// for up to two problems of the same shape (actor and critic bodies) in one grid.  One CTA (384 threads) owns a 64-row block:
+//   warps 0-7   two consumer warpgroups; warpgroup g computes columns [g N2 / 2, (g + 1) N2 / 2) of y2 and [g N3 / 2, (g + 1) N3 / 2) of y3
+//               for all 64 rows (wgmma, accumulators in registers).  y2 = ELU(acc + b2) goes from the registers to shared memory once,
+//               K-major and 128B-swizzled, and from there BOTH to the tensor core (A operand of product 2) and to global memory (one TMA
+//               store per 32 x 32 block: the backward pass needs y2); y3 is stored from registers; the head's partial dot products
+//               are taken on the accumulator fragments, reduced over the four lanes that share a row, and the two warpgroups' halves
+//               meet in shared memory.
+//   warp 8      TMA producer: ring 1 streams x and W2 k-blocks, ring 2 the W3 k-blocks; it runs ahead into the next block's product 1
+//               while the consumers are in product 2 and the head.
 // ---------------------------------------------------------------------------------------------------------------
-constexpr int TAIL_MAXP = 2, TAIL_G = 4, TAIL_NEPI = 16, TAIL_HPW = 12;
+constexpr int TAIL_MAXP = 2, TAIL_HPW = 12, TAIL_BM = 64;
 struct TailProb { const float* b2; const float* b3; const float* Wh; const float* bh; float* y3; float* out; int ldy3, ldout, nh, wh_row0; };
 struct TailArgs { TailProb p[TAIL_MAXP]; int nprob, M, tiles_per_prob, tiles; };
 struct TailMaps { CUtensorMap x[TAIL_MAXP], w2[TAIL_MAXP], w3[TAIL_MAXP], y2[TAIL_MAXP]; };
 
 template <int K1, int N2, int N3>
 struct TailSmem {
-    static constexpr int S1 = 3, S2 = (N3 > 0) ? 3 : 0;
+    static constexpr int S1 = (N3 > 0) ? 2 : 3, S2 = (N3 > 0) ? 2 : 0;
     static constexpr int KB1 = K1 / BK, KB2 = N2 / BK;
-    static constexpr int STAGE1 = (BM + N2) * BK * 4;
-    static constexpr int Y2TILE = KB2 * BM * BK * 4;
-    static constexpr int R1 = (N3 > 0 && Y2TILE > S1 * STAGE1) ? Y2TILE : S1 * STAGE1;      // ring 1; in the three-layer tail overlaid by the y2 tile
+    static constexpr int STAGE1 = (TAIL_BM + N2) * BK * 4;
+    static constexpr int Y2TILE = KB2 * TAIL_BM * BK * 4;
     static constexpr int STAGE2 = (N3 > 0 ? N3 : 8) * BK * 4;
-    static constexpr int R2 = S2 * STAGE2;
-    static constexpr int YSTG = (N3 > 0) ? 0 : TAIL_NEPI * 4096;        // two-layer tail: per-warp staging of the y2 blocks for their TMA stores
     static constexpr int NL = (N3 > 0) ? N3 : N2;
     static constexpr int PARAMS = (TAIL_MAXP * (N2 + N3) + 16 * NL + TAIL_MAXP * 16) * 4;
-    static constexpr int HP = (TAIL_G - 1) * TAIL_HPW * BM * 4;
-    static constexpr int BARS = (2 * S1 + 2 * (S2 > 0 ? S2 : 1) + 5) * 8 + 16;
-    static constexpr int TOTAL = R1 + R2 + YSTG + PARAMS + HP + BARS + 1024;
+    static constexpr int HP = TAIL_HPW * TAIL_BM * 4;
+    static constexpr int BARS = (2 * S1 + 2 * (S2 > 0 ? S2 : 1)) * 8 + 16;
+    static constexpr int TOTAL = S1 * STAGE1 + Y2TILE + S2 * STAGE2 + PARAMS + HP + BARS + 1024;
 };
 
+// partial dot products of the head on an accumulator fragment: hp[r][n] += sum over this thread's columns of v[row r][col] * Wh[n][col]
+template <int NJ>
+__device__ __forceinline__ void head_partial(const float (&v)[4 * NJ], const float* wh, const int NL, const int nh, const int col_base, const int lane, float (&hp)[2][TAIL_HPW]) {
+#pragma unroll
+    for (int n = 0; n < TAIL_HPW; n++) {
+        if (n < nh) {
+            const float* wr = wh + n * NL + col_base + 2 * (lane & 3);
+            float a0 = hp[0][n], a1 = hp[1][n];
+#pragma unroll
+            for (int j = 0; j < NJ; j++) {
+                const float2 ww = *reinterpret_cast<const float2*>(wr + 8 * j);
+                a0 = fmaf(v[4 * j], ww.x, a0); a0 = fmaf(v[4 * j + 1], ww.y, a0);
+                a1 = fmaf(v[4 * j + 2], ww.x, a1); a1 = fmaf(v[4 * j + 3], ww.y, a1);
+            }
+            hp[0][n] = a0; hp[1][n] = a1;
+        }
+    }
+}
+
 template <int K1, int N2, int N3>
-__global__ void __launch_bounds__(64 + 128 * TAIL_G, 1) mlp_tail_fwd_kernel(const __grid_constant__ TailMaps maps, const TailArgs g) {
+__global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_kernel(const __grid_constant__ TailMaps maps, const TailArgs g) {
     using L = TailSmem<K1, N2, N3>;
     constexpr int S1 = L::S1, S2 = (L::S2 > 0 ? L::S2 : 1), KB1 = L::KB1, KB2 = L::KB2, STAGE1 = L::STAGE1, STAGE2 = L::STAGE2, NL = L::NL;
-    constexpr uint32_t TMEM_COLS = (N3 > 0) ? 512u : (uint32_t)N2;
-    constexpr int G = TAIL_G;
+    constexpr int NH2 = N2 / 2, NH3 = (N3 > 0 ? N3 : 64) / 2;      // columns per warpgroup
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* base = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t* r1 = base;
-    uint8_t* r2 = base + L::R1;
-    uint8_t* ystg = r2 + L::R2;
-    float* s_b2 = (float*)(ystg + L::YSTG);                 // [MAXP][N2]
+    uint8_t* y2t = r1 + S1 * STAGE1;                         // [KB2][64 rows][128 B]
+    uint8_t* r2 = y2t + L::Y2TILE;
+    float* s_b2 = (float*)(r2 + L::S2 * STAGE2);             // [MAXP][N2]
     float* s_b3 = s_b2 + TAIL_MAXP * N2;                     // [MAXP][N3]
     float* s_wh = s_b3 + TAIL_MAXP * N3;                     // [16][NL]: the head rows of all problems (problem p starts at row wh_row0)
     float* s_bh = s_wh + 16 * NL;                            // [MAXP][16]
-    float* s_hp = s_bh + TAIL_MAXP * 16;                     // [G-1][HPW][128]: head partial sums of column groups 1..G-1
-    uint64_t* full1 = (uint64_t*)(s_hp + (G - 1) * TAIL_HPW * BM);
+    float* s_hp = s_bh + TAIL_MAXP * 16;                     // [HPW][64]: head partial sums of warpgroup 1
+    uint64_t* full1 = (uint64_t*)(s_hp + TAIL_HPW * TAIL_BM);
     uint64_t* empty1 = full1 + S1;
     uint64_t* full2 = empty1 + S1;
     uint64_t* empty2 = full2 + S2;
-    uint64_t* acc1_full = empty2 + S2;
-    uint64_t* acc2_full = acc1_full + 1;
-    uint64_t* y2_ready = acc2_full + 1;
-    uint64_t* r1_free = y2_ready + 1;
-    uint64_t* y2_stored = r1_free + 1;
-    uint32_t* tmem_slot = (uint32_t*)(y2_stored + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int p = 0; p < g.nprob; p++) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.x[p]) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.w2[p]) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.y2[p]) : "memory");
             if (N3 > 0) asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.w3[p]) : "memory");
         }
-        for (int s = 0; s < S1; s++) { mbar_init(&full1[s], 1); mbar_init(&empty1[s], 1); }
-        for (int s = 0; s < S2; s++) { mbar_init(&full2[s], 1); mbar_init(&empty2[s], 1); }
-        mbar_init(acc1_full, 1); mbar_init(acc2_full, 1); mbar_init(y2_ready, 128 * G); mbar_init(r1_free, 1); mbar_init(y2_stored, TAIL_NEPI);
+        for (int s = 0; s < S1; s++) { mbar_init(&full1[s], 1); mbar_init(&empty1[s], NCONS); }
+        for (int s = 0; s < S2; s++) { mbar_init(&full2[s], 1); mbar_init(&empty2[s], NCONS); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    // biases and head weights: read by every epilogue thread for every row -> shared memory
+    // biases and head weights: read by every consumer thread for every row -> shared memory
     for (int i = threadIdx.x; i < TAIL_MAXP * N2; i += blockDim.x) { const int p = i / N2; s_b2[i] = (p < g.nprob && g.p[p].b2) ? __ldg(g.p[p].b2 + (i - p * N2)) : 0.f; }
     if (N3 > 0) for (int i = threadIdx.x; i < TAIL_MAXP * N3; i += blockDim.x) { const int p = i / (N3 > 0 ? N3 : 1); s_b3[i] = (p < g.nprob && g.p[p].b3) ? __ldg(g.p[p].b3 + (i - p * N3)) : 0.f; }
     for (int i = threadIdx.x; i < 16 * NL; i += blockDim.x) {
@@ -883,24 +672,20 @@ __global__ void __launch_bounds__(64 + 128 * TAIL_G, 1) mlp_tail_fwd_kernel(cons
         s_wh[i] = v;
     }
     if (threadIdx.x < TAIL_MAXP * 16) { const int p = threadIdx.x >> 4, n = threadIdx.x & 15; s_bh[threadIdx.x] = (p < g.nprob && n < g.p[p].nh && g.p[p].bh) ? __ldg(g.p[p].bh + n) : 0.f; }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == NCONS) {
         // ===== TMA producer =====
         if (elect_one()) {
-            int it1 = 0, it2 = 0, tl = 0;
-            for (int t = blockIdx.x; t < g.tiles; t += gridDim.x, tl++) {
-                const int p = t / g.tiles_per_prob, m0 = (t - p * g.tiles_per_prob) * BM;
-                if (N3 > 0 && tl > 0) { mbar_wait(r1_free, (tl - 1) & 1); mbar_wait(y2_stored, (tl - 1) & 1); }   // ring 1 held the previous tile's y2
+            int it1 = 0, it2 = 0;
+            for (int t = blockIdx.x; t < g.tiles; t += gridDim.x) {
+                const int p = t / g.tiles_per_prob, m0 = (t - p * g.tiles_per_prob) * TAIL_BM;
                 for (int i = 0; i < KB1; i++, it1++) {
                     const int s = it1 % S1, ph = (it1 / S1) & 1;
                     mbar_wait(&empty1[s], ph ^ 1);
                     mbar_expect_tx(&full1[s], STAGE1);
                     tma_load_2d(&maps.x[p], &full1[s], r1 + (size_t)s * STAGE1, i * BK, m0);
-                    tma_load_2d(&maps.w2[p], &full1[s], r1 + (size_t)s * STAGE1 + BM * BK * 4, i * BK, 0);
+                    tma_load_2d(&maps.w2[p], &full1[s], r1 + (size_t)s * STAGE1 + TAIL_BM * BK * 4, i * BK, 0);
                 }
                 if (N3 > 0) {
                     for (int i = 0; i < KB2; i++, it2++) {
@@ -912,159 +697,112 @@ __global__ void __launch_bounds__(64 + 128 * TAIL_G, 1) mlp_tail_fwd_kernel(cons
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        const uint32_t idesc1 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N2 >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        const uint32_t idesc2 = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)((N3 > 0 ? N3 : 8) >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        int it1 = 0, it2 = 0, tl = 0;
-        for (int t = blockIdx.x; t < g.tiles; t += gridDim.x, tl++) {
-            // accumulator 1 is free: the epilogue read it before y2_ready of the previous tile, which product 2 of that tile (issued by
-            // this warp, in order) waited for.  The two-layer tail has no product 2: wait for y2_ready of the previous tile here.
-            if (N3 == 0 && tl > 0) { mbar_wait(y2_ready, (tl - 1) & 1); asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+        return;
+    }
+    if (warp > NCONS) return;
+
+    // ===== consumers =====
+    const int wgi = warp >> 2, w = warp & 3;
+    const int rA = 16 * w + (lane >> 2);                     // this thread's fragment rows: rA and rA + 8
+    int it1 = 0, it2 = 0;
+    for (int t = blockIdx.x; t < g.tiles; t += gridDim.x) {
+        const int p = t / g.tiles_per_prob, m0 = (t - p * g.tiles_per_prob) * TAIL_BM;
+        const TailProb& pr = g.p[p];
+        const bool ok0 = m0 + rA < g.M, ok1 = m0 + rA + 8 < g.M;
+        float hp[2][TAIL_HPW];
+#pragma unroll
+        for (int n = 0; n < TAIL_HPW; n++) hp[0][n] = hp[1][n] = 0.f;
+        const float* wh = s_wh + (size_t)pr.wh_row0 * NL;
+        {
+            // ---- product 1 and y2
+            float acc[NH2 / 2];
+            int prev = -1;
             for (int i = 0; i < KB1; i++, it1++) {
                 const int s = it1 % S1, ph = (it1 / S1) & 1;
                 mbar_wait(&full1[s], ph);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (elect_one()) {
-                    const uint64_t da = make_desc(r1 + (size_t)s * STAGE1), db = make_desc(r1 + (size_t)s * STAGE1 + BM * BK * 4);
-#pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; k++) umma_tf32(tmem_base, da + 2 * k, db + 2 * k, idesc1, (i > 0 || k > 0) ? 1u : 0u);
-                    umma_commit(&empty1[s]);
-                    if (i == KB1 - 1) umma_commit(acc1_full);
-                }
-                __syncwarp();
+                const uint8_t* a = r1 + (size_t)s * STAGE1;
+                wg::fence();
+                wg::mma_kblock<NH2>(acc, a, a + TAIL_BM * BK * 4 + (size_t)wgi * NH2 * 128, i > 0);
+                wg::commit();
+                if (prev >= 0) { wg::wait<1>(); if (lane == 0) mbar_arrive(&empty1[prev]); }
+                prev = s;
             }
-            if (N3 > 0) {
-                mbar_wait(y2_ready, tl & 1);                                   // the epilogue has laid the y2 tile out in ring 1
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                for (int i = 0; i < KB2; i++, it2++) {
-                    const int s = it2 % S2, ph = (it2 / S2) & 1;
-                    mbar_wait(&full2[s], ph);
-                    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                    if (elect_one()) {
-                        const uint64_t da = make_desc(r1 + (size_t)i * BM * BK * 4), db = make_desc(r2 + (size_t)s * STAGE2);
-#pragma unroll
-                        for (int k = 0; k < BK / UMMA_K; k++) umma_tf32(tmem_base + 256u, da + 2 * k, db + 2 * k, idesc2, (i > 0 || k > 0) ? 1u : 0u);
-                        umma_commit(&empty2[s]);
-                        if (i == KB2 - 1) { umma_commit(acc2_full); umma_commit(r1_free); }
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-    } else {
-        // ===== epilogue: 16 warps; warp = (TMEM lane quarter q, column group grp); thread = one row of the block =====
-        const int ew = warp - 2, q = warp & 3, grp = ew >> 2, rl = 32 * q + lane;
-        int tl = 0;
-        for (int t = blockIdx.x; t < g.tiles; t += gridDim.x, tl++) {
-            const int p = t / g.tiles_per_prob, m0 = (t - p * g.tiles_per_prob) * BM;
-            const TailProb& pr = g.p[p];
-            const int row = m0 + rl;
-            const bool row_ok = row < g.M;
+            wg::wait<0>();
+            if (lane == 0) mbar_arrive(&empty1[prev]);
             const float* b2 = s_b2 + p * N2;
-            float h[TAIL_HPW];
 #pragma unroll
-            for (int n = 0; n < TAIL_HPW; n++) h[n] = 0.f;
-            mbar_wait(acc1_full, tl & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (N3 == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");      // the previous tile's block has left the staging buffer
-            if (N3 == 0) __syncwarp();
-#pragma unroll 1
-            for (int c = grp; c < N2 / 32; c += G) {
-                uint32_t r[32];
-                tmem_ld32(tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(32 * c), r);
-                float v[32];
-#pragma unroll
-                for (int j = 0; j < 32; j++) v[j] = elu_fast(__uint_as_float(r[j]) + b2[32 * c + j]);
-                // the warp's 32 x 32 block, 128-byte rows, 16-byte chunks XOR-swizzled by row % 8: the layout TMA reads / writes with
-                // CU_TENSOR_MAP_SWIZZLE_128B and the K-major UMMA descriptor expects.  Three-layer tail: k-block c of product 2's A operand.
-                uint8_t* blk = (N3 > 0) ? (r1 + (size_t)c * (BM * BK * 4) + (size_t)(32 * q) * 128) : (ystg + (size_t)ew * 4096);
-                uint8_t* trow = blk + (size_t)lane * 128;
-#pragma unroll
-                for (int j = 0; j < 8; j++)
-                    *reinterpret_cast<float4*>(trow + ((j ^ (lane & 7)) << 4)) = row_ok ? make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3])
-                                                                                     : make_float4(0.f, 0.f, 0.f, 0.f);
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // generic-proxy stores -> visible to the async proxy (tensor core, TMA store)
-                __syncwarp();
-                if (lane == 0) {
-                    tma_store_2d(&maps.y2[p], blk, 32 * c, m0 + 32 * q);           // rows beyond M are clipped
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                }
-                if (N3 == 0) {      // two-layer tail: the head reads y2 from registers
-                    const float* wh = s_wh + (size_t)pr.wh_row0 * NL + 32 * c;
-#pragma unroll
-                    for (int n = 0; n < TAIL_HPW; n++) {
-                        if (n < pr.nh) {
-                            const float4* w = reinterpret_cast<const float4*>(wh + n * NL);
-                            float a = h[n];
-#pragma unroll
-                            for (int j = 0; j < 8; j++) { const float4 ww = w[j]; a = fmaf(v[4 * j], ww.x, a); a = fmaf(v[4 * j + 1], ww.y, a); a = fmaf(v[4 * j + 2], ww.z, a); a = fmaf(v[4 * j + 3], ww.w, a); }
-                            h[n] = a;
-                        }
-                    }
-                }
+            for (int j = 0; j < NH2 / 8; j++) {
+                const float2 bb = *reinterpret_cast<const float2*>(b2 + wgi * NH2 + 8 * j + 2 * (lane & 3));
+                acc[4 * j] = ok0 ? elu_fast(acc[4 * j] + bb.x) : 0.f; acc[4 * j + 1] = ok0 ? elu_fast(acc[4 * j + 1] + bb.y) : 0.f;
+                acc[4 * j + 2] = ok1 ? elu_fast(acc[4 * j + 2] + bb.x) : 0.f; acc[4 * j + 3] = ok1 ? elu_fast(acc[4 * j + 3] + bb.y) : 0.f;
             }
-            asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-            mbar_arrive(y2_ready);
-            if (N3 > 0) {
-                mbar_wait(acc2_full, tl & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                if (lane == 0) { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); mbar_arrive(y2_stored); }      // the y2 stores have read ring 1
-                const float* b3 = s_b3 + p * N3;
-#pragma unroll 1
-                for (int c = grp; c < (N3 > 0 ? N3 : 32) / 32; c += G) {
-                    uint32_t r[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(32 * q) << 16) + 256u + (uint32_t)(32 * c), r);
-                    float v[32];
-#pragma unroll
-                    for (int j = 0; j < 32; j++) v[j] = elu_fast(__uint_as_float(r[j]) + b3[32 * c + j]);
-                    if (row_ok) {
-                        float4* dst = reinterpret_cast<float4*>(pr.y3 + (size_t)row * pr.ldy3 + 32 * c);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) dst[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                    }
-                    const float* wh = s_wh + (size_t)pr.wh_row0 * NL + 32 * c;
-#pragma unroll
-                    for (int n = 0; n < TAIL_HPW; n++) {
-                        if (n < pr.nh) {
-                            const float4* w = reinterpret_cast<const float4*>(wh + n * NL);
-                            float a = h[n];
-#pragma unroll
-                            for (int j = 0; j < 8; j++) { const float4 ww = w[j]; a = fmaf(v[4 * j], ww.x, a); a = fmaf(v[4 * j + 1], ww.y, a); a = fmaf(v[4 * j + 2], ww.z, a); a = fmaf(v[4 * j + 3], ww.w, a); }
-                            h[n] = a;
-                        }
-                    }
-                }
-            }
-            // the head: partial sums of column groups 1..G-1 meet group 0's in shared memory ([group][output][row]: conflict-free)
-            if (grp > 0) {
-#pragma unroll
-                for (int n = 0; n < TAIL_HPW; n++) if (n < pr.nh) s_hp[((grp - 1) * TAIL_HPW + n) * BM + rl] = h[n];
-            }
-            asm volatile("bar.sync 1, %0;" ::"r"(128 * G) : "memory");
-            if (grp == 0 && row_ok) {
-                const float* bh = s_bh + p * 16;
-#pragma unroll
-                for (int n = 0; n < TAIL_HPW; n++) {
-                    if (n < pr.nh) {
-                        float a = h[n] + bh[n];
-#pragma unroll
-                        for (int gg = 0; gg < G - 1; gg++) a += s_hp[(gg * TAIL_HPW + n) * BM + rl];
-                        pr.out[(size_t)row * pr.ldout + n] = a;
-                    }
-                }
-            }
-            // Three-layer tail: s_hp is rewritten only after the next tile's acc2_full, i.e. after y2_ready of that tile, which group 0's threads
-            // reach after these reads.  Two-layer tail: the next tile's partial sums can be ready sooner, so hold everybody until they are read.
-            if (N3 == 0) asm volatile("bar.sync 1, %0;" ::"r"(128 * G) : "memory");
+            // (the previous block's readers of the y2 tile -- product 2 and the TMA stores -- were waited for at the end of that block)
+            store_fragment<NH2 / 8>(acc, y2t, wgi * NH2, w, lane, [](float2 v, int, int) { return v; });
+            if (N3 == 0) head_partial<NH2 / 8>(acc, wh, NL, pr.nh, wgi * NH2, lane, hp);       // two-layer tail: the head reads y2
         }
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+        fence_async_smem();                                  // generic-proxy stores -> visible to the async proxy (tensor core, TMA store)
+        cons_sync();
+        if (lane == 0) {
+            for (int b = warp; b < 2 * KB2; b += NCONS) tma_store_2d(&maps.y2[p], y2t + (size_t)b * 4096, 32 * (b >> 1), m0 + 32 * (b & 1));      // rows beyond M are clipped
+            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+        }
+        if (N3 > 0) {
+            // ---- product 2 (A = the y2 tile), y3 and the head
+            float acc[NH3 / 2];
+            int prev = -1;
+            for (int i = 0; i < KB2; i++, it2++) {
+                const int s = it2 % S2, ph = (it2 / S2) & 1;
+                mbar_wait(&full2[s], ph);
+                wg::fence();
+                wg::mma_kblock<NH3>(acc, y2t + (size_t)i * (TAIL_BM * 128), r2 + (size_t)s * STAGE2 + (size_t)wgi * NH3 * 128, i > 0);
+                wg::commit();
+                if (prev >= 0) { wg::wait<1>(); if (lane == 0) mbar_arrive(&empty2[prev]); }
+                prev = s;
+            }
+            wg::wait<0>();
+            if (lane == 0) mbar_arrive(&empty2[prev]);
+            const float* b3 = s_b3 + p * N3;
+#pragma unroll
+            for (int j = 0; j < NH3 / 8; j++) {
+                const int col = wgi * NH3 + 8 * j + 2 * (lane & 3);
+                const float2 bb = *reinterpret_cast<const float2*>(b3 + col);
+                acc[4 * j] = elu_fast(acc[4 * j] + bb.x); acc[4 * j + 1] = elu_fast(acc[4 * j + 1] + bb.y);
+                acc[4 * j + 2] = elu_fast(acc[4 * j + 2] + bb.x); acc[4 * j + 3] = elu_fast(acc[4 * j + 3] + bb.y);
+                if (ok0) *reinterpret_cast<float2*>(pr.y3 + (size_t)(m0 + rA) * pr.ldy3 + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+                if (ok1) *reinterpret_cast<float2*>(pr.y3 + (size_t)(m0 + rA + 8) * pr.ldy3 + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+            }
+            head_partial<NH3 / 8>(acc, wh, NL, pr.nh, wgi * NH3, lane, hp);
+        }
+        // the head: sum over the four lanes that share a row, then warpgroup 1's half meets warpgroup 0's in shared memory
+#pragma unroll
+        for (int n = 0; n < TAIL_HPW; n++) {
+            if (n < pr.nh) {
+#pragma unroll
+                for (int r = 0; r < 2; r++) {
+                    float a = hp[r][n];
+                    a += __shfl_xor_sync(0xffffffffu, a, 1);
+                    a += __shfl_xor_sync(0xffffffffu, a, 2);
+                    hp[r][n] = a;
+                }
+                if (wgi == 1 && (lane & 3) == 0) { s_hp[n * TAIL_BM + rA] = hp[0][n]; s_hp[n * TAIL_BM + rA + 8] = hp[1][n]; }
+            }
+        }
+        cons_sync();
+        if (wgi == 0 && (lane & 3) == 0) {
+            const float* bh = s_bh + p * 16;
+#pragma unroll
+            for (int n = 0; n < TAIL_HPW; n++) {
+                if (n < pr.nh) {
+                    if (ok0) pr.out[(size_t)(m0 + rA) * pr.ldout + n] = hp[0][n] + s_hp[n * TAIL_BM + rA] + bh[n];
+                    if (ok1) pr.out[(size_t)(m0 + rA + 8) * pr.ldout + n] = hp[1][n] + s_hp[n * TAIL_BM + rA + 8] + bh[n];
+                }
+            }
+        }
+        // the y2 tile and the head exchange are rewritten by the next block: the TMA stores have read the tile, every warp is past its reads
+        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        cons_sync();
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS) : "memory");
-    }
+    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
 template <int K1, int N2, int N3>
@@ -1078,10 +816,9 @@ int launch_tail(const TailMaps& maps, const TailArgs& g, cudaStream_t st) {
         if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
         configured = true;
     }
-    static int sms = 0;
-    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
+    const int sms = sm_count();
     const int grid = g.tiles < sms ? g.tiles : sms;
-    mlp_tail_fwd_kernel<K1, N2, N3><<<grid, 64 + 128 * TAIL_G, smem, st>>>(maps, g);
+    mlp_tail_fwd_kernel<K1, N2, N3><<<grid, 32 * NCONS + 128, smem, st>>>(maps, g);
     go1_count_launch(1);
     return 0;
 }
@@ -1089,25 +826,26 @@ int launch_tail(const TailMaps& maps, const TailArgs& g, cudaStream_t st) {
 // ---------------------------------------------------------------------------------------------------------------
 // Fused MLP tail, backward (first half): for the bodies 512-256-128-head (actor_critic.py:38-77), from the gradient of the head's output,
 //     dz3 = (dout Wh) * ELU'(y3)   [M][128]     CUDA cores: K = nh <= 12
-//     dz2 = (dz3 W3) * ELU'(y2)    [M][256]     tensor core: A = the dz3 tile the epilogue warps laid out in shared memory, B = W3 (resident)
+//     dz2 = (dz3 W3) * ELU'(y2)    [M][256]     tensor core: A = the dz3 tile the consumer warps laid out in shared memory, B = W3 (resident)
 // plus the bias gradients gb3 = colsum(dz3), gb2 = colsum(dz2), for up to two problems (actor + critic) in one grid.  This replaces, per
-// body, a skinny dgrad launch and a 24576 x 256 x 128 tcgen05 dgrad launch (which re-reads dz3 from memory and whose tiles are too
-// short to hide their epilogue): dz3 never leaves the SM between the two products.  The wgrads (dz3^T y2, dz2^T y1) and the last dgrad
-// (dz1) stay separate products.  One CTA (576 threads) per 128-row block:
-//   warp 0      loads W3 (128 KB, MN-major boxes) once per problem it meets
-//   warp 1      one product per block: 16 tcgen05.mma (M = 128, N = 256, K = 8) -> TMEM columns [0, 256)
-//   warps 2-17  (TMEM lane quarter q, column group grp): E0 builds dz3 chunk grp of the block from dout, Wh (shared memory) and y3,
-//               writes it swizzled into the A tile and sends it to global memory by TMA; E1 drains the accumulator chunks grp, grp + 4,
-//               multiplies by ELU'(y2), stages them in the warp's own (by then consumed) 4 KB block of the A tile and sends them by TMA.
+// body, a skinny dgrad launch and a 24576 x 256 x 128 dgrad launch (which re-reads dz3 from memory and whose tiles are too short to hide
+// their epilogue): dz3 never leaves the SM between the two products.  The wgrads (dz3^T y2, dz2^T y1) and the last dgrad (dz1) stay
+// separate products.  One CTA (384 threads) per 64-row block:
+//   warp 8      loads W3 ([K = 128][N = 256], MN-major) as four unswizzled [32][256] boxes whenever the CTA meets a new problem
+//   warps 0-7   transpose those boxes into the resident K-major operand (128 KB); per block: E0, warp = (32-row half, 32-column chunk),
+//               builds a dz3 chunk from dout, Wh (shared memory) and y3, writes it swizzled into the A tile and sends it to global memory
+//               by TMA; then warpgroup g multiplies the tile by columns [128 g, 128 g + 128) of W3 (16 wgmma) and E1 multiplies the
+//               accumulator fragments by ELU'(y2) and stores dz2 from registers.
 // Column sums meet in shared memory (atomics) and are flushed once per CTA.
 // ---------------------------------------------------------------------------------------------------------------
-struct TailBwdProb { const float* dout; const float* Wh; const float* y3; const float* y2; float* gb3; float* gb2; int lddout, nh, ldy3, ldy2; };
+struct TailBwdProb { const float* dout; const float* Wh; const float* y3; const float* y2; float* dz2; float* gb3; float* gb2; int lddout, nh, ldy3, ldy2, lddz2; };
 struct TailBwdArgs { TailBwdProb p[TAIL_MAXP]; int nprob, M, tiles_per_prob, tiles; };
-struct TailBwdMaps { CUtensorMap w3[TAIL_MAXP], dz3[TAIL_MAXP], dz2[TAIL_MAXP]; };
+struct TailBwdMaps { CUtensorMap w3[TAIL_MAXP], dz3[TAIL_MAXP]; };
 constexpr int TB_N3 = 128, TB_N2 = 256;
-constexpr int TB_W3_BYTES = TB_N3 * TB_N2 * 4;                 // 128 KB: 4 k-blocks x 8 boxes x 4 KB
-constexpr int TB_Z3_BYTES = BM * TB_N3 * 4;                    // 64 KB: 4 k-blocks x [128 rows][32 floats]
-constexpr int TB_SMEM = TB_W3_BYTES + TB_Z3_BYTES + (TAIL_MAXP * TAIL_HPW * TB_N3 + TAIL_MAXP * (TB_N3 + TB_N2)) * 4 + 8 * 8 + 16 + 1024;
+constexpr int TB_W3_BYTES = TB_N3 * TB_N2 * 4;                 // 128 KB: 4 k-blocks x [256 n][32 k]
+constexpr int TB_RAW_BYTES = BK * TB_N2 * 4;                   // 32 KB: one box [32 k][256 n]
+constexpr int TB_Z3_BYTES = TAIL_BM * TB_N3 * 4;               // 32 KB: 4 k-blocks x [64 rows][32 floats]
+constexpr int TB_SMEM = TB_W3_BYTES + TB_RAW_BYTES + TB_Z3_BYTES + (TAIL_MAXP * TAIL_HPW * TB_N3 + TAIL_MAXP * (TB_N3 + TB_N2)) * 4 + 2 * 8 + 16 + 1024;
 
 // column sums of a 32 x 32 block held one row per lane (v[j] = column j): 31 shuffles; lane l ends up with column l
 __device__ __forceinline__ float warp_colsum32(const float (&v)[32], const int lane) {
@@ -1127,200 +865,157 @@ __device__ __forceinline__ float warp_colsum32(const float (&v)[32], const int l
     return sred[0];
 }
 
-__global__ void __launch_bounds__(64 + 128 * TAIL_G, 1) mlp_tail_bwd_kernel(const __grid_constant__ TailBwdMaps maps, const TailBwdArgs g) {
-    constexpr int G = TAIL_G;
+__global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_bwd_kernel(const __grid_constant__ TailBwdMaps maps, const TailBwdArgs g) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* base = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint8_t* w3s = base;                                     // B operand: [4 k-blocks][8 boxes][32 k-rows][32 n-floats]
-    uint8_t* z3 = base + TB_W3_BYTES;                        // A operand: [4 k-blocks][128 rows][32 floats], 128B-swizzled
+    uint8_t* w3s = base;                                     // B operand: [4 k-blocks][256 n][32 k], 128B-swizzled
+    uint8_t* raw = base + TB_W3_BYTES;                       // one W3 box as TMA delivers it
+    uint8_t* z3 = raw + TB_RAW_BYTES;                        // A operand: [4 k-blocks][64 rows][32 floats], 128B-swizzled
     float* s_wh = (float*)(z3 + TB_Z3_BYTES);                // [MAXP][HPW][128]
     float* s_cs = s_wh + TAIL_MAXP * TAIL_HPW * TB_N3;       // [MAXP][128 + 256] column sums (bias gradients)
-    uint64_t* w3_full = (uint64_t*)(s_cs + TAIL_MAXP * (TB_N3 + TB_N2));
-    uint64_t* w3_free = w3_full + 1;
-    uint64_t* z3_ready = w3_free + 1;
-    uint64_t* acc_full = z3_ready + 1;
-    uint32_t* tmem_slot = (uint32_t*)(acc_full + 1);
+    uint64_t* raw_full = (uint64_t*)(s_cs + TAIL_MAXP * (TB_N3 + TB_N2));
+    uint64_t* raw_free = raw_full + 1;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int p = 0; p < g.nprob; p++) {
             asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.w3[p]) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.dz3[p]) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.dz2[p]) : "memory");
         }
-        mbar_init(w3_full, 1); mbar_init(w3_free, 1); mbar_init(z3_ready, 128 * G); mbar_init(acc_full, 1);
+        mbar_init(raw_full, 1); mbar_init(raw_free, NCONS);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(256u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
     }
     for (int i = threadIdx.x; i < TAIL_MAXP * TAIL_HPW * TB_N3; i += blockDim.x) {
         const int p = i / (TAIL_HPW * TB_N3), r = (i / TB_N3) % TAIL_HPW, k = i % TB_N3;
         s_wh[i] = (p < g.nprob && r < g.p[p].nh) ? __ldg(g.p[p].Wh + (size_t)r * TB_N3 + k) : 0.f;
     }
     for (int i = threadIdx.x; i < TAIL_MAXP * (TB_N3 + TB_N2); i += blockDim.x) s_cs[i] = 0.f;
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
-        // ===== W3 loader: the weights of the problem this CTA's blocks belong to stay resident; reloaded when the problem changes =====
+    if (warp == NCONS) {
+        // ===== W3 loader: one box at a time, for every new problem among this CTA's blocks (the consumers follow the same sequence) =====
         if (elect_one()) {
-            int cur = -1, tl = 0;
-            for (int t = blockIdx.x; t < g.tiles; t += gridDim.x, tl++) {
+            int cur = -1, nbox = 0;
+            for (int t = blockIdx.x; t < g.tiles; t += gridDim.x) {
                 const int p = t / g.tiles_per_prob;
-                // follow the products block by block (every phase of w3_free is consumed in order: a parity wait that skipped phases would
-                // alias and let this thread run two loads ahead): block tl - 1's product has read the weights
-                if (tl > 0) mbar_wait(w3_free, (tl - 1) & 1);
                 if (p == cur) continue;
                 cur = p;
-                mbar_expect_tx(w3_full, TB_W3_BYTES);
-                for (int kb = 0; kb < TB_N3 / BK; kb++)
-#pragma unroll
-                    for (int x = 0; x < TB_N2 / 32; x++) tma_load_2d(&maps.w3[p], w3_full, w3s + (size_t)kb * (TB_N2 * BK * 4) + (size_t)x * (32 * BK * 4), 32 * x, kb * BK);
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer: A = dz3 tile (K-major), B = W3 given as [K = 128][N = 256] (MN-major) =====
-        const uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 16) | ((uint32_t)(TB_N2 >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-        int cur = -1, nload = 0, tl = 0;
-        for (int t = blockIdx.x; t < g.tiles; t += gridDim.x, tl++) {
-            const int p = t / g.tiles_per_prob;
-            if (p != cur) { cur = p; mbar_wait(w3_full, nload & 1); nload++; }
-            mbar_wait(z3_ready, tl & 1);                                   // the dz3 tile is in shared memory; the previous accumulator has been drained
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            if (elect_one()) {
-#pragma unroll
-                for (int kb = 0; kb < TB_N3 / BK; kb++) {
-                    const uint64_t da = make_desc(z3 + (size_t)kb * (BM * BK * 4)), db = make_desc_mn(w3s + (size_t)kb * (TB_N2 * BK * 4));
-#pragma unroll
-                    for (int k = 0; k < BK / UMMA_K; k++) umma_tf32(tmem_base, da + 2 * k, db + (uint64_t)(1024 >> 4) * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
+                for (int kb = 0; kb < TB_N3 / BK; kb++, nbox++) {
+                    mbar_wait(raw_free, (nbox & 1) ^ 1);
+                    mbar_expect_tx(raw_full, TB_RAW_BYTES);
+                    tma_load_2d(&maps.w3[p], raw_full, raw, 0, kb * BK);
                 }
-                umma_commit(acc_full);
-                umma_commit(w3_free);
             }
-            __syncwarp();
         }
-    } else {
-        // ===== epilogue warps =====
-        const int ew = warp - 2, q = warp & 3, grp = ew >> 2;
-        uint8_t* myblk = z3 + (size_t)(4 * grp + q) * 4096;           // chunk grp, rows 32 q .. 32 q + 31 of the A tile; later this warp's staging
-        int tl = 0;
-        for (int t = blockIdx.x; t < g.tiles; t += gridDim.x, tl++) {
-            const int p = t / g.tiles_per_prob, m0 = (t - p * g.tiles_per_prob) * BM;
-            const TailBwdProb& pr = g.p[p];
-            const int row = m0 + 32 * q + lane;
+        return;
+    }
+    if (warp > NCONS) return;
+
+    // ===== consumers =====
+    const int wgi = warp >> 2, w = warp & 3, ctid = threadIdx.x;
+    const int h = warp & 1, cg = warp >> 1;                             // E0: rows 32 h .. 32 h + 31 of the block, dz3 columns 32 cg .. 32 cg + 31
+    uint8_t* myblk = z3 + (size_t)cg * (TAIL_BM * 128) + h * 4096;
+    const int rA = 16 * w + (lane >> 2);                                // E1: this thread's fragment rows rA and rA + 8
+    int cur = -1, nbox = 0;
+    for (int t = blockIdx.x; t < g.tiles; t += gridDim.x) {
+        const int p = t / g.tiles_per_prob, m0 = (t - p * g.tiles_per_prob) * TAIL_BM;
+        const TailBwdProb& pr = g.p[p];
+        float* cs = s_cs + p * (TB_N3 + TB_N2);
+        if (p != cur) {      // the previous problem's products are complete (end-of-block barrier): bring this problem's W3 into K-major form
+            cur = p;
+            for (int kb = 0; kb < TB_N3 / BK; kb++, nbox++) {
+                mbar_wait(raw_full, nbox & 1);
+                transpose_tile<TB_N2>((const float*)raw, w3s + (size_t)kb * (TB_N2 * 128), ctid);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(raw_free);
+            }
+        }
+        // ---- E0: dz3 chunk cg = (dout Wh)[.., 32 cg ..] * ELU'(y3)
+        {
+            const int row = m0 + 32 * h + lane;
             const bool row_ok = row < g.M;
-            float* cs = s_cs + p * (TB_N3 + TB_N2);
-            // ---- E0: dz3 chunk grp = (dout Wh)[.., 32 grp ..] * ELU'(y3)
-            {
-                float4 y[8];
-                const float4* yrow = reinterpret_cast<const float4*>(pr.y3 + (size_t)(row_ok ? row : 0) * pr.ldy3 + 32 * grp);
+            float4 y[8];
+            const float4* yrow = reinterpret_cast<const float4*>(pr.y3 + (size_t)(row_ok ? row : 0) * pr.ldy3 + 32 * cg);
 #pragma unroll
-                for (int j = 0; j < 8; j++) y[j] = __ldg(yrow + j);
-                float d[TAIL_HPW];
+            for (int j = 0; j < 8; j++) y[j] = __ldg(yrow + j);
+            float d[TAIL_HPW];
 #pragma unroll
-                for (int n = 0; n < TAIL_HPW; n++) d[n] = (row_ok && n < pr.nh) ? __ldg(pr.dout + (size_t)row * pr.lddout + n) : 0.f;
-                float v[32];
+            for (int n = 0; n < TAIL_HPW; n++) d[n] = (row_ok && n < pr.nh) ? __ldg(pr.dout + (size_t)row * pr.lddout + n) : 0.f;
+            float v[32];
 #pragma unroll
-                for (int j = 0; j < 32; j++) v[j] = 0.f;
-                const float* wh = s_wh + (size_t)p * TAIL_HPW * TB_N3 + 32 * grp;
+            for (int j = 0; j < 32; j++) v[j] = 0.f;
+            const float* wh = s_wh + (size_t)p * TAIL_HPW * TB_N3 + 32 * cg;
 #pragma unroll
-                for (int n = 0; n < TAIL_HPW; n++) {
-                    if (n < pr.nh) {
-                        const float4* w = reinterpret_cast<const float4*>(wh + n * TB_N3);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) {
-                            const float4 ww = w[j];
-                            v[4 * j] = fmaf(d[n], ww.x, v[4 * j]); v[4 * j + 1] = fmaf(d[n], ww.y, v[4 * j + 1]);
-                            v[4 * j + 2] = fmaf(d[n], ww.z, v[4 * j + 2]); v[4 * j + 3] = fmaf(d[n], ww.w, v[4 * j + 3]);
-                        }
-                    }
-                }
-#pragma unroll
-                for (int j = 0; j < 8; j++) {
-                    v[4 * j] *= (y[j].x > 0.f ? 1.0f : y[j].x + 1.0f); v[4 * j + 1] *= (y[j].y > 0.f ? 1.0f : y[j].y + 1.0f);
-                    v[4 * j + 2] *= (y[j].z > 0.f ? 1.0f : y[j].z + 1.0f); v[4 * j + 3] *= (y[j].w > 0.f ? 1.0f : y[j].w + 1.0f);
-                }
-                if (!row_ok) {
-#pragma unroll
-                    for (int j = 0; j < 32; j++) v[j] = 0.f;
-                }
-                const float c3 = warp_colsum32(v, lane);
-                atomicAdd(cs + 32 * grp + lane, c3);
-                if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");      // the previous block's dz2 store has left this warp's block
-                __syncwarp();
-                uint8_t* trow = myblk + (size_t)lane * 128;
-#pragma unroll
-                for (int j = 0; j < 8; j++)
-                    *reinterpret_cast<float4*>(trow + ((j ^ (lane & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                __syncwarp();
-                if (lane == 0) {
-                    tma_store_2d(&maps.dz3[p], myblk, 32 * grp, m0 + 32 * q);
-                    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-                }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-                mbar_arrive(z3_ready);
-            }
-            // ---- E1: dz2 chunks grp, grp + 4 = accumulator * ELU'(y2)
-            {
-                float4 y[8];
-                const float4* yrow = reinterpret_cast<const float4*>(pr.y2 + (size_t)(row_ok ? row : 0) * pr.ldy2 + 32 * grp);
-#pragma unroll
-                for (int j = 0; j < 8; j++) y[j] = __ldg(yrow + j);                 // in flight while the product runs
-                mbar_wait(acc_full, tl & 1);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-                for (int c = grp; c < TB_N2 / 32; c += G) {
-                    if (c != grp) {
-                        const float4* yr2 = reinterpret_cast<const float4*>(pr.y2 + (size_t)(row_ok ? row : 0) * pr.ldy2 + 32 * c);
-#pragma unroll
-                        for (int j = 0; j < 8; j++) y[j] = __ldg(yr2 + j);
-                    }
-                    uint32_t r[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(32 * q) << 16) + (uint32_t)(32 * c), r);
-                    float v[32];
+            for (int n = 0; n < TAIL_HPW; n++) {
+                if (n < pr.nh) {
+                    const float4* wv = reinterpret_cast<const float4*>(wh + n * TB_N3);
 #pragma unroll
                     for (int j = 0; j < 8; j++) {
-                        v[4 * j] = __uint_as_float(r[4 * j]) * (y[j].x > 0.f ? 1.0f : y[j].x + 1.0f);
-                        v[4 * j + 1] = __uint_as_float(r[4 * j + 1]) * (y[j].y > 0.f ? 1.0f : y[j].y + 1.0f);
-                        v[4 * j + 2] = __uint_as_float(r[4 * j + 2]) * (y[j].z > 0.f ? 1.0f : y[j].z + 1.0f);
-                        v[4 * j + 3] = __uint_as_float(r[4 * j + 3]) * (y[j].w > 0.f ? 1.0f : y[j].w + 1.0f);
-                    }
-                    if (!row_ok) {
-#pragma unroll
-                        for (int j = 0; j < 32; j++) v[j] = 0.f;
-                    }
-                    const float c2 = warp_colsum32(v, lane);
-                    atomicAdd(cs + TB_N3 + 32 * c + lane, c2);
-                    if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // dz3 store (first chunk) / previous dz2 store has read the block
-                    __syncwarp();
-                    uint8_t* trow = myblk + (size_t)lane * 128;
-#pragma unroll
-                    for (int j = 0; j < 8; j++)
-                        *reinterpret_cast<float4*>(trow + ((j ^ (lane & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    __syncwarp();
-                    if (lane == 0) {
-                        tma_store_2d(&maps.dz2[p], myblk, 32 * c, m0 + 32 * q);
-                        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+                        const float4 ww = wv[j];
+                        v[4 * j] = fmaf(d[n], ww.x, v[4 * j]); v[4 * j + 1] = fmaf(d[n], ww.y, v[4 * j + 1]);
+                        v[4 * j + 2] = fmaf(d[n], ww.z, v[4 * j + 2]); v[4 * j + 3] = fmaf(d[n], ww.w, v[4 * j + 3]);
                     }
                 }
-                asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+            }
+#pragma unroll
+            for (int j = 0; j < 8; j++) {
+                v[4 * j] *= (y[j].x > 0.f ? 1.0f : y[j].x + 1.0f); v[4 * j + 1] *= (y[j].y > 0.f ? 1.0f : y[j].y + 1.0f);
+                v[4 * j + 2] *= (y[j].z > 0.f ? 1.0f : y[j].z + 1.0f); v[4 * j + 3] *= (y[j].w > 0.f ? 1.0f : y[j].w + 1.0f);
+            }
+            if (!row_ok) {
+#pragma unroll
+                for (int j = 0; j < 32; j++) v[j] = 0.f;
+            }
+            const float c3 = warp_colsum32(v, lane);
+            atomicAdd(cs + 32 * cg + lane, c3);
+            uint8_t* trow = myblk + (size_t)lane * 128;
+#pragma unroll
+            for (int j = 0; j < 8; j++)
+                *reinterpret_cast<float4*>(trow + ((j ^ (lane & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+            fence_async_smem();
+            __syncwarp();
+            if (lane == 0) {
+                tma_store_2d(&maps.dz3[p], myblk, 32 * cg, m0 + 32 * h);
+                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             }
         }
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+        cons_sync();                                                    // the dz3 tile (and, for a new problem, W3) is in shared memory
+        // ---- the product and E1: dz2 columns [128 wgi, 128 wgi + 128) = accumulator * ELU'(y2)
+        {
+            float acc[64];
+            wg::fence();
+#pragma unroll
+            for (int kb = 0; kb < TB_N3 / BK; kb++)
+                wg::mma_kblock<128>(acc, z3 + (size_t)kb * (TAIL_BM * 128), w3s + (size_t)kb * (TB_N2 * 128) + (size_t)wgi * 128 * 128, kb > 0);
+            wg::commit();
+            wg::wait<0>();
+            const bool ok0 = m0 + rA < g.M, ok1 = m0 + rA + 8 < g.M;
+            const float* y0 = pr.y2 + (size_t)(ok0 ? m0 + rA : 0) * pr.ldy2;
+            const float* y1 = pr.y2 + (size_t)(ok1 ? m0 + rA + 8 : 0) * pr.ldy2;
+#pragma unroll
+            for (int j = 0; j < 16; j++) {
+                const int col = 128 * wgi + 8 * j + 2 * (lane & 3);
+                const float2 ya = __ldg(reinterpret_cast<const float2*>(y0 + col)), yb = __ldg(reinterpret_cast<const float2*>(y1 + col));
+                float2 va = make_float2(acc[4 * j] * (ya.x > 0.f ? 1.0f : ya.x + 1.0f), acc[4 * j + 1] * (ya.y > 0.f ? 1.0f : ya.y + 1.0f));
+                float2 vb = make_float2(acc[4 * j + 2] * (yb.x > 0.f ? 1.0f : yb.x + 1.0f), acc[4 * j + 3] * (yb.y > 0.f ? 1.0f : yb.y + 1.0f));
+                if (!ok0) va = make_float2(0.f, 0.f);
+                if (!ok1) vb = make_float2(0.f, 0.f);
+                if (ok0) *reinterpret_cast<float2*>(pr.dz2 + (size_t)(m0 + rA) * pr.lddz2 + col) = va;
+                if (ok1) *reinterpret_cast<float2*>(pr.dz2 + (size_t)(m0 + rA + 8) * pr.lddz2 + col) = vb;
+                float sx = va.x + vb.x, sy = va.y + vb.y;              // column sums over the warp's 16 rows: lanes with equal lane % 4 share columns
+#pragma unroll
+                for (int off = 4; off <= 16; off <<= 1) { sx += __shfl_xor_sync(0xffffffffu, sx, off); sy += __shfl_xor_sync(0xffffffffu, sy, off); }
+                if (lane < 4) { atomicAdd(cs + TB_N3 + col, sx); atomicAdd(cs + TB_N3 + col + 1, sy); }
+            }
+        }
+        // the dz3 tile is rewritten by the next block: its TMA stores have read it, both warpgroups' products are complete
+        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+        cons_sync();
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
-    }
+    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    cons_sync();
     // bias gradients: one set of atomics per CTA
-    for (int i = threadIdx.x; i < g.nprob * (TB_N3 + TB_N2); i += blockDim.x) {
+    for (int i = ctid; i < g.nprob * (TB_N3 + TB_N2); i += 32 * NCONS) {
         const int p = i / (TB_N3 + TB_N2), c = i - p * (TB_N3 + TB_N2);
         const float vsum = s_cs[p * (TB_N3 + TB_N2) + c];
         if (vsum != 0.f) atomicAdd(c < TB_N3 ? g.p[p].gb3 + c : g.p[p].gb2 + (c - TB_N3), vsum);
@@ -1328,9 +1023,6 @@ __global__ void __launch_bounds__(64 + 128 * TAIL_G, 1) mlp_tail_bwd_kernel(cons
 }
 
 }  // namespace
-
-static int g_tf32_wide = 1;   // wide = 128 x 256 tiles / cta_group::2 pairs where the heuristic in go1_gemm_tf32 says they pay
-extern "C" void go1_gemm_tf32_set_wide(int on) { g_tf32_wide = on; }
 
 // ---- optional per-launch timing of the tensor-core GEMM (bench.py's roofline): CUDA events on the launch stream around every
 // go1_gemm impl=1 call between go1_gemm_timing(1, ..) and go1_gemm_timing(0, ..)
@@ -1359,7 +1051,7 @@ extern "C" int go1_gemm_timing(int on, double* total_ms, double* total_flop, lon
         if (csv && i / 2 < g_time_recs.size()) {
             const TimeRec& r = g_time_recs[i / 2];
             fprintf(csv, "%d,%d,%d,%d,%d,%d,%d,%d,%s,%d,%.2f\n", r.M, r.N, r.K, r.amn, r.bmn, r.act, r.nex, r.splits,
-                    r.kern >= 1000 ? (r.kern == 1004 ? "tailbwd" : (r.kern == 1003 ? "tail3" : "tail2")) : r.kern == 2 ? "2cta" : (r.kern == 256 ? "p256" : (r.kern == 128 ? "p128" : (r.kern == 64 ? "p64" : "p32"))), r.colsum, 1e3 * t);
+                    r.kern >= 1000 ? (r.kern == 1004 ? "tailbwd" : (r.kern == 1003 ? "tail3" : "tail2")) : (r.kern == 128 ? "p128" : (r.kern == 64 ? "p64" : "p32")), r.colsum, 1e3 * t);
         }
     }
     if (csv) fclose(csv);
@@ -1390,38 +1082,28 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     if (g.nex < 0 || g.nex > 4) return go1_set_error("go1_gemm_ex: num_extra must be 0..4");
     if (act == 2 && !g.aux) return go1_set_error("go1_gemm_ex: act 2 needs dact_y");
     const int num_kb = (K + BK - 1) / BK;
-    // Tile selection.  The products with fp32 operands sit at the chip's L2 -> SM throughput cap (ncu: 11.4 TB/s), so bytes per flop decide:
-    // "wide" shapes (K >= 1024, N >= 256) run as cta_group::2 256 x 256 tile pairs (0.5x the bytes of the 128 x 128 tiling; 128 x 256
-    // single-CTA tiles when M < 256) -- when the tile count still fills the SMs evenly (a 160-tile product would run two half-empty rounds)
-    // or split-K makes up for it; everything else runs 128 x BN tiles on the persistent kernel with the staged epilogue.
-    static const int wide_min_k = getenv("GO1_TF32_WIDE_MINK") ? atoi(getenv("GO1_TF32_WIDE_MINK")) : 1024;
-    static const int wide_min_tiles = getenv("GO1_TF32_WIDE_MINTILES") ? atoi(getenv("GO1_TF32_WIDE_MINTILES")) : 9;      // 9: the 256 x 2100 x 24576 adaptation wgrad takes cta_group::2 pairs + split-K (74 -> 62 us)
-    static const int split_ctas = getenv("GO1_TF32_SPLIT_CTAS") ? atoi(getenv("GO1_TF32_SPLIT_CTAS")) : 2 * 148;
+    // Tile selection: 128 x BN tiles, BN = the smallest of 32 / 64 / 128 that covers N (128 beyond).  Products whose tiles do not fill the SMs
+    // and whose reduction is long are split along K (partial tiles meet in C by vector reductions).
+    static const int split_ctas = getenv("GO1_TF32_SPLIT_CTAS") ? atoi(getenv("GO1_TF32_SPLIT_CTAS")) : 2 * sm_count();
     static const int split_min_kb = getenv("GO1_TF32_SPLIT_MINKB") ? atoi(getenv("GO1_TF32_SPLIT_MINKB")) : 16;
-    const int wtiles = ((M + BM - 1) / BM) * ((N + 255) / 256);
-    static const double wide_min_fill = getenv("GO1_TF32_WIDE_MINFILL") ? atof(getenv("GO1_TF32_WIDE_MINFILL")) : 0.85;
-    const bool fills = wtiles < 148 ? wtiles >= wide_min_tiles : (double)wtiles / (148.0 * ((wtiles + 147) / 148)) >= wide_min_fill;
-    const bool wide = g_tf32_wide && K >= wide_min_k && N >= 256 && (N % 256 == 0 || N >= 1024) && fills;
-    static const int use_2cta = getenv("GO1_TF32_2CTA") ? atoi(getenv("GO1_TF32_2CTA")) : 1;      // cta_group::2 pairs for the wide shapes
-    const bool two_cta = use_2cta && wide && M >= 256 && nprob == 1;
-    const int BN = (wide && nprob == 1) ? 256 : ((N > 64) ? 128 : (N > 32 ? 64 : 32));
+    const int BN = (N > 64) ? 128 : (N > 32 ? 64 : 32);
     const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * nprob;
     int splits = 1;
-    if (tiles < 148 && num_kb >= split_min_kb && g.nex == 0 && act != 2 && g.lead <= 0 && !g.colsum && g.nbx == 0) {      // split-K: about two CTA-units per SM, >= 16 k-blocks each
-        splits = (nprob > 1 ? 148 : split_ctas) / tiles;      // grouped: one CTA-unit per SM (fewer, longer partial sums: less same-address red traffic)
-        if (splits > num_kb / split_min_kb) splits = num_kb / split_min_kb; if (splits < 1) splits = 1;
+    if (tiles < sm_count() && num_kb >= split_min_kb && g.nex == 0 && act != 2 && g.lead <= 0 && !g.colsum && g.nbx == 0) {      // split-K: about two CTA-units per SM, >= 16 k-blocks each
+        splits = (nprob > 1 ? sm_count() : split_ctas) / tiles;      // grouped: one CTA-unit per SM (fewer, longer partial sums: less same-address red traffic)
+        if (splits > num_kb / split_min_kb) splits = num_kb / split_min_kb;
+        if (splits < 1) splits = 1;
     }
     g.kb_per_split = (num_kb + splits - 1) / splits;
     splits = (num_kb + g.kb_per_split - 1) / g.kb_per_split;
     GemmMaps gm;
-    // K-major: rows = M (or N), cols = K, box BK x tile rows.  MN-major: rows = K, cols = M (or N), box 32 mn x BK k-rows.
+    // K-major: rows = M (or N), cols = K, box BK x tile rows.  MN-major: rows = K, cols = M (or N), box tile width x BK k-rows.
     for (int p = 0; p < nprob; p++) {
-        if (int e = amn ? make_map(&gm.a[p], As[p], K, M, lda, BK, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B) : make_map(&gm.a[p], As[p], M, K, lda, BM)) return e;
-        if (int e = bmn ? make_map(&gm.b[p], Bs[p], K, N, ldb, BK, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B) : make_map(&gm.b[p], Bs[p], N, K, ldb, two_cta ? 128 : BN)) return e;
+        if (int e = amn ? make_map_mn(&gm.a[p], As[p], K, M, lda, BM) : make_map(&gm.a[p], As[p], M, K, lda, BM)) return e;
+        if (int e = bmn ? make_map_mn(&gm.b[p], Bs[p], K, N, ldb, BN) : make_map(&gm.b[p], Bs[p], N, K, ldb, BN)) return e;
     }
     for (int p = nprob; p < GEMM_MAXP; p++) { gm.a[p] = gm.a[0]; gm.b[p] = gm.b[0]; }
     const CUtensorMap& ma = gm.a[0];
-    const CUtensorMap& mb = gm.b[0];
     if (splits > 1) {
         if (!accumulate)
             for (int p = 0; p < nprob; p++) { const size_t tot = (size_t)M * N; zero_strided<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cs[p], ldc, M, N); go1_count_launch(1); }
@@ -1431,14 +1113,14 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     const bool timed = g_time_on && cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone;
     if (timed) {
         cudaEventRecord(timing_event(), st); g_time_flop += 2.0 * (double)M * (double)N * (double)K * nprob;
-        g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, two_cta ? 2 : BN, g.colsum ? 1 : 0});
+        g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, BN, g.colsum ? 1 : 0});
     }
     int e;
-    // staged epilogue (BN <= 128 kernels): C blocks through shared memory + TMA store, the ELU' operand through TMA loads
+    // staged epilogue: C blocks leave the accumulator staging by TMA store, the ELU' operand arrives through TMA loads
     static const int use_staged = getenv("GO1_TF32_STAGED") ? atoi(getenv("GO1_TF32_STAGED")) : 1;
     CUtensorMap mc = ma, my = ma;
     g.tma_store = g.tma_aux = 0;
-    if (use_staged && !two_cta && nprob == 1 && BN <= 128 && splits == 1 && !accumulate && N >= 32 && (ldc & 3) == 0 && (((uintptr_t)Cm) & 15) == 0) {
+    if (use_staged && nprob == 1 && splits == 1 && !accumulate && N >= 32 && (ldc & 3) == 0 && (((uintptr_t)Cm) & 15) == 0) {
         if (int e2 = make_map(&mc, Cm, M, N, ldc, 32)) return e2;
         g.tma_store = 1;
         if (g.act == 2 && (g.ldaux & 3) == 0 && (((uintptr_t)g.aux) & 15) == 0) {
@@ -1446,11 +1128,9 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
             g.tma_aux = 1;
         }
     }
-    if (two_cta) e = launch_2cta<6, 4>(ma, mb, g, splits, st);
-    else if (BN == 256) e = launch_persistent<256, 4, false>(gm, mc, my, g, splits, st);
-    else if (BN == 128) e = launch_persistent<128, 4, true>(gm, mc, my, g, splits, st);
-    else if (BN == 64) e = launch_persistent<64, 2, true>(gm, mc, my, g, splits, st);
-    else e = launch_persistent<32, 1, true>(gm, mc, my, g, splits, st);
+    if (BN == 128) e = launch_gemm<128, true>(gm, mc, my, g, splits, st);
+    else if (BN == 64) e = launch_gemm<64, true>(gm, mc, my, g, splits, st);
+    else e = launch_gemm<32, true>(gm, mc, my, g, splits, st);
     if (e) return e;
     if (splits > 1 && (bias || act))
         for (int p = 0; p < nprob; p++) { const size_t tot = (size_t)M * N; bias_act_strided<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cs[p], ldc, bias, M, N, act); go1_count_launch(1); }
@@ -1475,7 +1155,7 @@ extern "C" int go1_gemm_grouped(int transA, int transB, int M, int N, int K, int
     return gemm_tf32_impl(transA, transB, M, N, K, nprob, A, lda, B, ldb, C, ldc, &ep, (cudaStream_t)stream);
 }
 
-// dst[c][r] = src[r][c]  (32x32 smem tiles): brings dgrad/wgrad operands into the K-major form the tcgen05 kernel reads
+// dst[c][r] = src[r][c]  (32x32 smem tiles)
 __global__ void transpose_kernel(const float* __restrict__ src, int lds, float* __restrict__ dst, int ldd, int rows, int cols) {
     __shared__ float t[32][33];
     const int c0 = blockIdx.x * 32, r0 = blockIdx.y * 32;
@@ -1508,7 +1188,7 @@ extern "C" int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int npr
     if (!shape_a && !shape_b) return go1_set_error("go1_mlp_tail_forward: supported tails are 512-256-128-head and 256-128-head");
     TailMaps maps;
     TailArgs g;
-    g.nprob = nprob; g.M = M; g.tiles_per_prob = (M + BM - 1) / BM; g.tiles = g.tiles_per_prob * nprob;
+    g.nprob = nprob; g.M = M; g.tiles_per_prob = (M + TAIL_BM - 1) / TAIL_BM; g.tiles = g.tiles_per_prob * nprob;
     int rows = 0;
     for (int p = 0; p < nprob; p++) {
         const Go1TailProblem& q = probs[p];
@@ -1518,7 +1198,7 @@ extern "C" int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int npr
             ((((uintptr_t)q.x | (uintptr_t)q.W2 | (uintptr_t)q.y2 | (uintptr_t)(N3 > 0 ? (const void*)q.W3 : (const void*)q.W2) |
                (uintptr_t)(N3 > 0 ? (const void*)q.y3 : (const void*)q.y2)) & 15) != 0))
             return go1_set_error("go1_mlp_tail_forward: operands must be 16-byte aligned with row strides that are multiples of 4 floats");
-        if (int e = make_map(&maps.x[p], q.x, M, K1, q.ldx, BM)) return e;
+        if (int e = make_map(&maps.x[p], q.x, M, K1, q.ldx, TAIL_BM)) return e;
         if (int e = make_map(&maps.w2[p], q.W2, N2, K1, K1, N2)) return e;
         if (N3 > 0) { if (int e = make_map(&maps.w3[p], q.W3, N3, N2, N2, N3)) return e; } else maps.w3[p] = maps.w2[p];
         if (int e = make_map(&maps.y2[p], q.y2, M, N2, q.ldy2, 32)) return e;
@@ -1559,7 +1239,7 @@ extern "C" int go1_mlp_tail_backward_grouped(const Go1TailBwdProblem* probs, int
     if (N3 != TB_N3 || N2 != TB_N2) return go1_set_error("go1_mlp_tail_backward: the supported tail is ...-256-128-head");
     TailBwdMaps maps;
     TailBwdArgs g;
-    g.nprob = nprob; g.M = M; g.tiles_per_prob = (M + BM - 1) / BM; g.tiles = g.tiles_per_prob * nprob;
+    g.nprob = nprob; g.M = M; g.tiles_per_prob = (M + TAIL_BM - 1) / TAIL_BM; g.tiles = g.tiles_per_prob * nprob;
     for (int p = 0; p < nprob; p++) {
         const Go1TailBwdProblem& q = probs[p];
         if (!q.dout || !q.Wh || !q.y3 || !q.W3 || !q.y2 || !q.dz3 || !q.dz2 || !q.gb3 || !q.gb2 || q.nh < 1 || q.nh > TAIL_HPW || q.lddout < q.nh)
@@ -1567,21 +1247,19 @@ extern "C" int go1_mlp_tail_backward_grouped(const Go1TailBwdProblem* probs, int
         if ((q.ldy3 & 3) || (q.ldy2 & 3) || (q.lddz3 & 3) || (q.lddz2 & 3) ||
             ((((uintptr_t)q.y3 | (uintptr_t)q.y2 | (uintptr_t)q.W3 | (uintptr_t)q.dz3 | (uintptr_t)q.dz2) & 15) != 0))
             return go1_set_error("go1_mlp_tail_backward: operands must be 16-byte aligned with row strides that are multiples of 4 floats");
-        if (int e = make_map(&maps.w3[p], q.W3, N3, N2, N2, BK, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return e;
+        if (int e = make_map_mn(&maps.w3[p], q.W3, N3, N2, N2, N2)) return e;
         if (int e = make_map(&maps.dz3[p], q.dz3, M, N3, q.lddz3, 32)) return e;
-        if (int e = make_map(&maps.dz2[p], q.dz2, M, N2, q.lddz2, 32)) return e;
         TailBwdProb& d = g.p[p];
-        d.dout = q.dout; d.Wh = q.Wh; d.y3 = q.y3; d.y2 = q.y2; d.gb3 = q.gb3; d.gb2 = q.gb2; d.lddout = q.lddout; d.nh = q.nh; d.ldy3 = q.ldy3; d.ldy2 = q.ldy2;
+        d.dout = q.dout; d.Wh = q.Wh; d.y3 = q.y3; d.y2 = q.y2; d.dz2 = q.dz2; d.lddz2 = q.lddz2; d.gb3 = q.gb3; d.gb2 = q.gb2; d.lddout = q.lddout; d.nh = q.nh; d.ldy3 = q.ldy3; d.ldy2 = q.ldy2;
     }
-    for (int p = nprob; p < TAIL_MAXP; p++) { maps.w3[p] = maps.w3[0]; maps.dz3[p] = maps.dz3[0]; maps.dz2[p] = maps.dz2[0]; g.p[p] = g.p[0]; }
+    for (int p = nprob; p < TAIL_MAXP; p++) { maps.w3[p] = maps.w3[0]; maps.dz3[p] = maps.dz3[0]; g.p[p] = g.p[0]; }
     static bool configured = false;
     if (!configured) {
         cudaError_t e = cudaFuncSetAttribute(mlp_tail_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TB_SMEM);
         if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
         configured = true;
     }
-    static int sms = 0;
-    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
+    const int sms = sm_count();
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     const bool timed = g_time_on && cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone;
     if (timed) {
@@ -1592,7 +1270,7 @@ extern "C" int go1_mlp_tail_backward_grouped(const Go1TailBwdProblem* probs, int
         g_time_recs.push_back({M * nprob, N2, N3, 0, 1, 2, 0, 1, 1004, 1});
     }
     const int grid = g.tiles < sms ? g.tiles : sms;
-    mlp_tail_bwd_kernel<<<grid, 64 + 128 * TAIL_G, TB_SMEM, st>>>(maps, g);
+    mlp_tail_bwd_kernel<<<grid, 32 * NCONS + 128, TB_SMEM, st>>>(maps, g);
     go1_count_launch(1);
     if (timed) cudaEventRecord(timing_event(), st);
     cudaError_t ce = cudaGetLastError();

@@ -1,6 +1,6 @@
-// ppo_kernels.cu — learner-side kernels of go1_gym_learn/ppo_cse for sm_100a:
+// ppo_kernels.cu — learner-side kernels of go1_gym_learn/ppo_cse for sm_90a:
 //   GAE warp-scan (rollout_storage.py:74-88), fp32 CUDA-core GEMM with fused bias/ELU epilogue (the
-//   exact-fp32 path next to the tcgen05 TF32 path in gemm_tf32.cu), ELU backward, column sums, Normal
+//   exact-fp32 path next to the wgmma TF32 path in gemm_tf32.cu), ELU backward, column sums, Normal
 //   sampling/log-prob (actor_critic.py:113-126), PPO loss + gradients (ppo.py:113-152), MSE
 //   (ppo.py:168-186), global grad-norm + clip + Adam (ppo.py:155-158), row gather
 //   (rollout_storage.py:98-137).
@@ -257,7 +257,7 @@ extern "C" int go1_gemm_ex(int transA, int transB, int M, int N, int K, const fl
     const bool fused = ep.nex > 0 || act == 2;
     const int tiles = ((M + 127) / 128) * ((N + 127) / 128);
     int splitk = 1;
-    if (tiles < 148 && K >= 2048 && !fused) { splitk = min((148 * 2 + tiles - 1) / tiles, (K + 255) / 256); if (splitk < 1) splitk = 1; }
+    if (tiles < 132 && K >= 2048 && !fused) { splitk = min((132 * 2 + tiles - 1) / tiles, (K + 255) / 256); if (splitk < 1) splitk = 1; }
     int kchunk = ((K + splitk - 1) / splitk + 7) / 8 * 8;
     splitk = (K + kchunk - 1) / kchunk;
     dim3 grid((N + 127) / 128, (M + 127) / 128, splitk);
@@ -283,7 +283,7 @@ extern "C" int go1_gemm(int transA, int transB, int M, int N, int K, const float
     return go1_gemm_ex(transA, transB, M, N, K, A, lda, B, ldb, Cm, ldc, &ep, impl, stream);
 }
 
-// ELU, branch-free (the same polynomial / ex2 split as the tcgen05 epilogue, gemm_tf32.cu: absolute error ~1e-7)
+// ELU, branch-free (the same polynomial / ex2 split as the wgmma epilogue, gemm_tf32.cu: absolute error ~1e-7)
 __device__ __forceinline__ float elu_fast(float v) {
     float p = fmaf(v, 1.f / 5040.f, 1.f / 720.f);
     p = fmaf(p, v, 1.f / 120.f); p = fmaf(p, v, 1.f / 24.f); p = fmaf(p, v, 1.f / 6.f); p = fmaf(p, v, 0.5f);
@@ -358,7 +358,7 @@ extern "C" int go1_mlp_extra_forward(float* y, int ldy, const float* extra, int 
     if ((o & 3) == 0 && (ldy & 3) == 0 && (((uintptr_t)y) & 15) == 0 && o4 <= 256 && 256 % o4 == 0) {
         const int rpb = 256 / o4;
         int grid = (M + 4 * rpb - 1) / (4 * rpb);
-        if (grid > 148 * 16) grid = 148 * 16;
+        if (grid > 132 * 16) grid = 132 * 16;
         extra_fwd4_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(y, ldy, extra, ldex, w_extra, ldw, M, o4, E, act, 4 * rpb); go1_count_launch(1);
         return cuda_rc("go1_mlp_extra_forward");
     }
@@ -452,7 +452,7 @@ extern "C" int go1_skinny_wgrad_ex(const float* dz, int lddz, const float* x, in
     }
     if ((K & 3) == 0 && (ldx & 3) == 0 && (((uintptr_t)x) & 15) == 0) {
         const int kb = (K + 127) / 128;
-        int rpb4 = (M * kb + 147) / 148;                 // about one block per SM (more blocks measured slower: the per-block reduction and atomics dominate)
+        int rpb4 = (M * kb + 131) / 132;                 // about one block per SM (the per-block reduction and atomics dominate with more)
         rpb4 = (rpb4 + 7) / 8 * 8; if (rpb4 < 8) rpb4 = 8;
         dim3 grid4(kb, (M + rpb4 - 1) / rpb4);
         if (o <= 2) skinny_wgrad4_kernel<2><<<grid4, 256, 0, st>>>(dz, lddz, x, ldx, gW, ldg, gb, M, o, K, rpb4);
@@ -510,7 +510,7 @@ extern "C" int go1_copy_segments(const Go1CopySeg* segs, int n, void* stream) {
         if (w > work) work = w;
     }
     long long blocks = (work + 255) / 256;
-    if (blocks > 148 * 8) blocks = 148 * 8;
+    if (blocks > 132 * 8) blocks = 132 * 8;
     if (blocks < 1) blocks = 1;
     copy_segments_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(a); go1_count_launch(1);
     return cuda_rc("go1_copy_segments");
@@ -976,7 +976,7 @@ extern "C" int go1_skinny_dgrad_ex(const float* dz, int lddz, const float* W, in
                      ((((uintptr_t)W) | ((uintptr_t)dprev) | ((uintptr_t)(y_prev ? y_prev : W))) & 15) == 0;
     if (vec) {
         const int cb = (n + 127) / 128;
-        int rpb = (M * cb + 2 * 148 - 1) / (2 * 148);           // about two blocks per SM (four measured slower)
+        int rpb = (M * cb + 2 * 132 - 1) / (2 * 132);           // about two blocks per SM
         rpb = (rpb + 7) / 8 * 8; if (rpb < 8) rpb = 8;
         dim3 grid(cb, (M + rpb - 1) / rpb);
         if (o <= 2) skinny_dgrad4_kernel<2><<<grid, 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, colsum, M, o, n, rpb);
@@ -1036,7 +1036,7 @@ extern "C" int go1_skinny_forward(const float* x, int ldx, const float* W, int l
         return go1_set_error("go1_skinny_forward: bad arguments (o <= 16, K % 4 == 0, x 16-byte aligned rows)");
     const int rows_per_block = 32;
     int grid = (M + rows_per_block - 1) / rows_per_block;
-    if (grid > 148 * 8) grid = 148 * 8;
+    if (grid > 132 * 8) grid = 132 * 8;
     skinny_forward_kernel<<<grid, 256, (size_t)(o * K + 16) * 4, (cudaStream_t)stream>>>(x, ldx, W, ldw, b, out, ldo, M, o, K); go1_count_launch(1);
     return cuda_rc("go1_skinny_forward");
 }

@@ -155,7 +155,7 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise Go1Error(f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                       f"(nvcc, sm_100a). There is no CPU fallback.")
+                       f"(nvcc, sm_90a). There is no CPU fallback.")
     L = C.CDLL(LIB_PATH)
     L.go1_last_error.restype = C.c_char_p
     vp, ip, i64 = C.c_void_p, C.c_int, C.c_int64
@@ -183,7 +183,6 @@ def lib():
         "go1_mlp_tail_backward_grouped": ([C.POINTER(Go1TailBwdProblem), ip, ip, ip, ip, vp], ip),
         "go1_mlp_tail_forward_grouped": ([C.POINTER(Go1TailProblem), ip, ip, ip, ip, ip, vp], ip),
         "go1_mlp_tail_forward": ([vp, ip, ip, ip, vp, vp, ip, vp, ip, vp, vp, ip, vp, ip, vp, vp, ip, vp, ip, vp], ip),
-        "go1_gemm_tf32_set_wide": ([ip], None),
         "go1_transpose": ([vp, ip, vp, ip, ip, ip, vp], ip),
         "go1_elu_backward": ([vp, ip, vp, ip, vp, ip, ip, ip, vp], ip),
         "go1_mlp_extra_forward": ([vp, ip, vp, ip, vp, ip, ip, ip, ip, ip, vp], ip),

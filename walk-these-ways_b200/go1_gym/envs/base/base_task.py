@@ -9,7 +9,7 @@ class BaseTask:
         self.sim_device = sim_device
         self.headless = headless
         if not str(sim_device).startswith("cuda"):
-            raise RuntimeError("go1_gym (B200 build) runs on CUDA devices only: there is no CPU simulator")
+            raise RuntimeError("go1_gym (CUDA build) runs on CUDA devices only: there is no CPU simulator")
         self.device = sim_device
         self.num_obs = cfg.env.num_observations
         self.num_privileged_obs = cfg.env.num_privileged_obs

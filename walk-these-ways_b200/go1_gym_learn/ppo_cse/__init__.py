@@ -1,4 +1,4 @@
-"""go1_gym_learn.ppo_cse — Runner of the reference (go1_gym_learn/ppo_cse/__init__.py:44-308) on the B200 kernels.
+"""go1_gym_learn.ppo_cse — Runner of the reference (go1_gym_learn/ppo_cse/__init__.py:44-308) on the CUDA kernels of this repository.
 
 `Runner(env, device).learn(num_learning_iterations, init_at_random_ep_len, eval_freq)` keeps the reference's
 loop structure (24-step rollout -> compute_returns -> update -> logging/checkpoints with the same file names),

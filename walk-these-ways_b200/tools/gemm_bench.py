@@ -25,8 +25,6 @@ def main():
     if only:
         SHAPES = [sh for sh in SHAPES if sh[3] in only.split(";")]
     impls = (1,) if os.environ.get("GEMM_BENCH_TC_ONLY") else (0, 1)
-    if os.environ.get("GEMM_BENCH_WIDE"):
-        L.go1_gemm_tf32_set_wide(1)
     flush = torch.empty(256 * 1024 * 1024 // 4, device="cuda")
     print(f"{'shape':>24s} {'note':>26s} {'impl0 us':>10s} {'TF/s':>7s} {'impl1 us':>10s} {'TF/s':>7s}")
     for M, N, K, note in SHAPES:
