@@ -283,6 +283,16 @@ int go1_ppo_gae(const float* rewards, const uint8_t* dones, const float* values,
 int go1_ppo_normalize_advantages(float* advantages, const double* stats, int64_t global_count, int64_t local_count,
                                  void* stream);
 
+/* Hidden-layer activation of ActorCritic's MLPs (AC_Args.activation; the reference's get_activation, actor_critic.py:149-166, maps
+ * `crelu` to nn.ReLU as well).  ELU is 0: zero-initialised structs and callers that predate the other kinds mean ELU(alpha = 1).
+ * selu: lambda = 1.0507009873554805, alpha = 1.6732632423543772; lrelu: slope 0.01 (nn.LeakyReLU() default).  All backward kernels
+ * compute the derivative from the SAVED OUTPUT y = f(v): elu y > 0 ? 1 : y + 1; selu y > 0 ? lambda : y + lambda alpha; relu y > 0 ? 1 : 0;
+ * lrelu y > 0 ? 1 : 0.01; tanh 1 - y^2; sigmoid y (1 - y).  An unknown kind makes the entry point return non-zero before any launch. */
+typedef enum Go1Activation { GO1_ACT_ELU = 0, GO1_ACT_SELU, GO1_ACT_RELU, GO1_ACT_LRELU, GO1_ACT_TANH, GO1_ACT_SIGMOID } Go1Activation;
+/* `act` argument of the entry points that take a bare int: mode (0 none, 1 activation, 2 times its derivative) in bits 0..7, the
+ * Go1Activation in bits 8.. (so the plain modes 0 / 1 / 2 keep meaning ELU). */
+#define GO1_ACT(kind, mode) (((kind) << 8) | (mode))
+
 /* GEMM primitive behind every nn.Linear of ActorCritic (actor_critic.py:38-77; replaces the cuBLAS sgemm
  * calls issued by F.linear and its autograd): C[M][N] (+)= opA(A) opB(B) (+ bias[n]), optional ELU.
  *   transA == 0: A is row-major [M][K] (row stride lda);  transA == 1: A is [K][M]
@@ -292,15 +302,15 @@ int go1_ppo_normalize_advantages(float* advantages, const double* stats, int64_t
  * wgrad    dW = dz^T x        :  go1_gemm(1,0, N,K,M, dz,lddz, x,ldx, dW,lddw, NULL,0, acc, impl)
  * Row strides let a layer read/write column slices of wider buffers, so cat(obs_history, latent)
  * (actor_critic.py:115) is never materialised.  accumulate: add into C instead of overwriting
- * (bias/act are applied after the accumulation).  act: 0 none, 1 ELU(alpha=1).
+ * (bias/act are applied after the accumulation).  act: 0 none, 1 ELU(alpha=1), GO1_ACT(kind, 1) another activation.
  * impl: 0 = fp32 CUDA cores (exact-fp32 path), 1 = wgmma TF32 tensor cores with fp32 accumulation. */
 int go1_gemm(int transA, int transB, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
              float* C, int ldc, const float* bias, int act, int accumulate, int impl, void* stream);
 /* Same product with the full fused epilogue, applied in this order to each output element v = sum_k a*b:
  *   v += C_old (accumulate);  v += sum_e extra[m][e] * w_extra[n][e]  (num_extra <= 4: the 2 trailing input columns of
  *   the actor/critic first layer, i.e. cat(obs_history, latent) without the cat);  v += bias[n];
- *   act 1: v = ELU(v);  act 2: v *= ELU'(z) computed from the saved activation dact_y[m][n] (the autograd of nn.ELU fused
- *   into the dgrad GEMM). */
+ *   act 1: v = f(v);  act 2: v *= f'(z) computed from the saved activation dact_y[m][n] (the autograd of the activation module
+ *   fused into the dgrad GEMM);  f = the Go1Activation act_kind (0 = ELU). */
 typedef struct Go1GemmEpilogue {
     const float* bias; int32_t act, accumulate;
     const float* extra; int32_t ld_extra; const float* w_extra; int32_t ld_w_extra, num_extra;
@@ -314,6 +324,7 @@ typedef struct Go1GemmEpilogue {
      * d_extra[m][t] += sum_n C[m][n] bwd_w_extra[n][t]  (d_extra may be NULL; g_w_extra may be NULL when d_extra is given) */
     const float* bwd_extra; const float* bwd_w_extra; float* g_w_extra; float* d_extra;
     int32_t ld_bwd_extra, ld_bwd_w_extra, ld_g_w_extra, ld_d_extra, num_bwd_extra;
+    int32_t act_kind;    /* Go1Activation behind act 1 / 2 (0 = ELU) */
 } Go1GemmEpilogue;
 int go1_gemm_ex(int transA, int transB, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
                 float* C, int ldc, const Go1GemmEpilogue* ep, int impl, void* stream);
@@ -329,11 +340,12 @@ int go1_gemm_grouped(int transA, int transB, int M, int N, int K, int nprob, con
 int go1_mlp_tail_forward(const float* x, int ldx, int M, int K1, const float* W2, const float* b2, int N2, float* y2, int ldy2,
                          const float* W3, const float* b3, int N3, float* y3, int ldy3, const float* Wh, const float* bh, int nh,
                          float* out, int ldout, void* stream);
-/* The same for up to two problems of equal shape in ONE grid (the actor and critic bodies: 2 x 192 row blocks fill the 148 SMs in 3 even
+/* The same (ELU, or the problems' act_kind) for up to two problems of equal shape in ONE grid (the actor and critic bodies: 2 x 192 row blocks fill the 148 SMs in 3 even
  * rounds instead of 2 x 2 ragged ones).  nh <= 12 per problem. */
 typedef struct Go1TailProblem {
     const float* x; int32_t ldx; const float* W2; const float* b2; float* y2; int32_t ldy2;
     const float* W3; const float* b3; float* y3; int32_t ldy3; const float* Wh; const float* bh; int32_t nh; float* out; int32_t ldout;
+    int32_t act_kind;    /* Go1Activation in place of ELU (0 = ELU); the problems of one launch share it */
 } Go1TailProblem;
 int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int nprob, int M, int K1, int N2, int N3, void* stream);
 /* Backward of the same bodies, first half, for up to two problems in one grid (nn.Linear / nn.ELU autograd of actor_critic.py:38-77):
@@ -343,6 +355,7 @@ int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int nprob, int M, 
 typedef struct Go1TailBwdProblem {
     const float* dout; int32_t lddout, nh; const float* Wh; const float* y3; int32_t ldy3; const float* W3; const float* y2; int32_t ldy2;
     float* dz3; int32_t lddz3; float* dz2; int32_t lddz2; float* gb3; float* gb2;
+    int32_t act_kind;    /* Go1Activation whose derivative stands in for ELU' (0 = ELU); the problems of one launch share it */
 } Go1TailBwdProblem;
 int go1_mlp_tail_backward_grouped(const Go1TailBwdProblem* probs, int nprob, int M, int N3, int N2, void* stream);
 
@@ -356,8 +369,10 @@ void go1_kernel_launch_add(long long n);
 int go1_transpose(const float* src, int lds, float* dst, int ldd, int rows, int cols, void* stream);
 /* dz = dy * ELU'(z) computed from the saved layer output y (autograd of nn.ELU). dz may alias dy. */
 int go1_elu_backward(const float* y, int ldy, const float* dy, int lddy, float* dz, int lddz, int M, int N, void* stream);
+/* The same for any Go1Activation: dz = dy * f'(z) from the saved output y (go1_elu_backward is kind GO1_ACT_ELU of this kernel). */
+int go1_act_backward(const float* y, int ldy, const float* dy, int lddy, float* dz, int lddz, int M, int N, int kind, void* stream);
 /* Finishes a first layer whose trailing-input term was left out of the product: y = act(y + extra[m][:E] . w_extra[n][:E])
- * in place (E <= 4; act 0/1). */
+ * in place (E <= 4; act 0 / 1 / GO1_ACT(kind, 1)). */
 int go1_mlp_extra_forward(float* y, int ldy, const float* extra, int ldex, const float* w_extra, int ldw, int M, int o, int E, int act,
                           void* stream);
 /* Backward of the E (<= 4) trailing input columns of a first layer (the `latent` / privileged columns of
@@ -376,6 +391,9 @@ int go1_skinny_dgrad(const float* dz, int lddz, const float* W, int ldw, const f
  * the bias gradient of the layer below (nn.Linear backward), reduced while dprev is produced. */
 int go1_skinny_dgrad_ex(const float* dz, int lddz, const float* W, int ldw, const float* y_prev, int ldy, float* dprev, int lddp,
                         float* colsum, int M, int o, int n, void* stream);
+/* go1_skinny_dgrad_ex with the derivative of any Go1Activation in place of ELU'. */
+int go1_skinny_dgrad_act(const float* dz, int lddz, const float* W, int ldw, const float* y_prev, int ldy, float* dprev, int lddp,
+                         float* colsum, int M, int o, int n, int kind, void* stream);
 /* go1_skinny_wgrad + the layer's bias gradient gb[j] (+)= sum_m dz[m][j] (may be NULL; needs K % 4 == 0 and 16-byte aligned x rows). */
 int go1_skinny_wgrad_ex(const float* dz, int lddz, const float* x, int ldx, float* gW, int ldg, float* gb, int M, int o, int K, int accumulate, void* stream);
 /* wgrad of a narrow (o <= 16) output layer (the 12 / 2 / 1-wide heads): gW[j][k] (+)= sum_m dz[m][j] x[m][k]. */

@@ -1,6 +1,6 @@
 // gemm_tf32.cu — hand-written wgmma TF32 GEMM for sm_90a (the dense layers of ppo_cse's ActorCritic).
 //
-//   C[M][N] (+)= A[M][K] * B[N][K]^T (+ bias[n]) (ELU)          fp32 in HBM, TF32 multiply, fp32 accumulate
+//   C[M][N] (+)= A[M][K] * B[N][K]^T (+ bias[n]) (activation)   fp32 in HBM, TF32 multiply, fp32 accumulate
 //
 // The forward products read both operands K-major (A = activations row-major, B = torch.nn.Linear weight [out][in]).
 // dgrad (B = W as [K][N]) and wgrad (A = dz as [K][M], B = activations as [K][N]) have MN-major operands, and TF32 wgmma
@@ -10,7 +10,7 @@
 // Structure (persistent CTAs, one per SM, 384 threads, walking 128 x BN output tiles):
 //   warps 0-7   two consumer warpgroups, 64 rows x BN columns each: wgmma.mma_async m64nBNk8 (4 per k-block) with the accumulator
 //               in registers, then the epilogue: accumulator -> swizzled shared memory -> one 32 x 32 block per warp at a time,
-//               a row per lane -> bias / ELU / ELU' / column sums / trailing-input terms -> the same block -> one TMA store
+//               a row per lane -> bias / activation / its derivative / column sums / trailing-input terms -> the same block -> one TMA store
 //               (staged epilogue), red.global.add.v4 when split-K partitions the reduction
 //   warp 8      TMA producer: cp.async.bulk.tensor 2D loads of the A and B boxes of a k-block into a ring of 3-8 stages guarded by
 //               full / empty mbarriers; it runs ahead into the next tile while the consumers are in their epilogue
@@ -24,6 +24,7 @@
 #include <stdlib.h>
 #include "../../include/go1_b200.h"
 #include "wgmma_tf32.cuh"
+#include "activation.cuh"
 
 extern int go1_set_error(const char* m);
 void go1_count_launch(int n);
@@ -95,22 +96,14 @@ __device__ __forceinline__ void store_fragment(const float (&acc)[4 * NJ], uint8
     }
 }
 
-// ELU(v) = v > 0 ? v : expm1(v), branch-free: a degree-7 Taylor polynomial on (-0.35, 0] (truncation error < 2e-8 relative) and
-// ex2.approx(v log2 e) - 1 below it (absolute error ~1e-7 on a value >= 0.29); 13 instructions instead of expm1f's ~28 plus a
-// divergent branch.  The result feeds a TF32 product (relative operand rounding 5e-4) and ELU' = y + 1 in the backward pass.
-__device__ __forceinline__ float elu_fast(float v) {
-    float p = fmaf(v, 1.f / 5040.f, 1.f / 720.f);
-    p = fmaf(p, v, 1.f / 120.f); p = fmaf(p, v, 1.f / 24.f); p = fmaf(p, v, 1.f / 6.f); p = fmaf(p, v, 0.5f);
-    p = fmaf(p * v, v, v);
-    float e;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(v * 1.4426950408889634f));
-    const float n = v > -0.35f ? p : e - 1.0f;
-    return v > 0.f ? v : n;
-}
+// The activations are act_fast / act_deriv of activation.cuh: their results feed TF32 products (relative operand rounding 5e-4) and the
+// derivative-from-output forms of the backward pass.  The kind is a warp-uniform kernel argument; GO1_ACT_SWITCH dispatches on it around
+// each unrolled loop.  The kernels whose register budget is full (the persistent GEMM, the fused tails) exist twice: ANYKIND = false
+// is the ELU-only code (the switch folds away), ANYKIND = true carries the switch and serves the other kinds.
 
 struct GemmArgs {
     float* C; const float* bias;
-    int M, N, K, ldc, act, accumulate, kb_per_split;
+    int M, N, K, ldc, act, kind, accumulate, kb_per_split;      // kind: Go1Activation behind act 1 / 2
     const float* ex; const float* wex; const float* aux;      // fused epilogue operands (see Go1GemmEpilogue)
     int ldex, ldwex, nex, ldaux;
     int lead;                // > 0: extra columns + activation only for output columns < lead
@@ -118,7 +111,7 @@ struct GemmArgs {
     float* colsum;           // optional [N]: += column sums of the values written (bias gradient fused into the dgrad epilogue)
     const float* bx; const float* bwx; float* gwx; float* dx;     // fused trailing-input backward (see Go1GemmEpilogue)
     int ldbx, ldbwx, ldgwx, lddx, nbx;
-    int tma_store, tma_aux;  // staged epilogue (persistent kernel, STAGED): C blocks leave / ELU' operand blocks arrive through shared memory by TMA
+    int tma_store, tma_aux;  // staged epilogue (persistent kernel, STAGED): C blocks leave / derivative operand blocks arrive through shared memory by TMA
     // grouped launch (persistent kernel): nprob problems of the same shape and operand strides in one grid; tile t belongs to problem
     // t / tiles_per_prob, whose operands are maps.a/b[p] and whose output is Cg[p] (no per-problem epilogue operands: split-K wgrads)
     float* Cg[4]; int nprob, tiles_per_prob;
@@ -132,16 +125,47 @@ struct GemmMaps { CUtensorMap a[GEMM_MAXP], b[GEMM_MAXP]; };
 struct EpiStage {
     uint8_t* out;            // 4 KB, 1024-byte aligned: the block the values came from, or nullptr: direct global stores
     const CUtensorMap* mapC;
-    const uint8_t* aux;      // 4 KB block of the ELU' operand, fetched by TMA and already waited for, or nullptr
+    const uint8_t* aux;      // 4 KB block of the derivative operand (the saved activation), fetched by TMA and already waited for, or nullptr
 };
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                  ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
 }
 
+// act == 2 of one chunk: v[j] *= f'(z) from the saved activation, wherever this chunk's 32 values of it are (see epilogue_chunk)
+template <typename D>
+__device__ __forceinline__ void epilogue_dact(const D dact, const GemmArgs& g, float (&v)[32], const int row, const int col0, const int ncols, const int lane,
+                                              const float4 (&ypre)[8], const bool have_pre, const EpiStage& es) {
+    const float* arow = g.aux + (size_t)row * g.ldaux + col0;
+    if (es.aux) {          // the operand block sits in shared memory (TMA, 128B swizzle: 16-byte chunk j of row l at (j ^ (l & 7)))
+        const uint8_t* srow = es.aux + lane * 128;
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            const float4 y = *reinterpret_cast<const float4*>(srow + ((j ^ (lane & 7)) << 4));
+            v[4 * j] *= dact(y.x); v[4 * j + 1] *= dact(y.y); v[4 * j + 2] *= dact(y.z); v[4 * j + 3] *= dact(y.w);
+        }
+    } else if (have_pre) { // the operand was fetched before the accumulator was ready (epilogue_prefetch)
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            const float4 y = ypre[j];
+            v[4 * j] *= dact(y.x); v[4 * j + 1] *= dact(y.y); v[4 * j + 2] *= dact(y.z); v[4 * j + 3] *= dact(y.w);
+        }
+    } else if (ncols == 32 && (g.ldaux & 3) == 0 && ((((uintptr_t)g.aux) & 15) == 0) && ((col0 & 3) == 0)) {
+#pragma unroll
+        for (int j = 0; j < 8; j++) {
+            const float4 y = __ldg(reinterpret_cast<const float4*>(arow) + j);
+            v[4 * j] *= dact(y.x); v[4 * j + 1] *= dact(y.y); v[4 * j + 2] *= dact(y.z); v[4 * j + 3] *= dact(y.w);
+        }
+    } else {
+#pragma unroll
+        for (int j = 0; j < 32; j++) if (j < ncols) v[j] *= dact(__ldg(arow + j));
+    }
+}
+
 // Epilogue of one 32-column chunk held in registers (thread = output row, r[j] = column col0 + j).  Called by all 32 lanes
 // of an epilogue warp (the per-column operands -- bias, extra-input weights -- are loaded once per lane and broadcast
 // with shuffles instead of 32 x per-thread global loads, which made the rank-2 term the slowest part of the kernel).
+template <bool ANYKIND>
 __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const Cbase, uint32_t (&r)[32], const int row, const int col0, const bool split, const int lane,
                                                const float4 (&ypre)[8], const bool have_pre, const EpiStage& es) {
     if (col0 >= g.N) return;                                    // warp-uniform
@@ -203,39 +227,16 @@ __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const C
 #pragma unroll
         for (int j = 0; j < 32; j++) v[j] += __shfl_sync(0xffffffffu, bl, j);
     }
+    const int kind = ANYKIND ? g.kind : (int)GO1_ACT_ELU;
     if (row_ok) {
     if (g.act == 1) {
-        const int nlead = g.lead <= 0 ? 32 : max(0, min(32, g.lead - col0));      // leading columns of this chunk that get the ELU
-#pragma unroll
-        for (int j = 0; j < 32; j++) if (j < nlead) v[j] = elu_fast(v[j]);
-    } else if (g.act == 2) {   // multiply by ELU'(z) from the saved activation y: 1 if y > 0 else y + 1
-        const float* arow = g.aux + (size_t)row * g.ldaux + col0;
-        if (es.aux) {          // the operand block sits in shared memory (TMA, 128B swizzle: 16-byte chunk j of row l at (j ^ (l & 7)))
-            const uint8_t* srow = es.aux + lane * 128;
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const float4 y = *reinterpret_cast<const float4*>(srow + ((j ^ (lane & 7)) << 4));
-                v[4 * j] *= (y.x > 0.f ? 1.0f : y.x + 1.0f); v[4 * j + 1] *= (y.y > 0.f ? 1.0f : y.y + 1.0f);
-                v[4 * j + 2] *= (y.z > 0.f ? 1.0f : y.z + 1.0f); v[4 * j + 3] *= (y.w > 0.f ? 1.0f : y.w + 1.0f);
-            }
-        } else if (have_pre) { // the operand was fetched before the accumulator was ready (epilogue_prefetch)
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const float4 y = ypre[j];
-                v[4 * j] *= (y.x > 0.f ? 1.0f : y.x + 1.0f); v[4 * j + 1] *= (y.y > 0.f ? 1.0f : y.y + 1.0f);
-                v[4 * j + 2] *= (y.z > 0.f ? 1.0f : y.z + 1.0f); v[4 * j + 3] *= (y.w > 0.f ? 1.0f : y.w + 1.0f);
-            }
-        } else if (ncols == 32 && (g.ldaux & 3) == 0 && ((((uintptr_t)g.aux) & 15) == 0) && ((col0 & 3) == 0)) {
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                const float4 y = __ldg(reinterpret_cast<const float4*>(arow) + j);
-                v[4 * j] *= (y.x > 0.f ? 1.0f : y.x + 1.0f); v[4 * j + 1] *= (y.y > 0.f ? 1.0f : y.y + 1.0f);
-                v[4 * j + 2] *= (y.z > 0.f ? 1.0f : y.z + 1.0f); v[4 * j + 3] *= (y.w > 0.f ? 1.0f : y.w + 1.0f);
-            }
-        } else {
-#pragma unroll
-            for (int j = 0; j < 32; j++) if (j < ncols) { const float y = __ldg(arow + j); v[j] *= (y > 0.f ? 1.0f : y + 1.0f); }
-        }
+        const int nlead = g.lead <= 0 ? 32 : max(0, min(32, g.lead - col0));      // leading columns of this chunk that get the activation
+        GO1_ACT_SWITCH(kind, KD,
+            _Pragma("unroll")
+            for (int j = 0; j < 32; j++) if (j < nlead) v[j] = act_fast<KD>(v[j]);)
+    } else if (g.act == 2) {   // multiply by f'(z) from the saved activation y (ELU: 1 if y > 0 else y + 1)
+        if (ANYKIND) epilogue_dact(act_deriv_coefficients(kind), g, v, row, col0, ncols, lane, ypre, have_pre, es);
+        else epilogue_dact([](float y) { return act_deriv<GO1_ACT_ELU>(y); }, g, v, row, col0, ncols, lane, ypre, have_pre, es);
     }
     }
     if (g.colsum) {         // warp-uniform.  Column sums over the warp's 32 rows by a transpose-reduce: 31 shuffles for 32 columns
@@ -309,7 +310,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const C
     }
 }
 
-// ELU' operand of one 32-column chunk (act == 2), fetched into registers BEFORE the wait on the accumulator so that the HBM / L2
+// derivative operand (the saved activation) of one 32-column chunk (act == 2), fetched into registers BEFORE the wait on the accumulator so that the HBM / L2
 // latency of these row-per-lane loads overlaps the main loop of the tile.  Warp-uniform result; rows beyond M read row 0 (ignored).
 __device__ __forceinline__ bool epilogue_prefetch(const GemmArgs& g, const int row, const int col0, const bool split, float4 (&ypre)[8]) {
     if (g.act != 2 || split || col0 + 32 > g.N || (g.ldaux & 3) != 0 || ((((uintptr_t)g.aux) & 15) != 0) || (col0 & 3) != 0) return false;
@@ -321,12 +322,12 @@ __device__ __forceinline__ bool epilogue_prefetch(const GemmArgs& g, const int r
 
 // ---------------------------------------------------------------------------------------------------------------
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles t = blockIdx.x + i * gridDim.x (n fastest, so the CTAs of
-// one wave share A tiles through L2).  Shared memory: [ring: stages x (A | B)][X: 64 KB][ELU' operand staging 8 x 4 KB][barriers].
+// one wave share A tiles through L2).  Shared memory: [ring: stages x (A | B)][X: 64 KB][derivative operand staging 8 x 4 KB][barriers].
 // X serves the main loop as the double-buffered transposed tiles of MN-major operands (A 2 x 16 KB, B 2 x 16 KB) and the epilogue
 // as the accumulator / output staging (32 KB per warpgroup).
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int X_BYTES = 65536;
-template <int BN, bool STAGED>
+template <int BN, bool STAGED, bool ANYKIND>
 __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __grid_constant__ GemmMaps gm,
                                                                       const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
                                                                       const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
@@ -401,7 +402,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
     uint8_t* xwg = xreg + wgi * (X_BYTES / 2);          // this warpgroup's accumulator staging: [chunk][64 rows][128 B]
     uint8_t* my_aux = stage_aux + warp * 4096;
     uint64_t* my_bar = &aux_bar[warp];
-    // ELU' operand blocks run one chunk ahead of the epilogue: cursor (pt, pc) = the next chunk of this warp whose block has not been requested yet
+    // derivative operand blocks run one chunk ahead of the epilogue: cursor (pt, pc) = the next chunk of this warp whose block has not been requested yet
     int pt = blockIdx.x, pc = grp - G;
     auto next_chunk = [&]() -> bool {
         for (;;) {
@@ -476,7 +477,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
             EpiStage es;
             es.out = st_out ? blk : nullptr; es.mapC = &mapC; es.aux = st_aux ? my_aux : nullptr;
             if (st_aux) { mbar_wait(my_bar, aux_phase); aux_phase ^= 1; }
-            epilogue_chunk(g, Cbase, r, row, n0 + 32 * c, split, lane, ypre, have_pre && c == grp, es);
+            epilogue_chunk<ANYKIND>(g, Cbase, r, row, n0 + 32 * c, split, lane, ypre, have_pre && c == grp, es);
             if (st_aux) { __syncwarp(); request_aux(); }             // every lane has read the operand block: fetch the next one into it
         }
     }
@@ -541,17 +542,17 @@ __global__ void zero_strided(float* C, int ldc, int M, int N) {
     if (i >= (size_t)M * N) return;
     C[(i / N) * ldc + (i % N)] = 0.f;
 }
-__global__ void bias_act_strided(float* C, int ldc, const float* bias, int M, int N, int act) {
+__global__ void bias_act_strided(float* C, int ldc, const float* bias, int M, int N, int act, int kind) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)M * N) return;
     float* c = C + (i / N) * ldc + (i % N);
     float v = *c;
     if (bias) v += bias[i % N];
-    if (act == 1) v = v > 0.f ? v : expm1f(v);
+    if (act == 1) { GO1_ACT_SWITCH(kind, KD, v = act_exact<KD>(v);) }
     *c = v;
 }
 
-template <int BN, bool STAGED>
+template <int BN, bool STAGED, bool ANYKIND>
 int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st) {
     constexpr int STAGE_BYTES = (BM + BN) * BK * 4;
     const size_t staging = X_BYTES + ((STAGED && g.tma_aux) ? (size_t)NCONS * 4096 : 0);
@@ -563,7 +564,7 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
     const size_t smem = (size_t)stages * STAGE_BYTES + fixed;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tf32_wgmma<BN, STAGED>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget);
+        cudaError_t e = cudaFuncSetAttribute(gemm_tf32_wgmma<BN, STAGED, ANYKIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget);
         if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
         configured = true;
     }
@@ -572,19 +573,20 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
     const int total = g.tiles_per_prob * (g.nprob > 1 ? g.nprob : 1);
     const int sms = sm_count();
     const int grid = total < sms ? total : sms;          // one CTA per SM (the ring and the staging fill its shared memory)
-    gemm_tf32_wgmma<BN, STAGED><<<grid, 32 * NCONS + 128, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages);
+    gemm_tf32_wgmma<BN, STAGED, ANYKIND><<<grid, 32 * NCONS + 128, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages);
     go1_count_launch(1);
     return 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Fused MLP tail, forward: the layers behind a first layer of ActorCritic's MLPs (actor_critic.py:38-77) in ONE launch,
-//     y2 = ELU(x W2^T + b2)   [M][N2]        x = the first layer's activated output, K1 wide (a column slice of the fused first-layer product)
-//     y3 = ELU(y2 W3^T + b3)  [M][N3]        (N3 = 0: two-layer tail, the head reads y2)
+//     y2 = f(x W2^T + b2)     [M][N2]        x = the first layer's activated output, K1 wide (a column slice of the fused first-layer product)
+//     y3 = f(y2 W3^T + b3)    [M][N3]        (N3 = 0: two-layer tail, the head reads y2)
 //     out = y_last Wh^T + bh  [M][nh]        nh <= 12 (12 action means / 1 value / 2 latents): CUDA cores, from registers
+// (f = the launch's Go1Activation, ELU by default)
 // for up to two problems of the same shape (actor and critic bodies) in one grid.  One CTA (384 threads) owns a 64-row block:
 //   warps 0-7   two consumer warpgroups; warpgroup g computes columns [g N2 / 2, (g + 1) N2 / 2) of y2 and [g N3 / 2, (g + 1) N3 / 2) of y3
-//               for all 64 rows (wgmma, accumulators in registers).  y2 = ELU(acc + b2) goes from the registers to shared memory once,
+//               for all 64 rows (wgmma, accumulators in registers).  y2 = f(acc + b2) goes from the registers to shared memory once,
 //               K-major and 128B-swizzled, and from there BOTH to the tensor core (A operand of product 2) and to global memory (one TMA
 //               store per 32 x 32 block: the backward pass needs y2); y3 is stored from registers; the head's partial dot products
 //               are taken on the accumulator fragments, reduced over the four lanes that share a row, and the two warpgroups' halves
@@ -594,7 +596,7 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int TAIL_MAXP = 2, TAIL_HPW = 12, TAIL_BM = 64;
 struct TailProb { const float* b2; const float* b3; const float* Wh; const float* bh; float* y3; float* out; int ldy3, ldout, nh, wh_row0; };
-struct TailArgs { TailProb p[TAIL_MAXP]; int nprob, M, tiles_per_prob, tiles; };
+struct TailArgs { TailProb p[TAIL_MAXP]; int nprob, M, tiles_per_prob, tiles, kind; };
 struct TailMaps { CUtensorMap x[TAIL_MAXP], w2[TAIL_MAXP], w3[TAIL_MAXP], y2[TAIL_MAXP]; };
 
 template <int K1, int N2, int N3>
@@ -630,8 +632,9 @@ __device__ __forceinline__ void head_partial(const float (&v)[4 * NJ], const flo
     }
 }
 
-template <int K1, int N2, int N3>
+template <int K1, int N2, int N3, bool ANYKIND>
 __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_kernel(const __grid_constant__ TailMaps maps, const TailArgs g) {
+    const int kind = ANYKIND ? g.kind : (int)GO1_ACT_ELU;
     using L = TailSmem<K1, N2, N3>;
     constexpr int S1 = L::S1, S2 = (L::S2 > 0 ? L::S2 : 1), KB1 = L::KB1, KB2 = L::KB2, STAGE1 = L::STAGE1, STAGE2 = L::STAGE2, NL = L::NL;
     constexpr int NH2 = N2 / 2, NH3 = (N3 > 0 ? N3 : 64) / 2;      // columns per warpgroup
@@ -730,12 +733,14 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_kernel(const
             wg::wait<0>();
             if (lane == 0) mbar_arrive(&empty1[prev]);
             const float* b2 = s_b2 + p * N2;
-#pragma unroll
-            for (int j = 0; j < NH2 / 8; j++) {
-                const float2 bb = *reinterpret_cast<const float2*>(b2 + wgi * NH2 + 8 * j + 2 * (lane & 3));
-                acc[4 * j] = ok0 ? elu_fast(acc[4 * j] + bb.x) : 0.f; acc[4 * j + 1] = ok0 ? elu_fast(acc[4 * j + 1] + bb.y) : 0.f;
-                acc[4 * j + 2] = ok1 ? elu_fast(acc[4 * j + 2] + bb.x) : 0.f; acc[4 * j + 3] = ok1 ? elu_fast(acc[4 * j + 3] + bb.y) : 0.f;
-            }
+            // rows beyond M stay 0 by the guard, not by f(0): they are operand rows of product 2 and sigmoid(0) = 0.5
+            GO1_ACT_SWITCH(kind, KD,
+                _Pragma("unroll")
+                for (int j = 0; j < NH2 / 8; j++) {
+                    const float2 bb = *reinterpret_cast<const float2*>(b2 + wgi * NH2 + 8 * j + 2 * (lane & 3));
+                    acc[4 * j] = ok0 ? act_fast<KD>(acc[4 * j] + bb.x) : 0.f; acc[4 * j + 1] = ok0 ? act_fast<KD>(acc[4 * j + 1] + bb.y) : 0.f;
+                    acc[4 * j + 2] = ok1 ? act_fast<KD>(acc[4 * j + 2] + bb.x) : 0.f; acc[4 * j + 3] = ok1 ? act_fast<KD>(acc[4 * j + 3] + bb.y) : 0.f;
+                })
             // (the previous block's readers of the y2 tile -- product 2 and the TMA stores -- were waited for at the end of that block)
             store_fragment<NH2 / 8>(acc, y2t, wgi * NH2, w, lane, [](float2 v, int, int) { return v; });
             if (N3 == 0) head_partial<NH2 / 8>(acc, wh, NL, pr.nh, wgi * NH2, lane, hp);       // two-layer tail: the head reads y2
@@ -762,15 +767,16 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_kernel(const
             wg::wait<0>();
             if (lane == 0) mbar_arrive(&empty2[prev]);
             const float* b3 = s_b3 + p * N3;
-#pragma unroll
-            for (int j = 0; j < NH3 / 8; j++) {
-                const int col = wgi * NH3 + 8 * j + 2 * (lane & 3);
-                const float2 bb = *reinterpret_cast<const float2*>(b3 + col);
-                acc[4 * j] = elu_fast(acc[4 * j] + bb.x); acc[4 * j + 1] = elu_fast(acc[4 * j + 1] + bb.y);
-                acc[4 * j + 2] = elu_fast(acc[4 * j + 2] + bb.x); acc[4 * j + 3] = elu_fast(acc[4 * j + 3] + bb.y);
-                if (ok0) *reinterpret_cast<float2*>(pr.y3 + (size_t)(m0 + rA) * pr.ldy3 + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
-                if (ok1) *reinterpret_cast<float2*>(pr.y3 + (size_t)(m0 + rA + 8) * pr.ldy3 + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-            }
+            GO1_ACT_SWITCH(kind, KD,
+                _Pragma("unroll")
+                for (int j = 0; j < NH3 / 8; j++) {
+                    const int col = wgi * NH3 + 8 * j + 2 * (lane & 3);
+                    const float2 bb = *reinterpret_cast<const float2*>(b3 + col);
+                    acc[4 * j] = act_fast<KD>(acc[4 * j] + bb.x); acc[4 * j + 1] = act_fast<KD>(acc[4 * j + 1] + bb.y);
+                    acc[4 * j + 2] = act_fast<KD>(acc[4 * j + 2] + bb.x); acc[4 * j + 3] = act_fast<KD>(acc[4 * j + 3] + bb.y);
+                    if (ok0) *reinterpret_cast<float2*>(pr.y3 + (size_t)(m0 + rA) * pr.ldy3 + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+                    if (ok1) *reinterpret_cast<float2*>(pr.y3 + (size_t)(m0 + rA + 8) * pr.ldy3 + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+                })
             head_partial<NH3 / 8>(acc, wh, NL, pr.nh, wgi * NH3, lane, hp);
         }
         // the head: sum over the four lanes that share a row, then warpgroup 1's half meets warpgroup 0's in shared memory
@@ -805,28 +811,28 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_kernel(const
     if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
-template <int K1, int N2, int N3>
+template <int K1, int N2, int N3, bool ANYKIND>
 int launch_tail(const TailMaps& maps, const TailArgs& g, cudaStream_t st) {
     using L = TailSmem<K1, N2, N3>;
     static_assert(L::TOTAL <= 227 * 1024, "fused tail: shared memory budget");
     const size_t smem = L::TOTAL;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(mlp_tail_fwd_kernel<K1, N2, N3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(mlp_tail_fwd_kernel<K1, N2, N3, ANYKIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
         configured = true;
     }
     const int sms = sm_count();
     const int grid = g.tiles < sms ? g.tiles : sms;
-    mlp_tail_fwd_kernel<K1, N2, N3><<<grid, 32 * NCONS + 128, smem, st>>>(maps, g);
+    mlp_tail_fwd_kernel<K1, N2, N3, ANYKIND><<<grid, 32 * NCONS + 128, smem, st>>>(maps, g);
     go1_count_launch(1);
     return 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Fused MLP tail, backward (first half): for the bodies 512-256-128-head (actor_critic.py:38-77), from the gradient of the head's output,
-//     dz3 = (dout Wh) * ELU'(y3)   [M][128]     CUDA cores: K = nh <= 12
-//     dz2 = (dz3 W3) * ELU'(y2)    [M][256]     tensor core: A = the dz3 tile the consumer warps laid out in shared memory, B = W3 (resident)
+//     dz3 = (dout Wh) * f'(y3)     [M][128]     CUDA cores: K = nh <= 12
+//     dz2 = (dz3 W3) * f'(y2)      [M][256]     tensor core: A = the dz3 tile the consumer warps laid out in shared memory, B = W3 (resident)
 // plus the bias gradients gb3 = colsum(dz3), gb2 = colsum(dz2), for up to two problems (actor + critic) in one grid.  This replaces, per
 // body, a skinny dgrad launch and a 24576 x 256 x 128 dgrad launch (which re-reads dz3 from memory and whose tiles are too short to hide
 // their epilogue): dz3 never leaves the SM between the two products.  The wgrads (dz3^T y2, dz2^T y1) and the last dgrad (dz1) stay
@@ -835,11 +841,11 @@ int launch_tail(const TailMaps& maps, const TailArgs& g, cudaStream_t st) {
 //   warps 0-7   transpose those boxes into the resident K-major operand (128 KB); per block: E0, warp = (32-row half, 32-column chunk),
 //               builds a dz3 chunk from dout, Wh (shared memory) and y3, writes it swizzled into the A tile and sends it to global memory
 //               by TMA; then warpgroup g multiplies the tile by columns [128 g, 128 g + 128) of W3 (16 wgmma) and E1 multiplies the
-//               accumulator fragments by ELU'(y2) and stores dz2 from registers.
+//               accumulator fragments by f'(y2) and stores dz2 from registers.
 // Column sums meet in shared memory (atomics) and are flushed once per CTA.
 // ---------------------------------------------------------------------------------------------------------------
 struct TailBwdProb { const float* dout; const float* Wh; const float* y3; const float* y2; float* dz2; float* gb3; float* gb2; int lddout, nh, ldy3, ldy2, lddz2; };
-struct TailBwdArgs { TailBwdProb p[TAIL_MAXP]; int nprob, M, tiles_per_prob, tiles; };
+struct TailBwdArgs { TailBwdProb p[TAIL_MAXP]; int nprob, M, tiles_per_prob, tiles, kind; };
 struct TailBwdMaps { CUtensorMap w3[TAIL_MAXP], dz3[TAIL_MAXP]; };
 constexpr int TB_N3 = 128, TB_N2 = 256;
 constexpr int TB_W3_BYTES = TB_N3 * TB_N2 * 4;                 // 128 KB: 4 k-blocks x [256 n][32 k]
@@ -865,7 +871,8 @@ __device__ __forceinline__ float warp_colsum32(const float (&v)[32], const int l
     return sred[0];
 }
 
-__global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_bwd_kernel(const __grid_constant__ TailBwdMaps maps, const TailBwdArgs g) {
+template <typename D>
+__device__ __forceinline__ void mlp_tail_bwd_body(const TailBwdMaps& maps, const TailBwdArgs& g, const D dact) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* base = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t* w3s = base;                                     // B operand: [4 k-blocks][256 n][32 k], 128B-swizzled
@@ -930,7 +937,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_bwd_kernel(const
                 if (lane == 0) mbar_arrive(raw_free);
             }
         }
-        // ---- E0: dz3 chunk cg = (dout Wh)[.., 32 cg ..] * ELU'(y3)
+        // ---- E0: dz3 chunk cg = (dout Wh)[.., 32 cg ..] * f'(y3)
         {
             const int row = m0 + 32 * h + lane;
             const bool row_ok = row < g.M;
@@ -959,8 +966,8 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_bwd_kernel(const
             }
 #pragma unroll
             for (int j = 0; j < 8; j++) {
-                v[4 * j] *= (y[j].x > 0.f ? 1.0f : y[j].x + 1.0f); v[4 * j + 1] *= (y[j].y > 0.f ? 1.0f : y[j].y + 1.0f);
-                v[4 * j + 2] *= (y[j].z > 0.f ? 1.0f : y[j].z + 1.0f); v[4 * j + 3] *= (y[j].w > 0.f ? 1.0f : y[j].w + 1.0f);
+                v[4 * j] *= dact(y[j].x); v[4 * j + 1] *= dact(y[j].y);
+                v[4 * j + 2] *= dact(y[j].z); v[4 * j + 3] *= dact(y[j].w);
             }
             if (!row_ok) {
 #pragma unroll
@@ -980,7 +987,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_bwd_kernel(const
             }
         }
         cons_sync();                                                    // the dz3 tile (and, for a new problem, W3) is in shared memory
-        // ---- the product and E1: dz2 columns [128 wgi, 128 wgi + 128) = accumulator * ELU'(y2)
+        // ---- the product and E1: dz2 columns [128 wgi, 128 wgi + 128) = accumulator * f'(y2)
         {
             float acc[64];
             wg::fence();
@@ -996,8 +1003,8 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_bwd_kernel(const
             for (int j = 0; j < 16; j++) {
                 const int col = 128 * wgi + 8 * j + 2 * (lane & 3);
                 const float2 ya = __ldg(reinterpret_cast<const float2*>(y0 + col)), yb = __ldg(reinterpret_cast<const float2*>(y1 + col));
-                float2 va = make_float2(acc[4 * j] * (ya.x > 0.f ? 1.0f : ya.x + 1.0f), acc[4 * j + 1] * (ya.y > 0.f ? 1.0f : ya.y + 1.0f));
-                float2 vb = make_float2(acc[4 * j + 2] * (yb.x > 0.f ? 1.0f : yb.x + 1.0f), acc[4 * j + 3] * (yb.y > 0.f ? 1.0f : yb.y + 1.0f));
+                float2 va = make_float2(acc[4 * j] * dact(ya.x), acc[4 * j + 1] * dact(ya.y));
+                float2 vb = make_float2(acc[4 * j + 2] * dact(yb.x), acc[4 * j + 3] * dact(yb.y));
                 if (!ok0) va = make_float2(0.f, 0.f);
                 if (!ok1) vb = make_float2(0.f, 0.f);
                 if (ok0) *reinterpret_cast<float2*>(pr.dz2 + (size_t)(m0 + rA) * pr.lddz2 + col) = va;
@@ -1020,6 +1027,11 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_bwd_kernel(const
         const float vsum = s_cs[p * (TB_N3 + TB_N2) + c];
         if (vsum != 0.f) atomicAdd(c < TB_N3 ? g.p[p].gb3 + c : g.p[p].gb2 + (c - TB_N3), vsum);
     }
+}
+template <bool ANYKIND>
+__global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_bwd_kernel(const __grid_constant__ TailBwdMaps maps, const TailBwdArgs g) {
+    if (ANYKIND) mlp_tail_bwd_body(maps, g, act_deriv_coefficients(g.kind));
+    else mlp_tail_bwd_body(maps, g, [](float y) { return act_deriv<GO1_ACT_ELU>(y); });
 }
 
 }  // namespace
@@ -1065,6 +1077,8 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
                           float* const* Cs, int ldc, const Go1GemmEpilogue* ep, cudaStream_t st) {
     float* Cm = Cs[0];
     const float* bias = ep->bias; const int act = ep->act, accumulate = ep->accumulate;
+    if (act < 0 || act > 2) return go1_set_error("go1_gemm_ex: act must be 0, 1 or 2");
+    if (!go1_act_kind_ok(ep->act_kind)) return go1_set_error("go1_gemm_ex: unknown activation kind (Go1Activation)");
     const int amn = transA ? 1 : 0, bmn = transB ? 0 : 1;     // A given as [K][M] / B given as [K][N]: MN-major operands
     for (int p = 0; p < nprob; p++)
         if ((lda & 3) || (ldb & 3) || (((uintptr_t)As[p] | (uintptr_t)Bs[p]) & 15) || !Cs[p])
@@ -1072,7 +1086,7 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     GemmArgs g;
     g.nprob = nprob; g.tiles_per_prob = 0;
     for (int p = 0; p < GEMM_MAXP; p++) g.Cg[p] = Cs[p < nprob ? p : 0];
-    g.C = Cm; g.bias = bias; g.M = M; g.N = N; g.K = K; g.ldc = ldc; g.act = act; g.accumulate = accumulate;
+    g.C = Cm; g.bias = bias; g.M = M; g.N = N; g.K = K; g.ldc = ldc; g.act = act; g.kind = ep->act_kind; g.accumulate = accumulate;
     g.ex = ep->extra; g.ldex = ep->ld_extra; g.wex = ep->w_extra; g.ldwex = ep->ld_w_extra; g.nex = ep->extra ? ep->num_extra : 0;
     g.aux = ep->dact_y; g.ldaux = ep->ld_dact_y;
     g.amn = amn; g.bmn = bmn; g.lead = ep->lead_cols; g.colsum = ep->colsum;
@@ -1116,7 +1130,7 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
         g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, BN, g.colsum ? 1 : 0});
     }
     int e;
-    // staged epilogue: C blocks leave the accumulator staging by TMA store, the ELU' operand arrives through TMA loads
+    // staged epilogue: C blocks leave the accumulator staging by TMA store, the derivative operand arrives through TMA loads
     static const int use_staged = getenv("GO1_TF32_STAGED") ? atoi(getenv("GO1_TF32_STAGED")) : 1;
     CUtensorMap mc = ma, my = ma;
     g.tma_store = g.tma_aux = 0;
@@ -1128,12 +1142,13 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
             g.tma_aux = 1;
         }
     }
-    if (BN == 128) e = launch_gemm<128, true>(gm, mc, my, g, splits, st);
-    else if (BN == 64) e = launch_gemm<64, true>(gm, mc, my, g, splits, st);
-    else e = launch_gemm<32, true>(gm, mc, my, g, splits, st);
+    const bool any = g.act != 0 && g.kind != GO1_ACT_ELU;
+    if (BN == 128) e = any ? launch_gemm<128, true, true>(gm, mc, my, g, splits, st) : launch_gemm<128, true, false>(gm, mc, my, g, splits, st);
+    else if (BN == 64) e = any ? launch_gemm<64, true, true>(gm, mc, my, g, splits, st) : launch_gemm<64, true, false>(gm, mc, my, g, splits, st);
+    else e = any ? launch_gemm<32, true, true>(gm, mc, my, g, splits, st) : launch_gemm<32, true, false>(gm, mc, my, g, splits, st);
     if (e) return e;
     if (splits > 1 && (bias || act))
-        for (int p = 0; p < nprob; p++) { const size_t tot = (size_t)M * N; bias_act_strided<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cs[p], ldc, bias, M, N, act); go1_count_launch(1); }
+        for (int p = 0; p < nprob; p++) { const size_t tot = (size_t)M * N; bias_act_strided<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cs[p], ldc, bias, M, N, act, ep->act_kind); go1_count_launch(1); }
     if (timed) cudaEventRecord(timing_event(), st);
     cudaError_t ce = cudaGetLastError();
     if (ce != cudaSuccess) return go1_set_error(cudaGetErrorString(ce));
@@ -1189,9 +1204,12 @@ extern "C" int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int npr
     TailMaps maps;
     TailArgs g;
     g.nprob = nprob; g.M = M; g.tiles_per_prob = (M + TAIL_BM - 1) / TAIL_BM; g.tiles = g.tiles_per_prob * nprob;
+    g.kind = probs[0].act_kind;
+    if (!go1_act_kind_ok(g.kind)) return go1_set_error("go1_mlp_tail_forward: unknown activation kind (Go1Activation)");
     int rows = 0;
     for (int p = 0; p < nprob; p++) {
         const Go1TailProblem& q = probs[p];
+        if (q.act_kind != g.kind) return go1_set_error("go1_mlp_tail_forward: the problems of one launch share their activation kind");
         if (!q.x || !q.W2 || !q.y2 || !q.Wh || !q.out || q.nh < 1 || q.nh > TAIL_HPW || q.ldout < q.nh) return go1_set_error("go1_mlp_tail_forward: bad arguments (head width 1..12)");
         if (N3 > 0 && (!q.W3 || !q.y3)) return go1_set_error("go1_mlp_tail_forward: the three-layer tail needs W3 / y3");
         if ((q.ldx & 3) || (q.ldy2 & 3) || (N3 > 0 && (q.ldy3 & 3)) ||
@@ -1217,7 +1235,9 @@ extern "C" int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int npr
         g_time_flop += fl;
         g_time_recs.push_back({M * nprob, N2, K1, 0, 0, 1, 0, 1, shape_a ? 1003 : 1002, 0});
     }
-    int e = shape_a ? launch_tail<512, 256, 128>(maps, g, st) : launch_tail<256, 128, 0>(maps, g, st);
+    int e;
+    if (g.kind == GO1_ACT_ELU) e = shape_a ? launch_tail<512, 256, 128, false>(maps, g, st) : launch_tail<256, 128, 0, false>(maps, g, st);
+    else e = shape_a ? launch_tail<512, 256, 128, true>(maps, g, st) : launch_tail<256, 128, 0, true>(maps, g, st);
     if (e) return e;
     if (timed) cudaEventRecord(timing_event(), st);
     cudaError_t ce = cudaGetLastError();
@@ -1227,7 +1247,7 @@ extern "C" int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int npr
 extern "C" int go1_mlp_tail_forward(const float* x, int ldx, int M, int K1, const float* W2, const float* b2, int N2, float* y2, int ldy2,
                                     const float* W3, const float* b3, int N3, float* y3, int ldy3, const float* Wh, const float* bh, int nh,
                                     float* out, int ldout, void* stream) {
-    Go1TailProblem q;
+    Go1TailProblem q = {};
     q.x = x; q.ldx = ldx; q.W2 = W2; q.b2 = b2; q.y2 = y2; q.ldy2 = ldy2; q.W3 = W3; q.b3 = b3; q.y3 = y3; q.ldy3 = ldy3; q.Wh = Wh; q.bh = bh; q.nh = nh; q.out = out; q.ldout = ldout;
     return go1_mlp_tail_forward_grouped(&q, 1, M, K1, N2, N3, stream);
 }
@@ -1240,8 +1260,11 @@ extern "C" int go1_mlp_tail_backward_grouped(const Go1TailBwdProblem* probs, int
     TailBwdMaps maps;
     TailBwdArgs g;
     g.nprob = nprob; g.M = M; g.tiles_per_prob = (M + TAIL_BM - 1) / TAIL_BM; g.tiles = g.tiles_per_prob * nprob;
+    g.kind = probs[0].act_kind;
+    if (!go1_act_kind_ok(g.kind)) return go1_set_error("go1_mlp_tail_backward: unknown activation kind (Go1Activation)");
     for (int p = 0; p < nprob; p++) {
         const Go1TailBwdProblem& q = probs[p];
+        if (q.act_kind != g.kind) return go1_set_error("go1_mlp_tail_backward: the problems of one launch share their activation kind");
         if (!q.dout || !q.Wh || !q.y3 || !q.W3 || !q.y2 || !q.dz3 || !q.dz2 || !q.gb3 || !q.gb2 || q.nh < 1 || q.nh > TAIL_HPW || q.lddout < q.nh)
             return go1_set_error("go1_mlp_tail_backward: bad arguments (head width 1..12)");
         if ((q.ldy3 & 3) || (q.ldy2 & 3) || (q.lddz3 & 3) || (q.lddz2 & 3) ||
@@ -1255,7 +1278,8 @@ extern "C" int go1_mlp_tail_backward_grouped(const Go1TailBwdProblem* probs, int
     for (int p = nprob; p < TAIL_MAXP; p++) { maps.w3[p] = maps.w3[0]; maps.dz3[p] = maps.dz3[0]; g.p[p] = g.p[0]; }
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(mlp_tail_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TB_SMEM);
+        cudaError_t e = cudaFuncSetAttribute(mlp_tail_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TB_SMEM);
+        if (e == cudaSuccess) e = cudaFuncSetAttribute(mlp_tail_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TB_SMEM);
         if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
         configured = true;
     }
@@ -1270,7 +1294,8 @@ extern "C" int go1_mlp_tail_backward_grouped(const Go1TailBwdProblem* probs, int
         g_time_recs.push_back({M * nprob, N2, N3, 0, 1, 2, 0, 1, 1004, 1});
     }
     const int grid = g.tiles < sms ? g.tiles : sms;
-    mlp_tail_bwd_kernel<<<grid, 32 * NCONS + 128, TB_SMEM, st>>>(maps, g);
+    if (g.kind == GO1_ACT_ELU) mlp_tail_bwd_kernel<false><<<grid, 32 * NCONS + 128, TB_SMEM, st>>>(maps, g);
+    else mlp_tail_bwd_kernel<true><<<grid, 32 * NCONS + 128, TB_SMEM, st>>>(maps, g);
     go1_count_launch(1);
     if (timed) cudaEventRecord(timing_event(), st);
     cudaError_t ce = cudaGetLastError();

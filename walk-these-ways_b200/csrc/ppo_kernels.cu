@@ -1,6 +1,6 @@
 // ppo_kernels.cu — learner-side kernels of go1_gym_learn/ppo_cse for sm_90a:
-//   GAE warp-scan (rollout_storage.py:74-88), fp32 CUDA-core GEMM with fused bias/ELU epilogue (the
-//   exact-fp32 path next to the wgmma TF32 path in gemm_tf32.cu), ELU backward, column sums, Normal
+//   GAE warp-scan (rollout_storage.py:74-88), fp32 CUDA-core GEMM with fused bias/activation epilogue (the
+//   exact-fp32 path next to the wgmma TF32 path in gemm_tf32.cu), activation backward, column sums, Normal
 //   sampling/log-prob (actor_critic.py:113-126), PPO loss + gradients (ppo.py:113-152), MSE
 //   (ppo.py:168-186), global grad-norm + clip + Adam (ppo.py:155-158), row gather
 //   (rollout_storage.py:98-137).
@@ -11,6 +11,7 @@
 #include <string.h>
 #include "../../include/go1_b200.h"
 #include "sim_math.cuh"
+#include "activation.cuh"
 void go1_count_launch(int n);
 
 extern int go1_set_error(const char* m);
@@ -116,18 +117,31 @@ extern "C" int go1_ppo_normalize_advantages(float* advantages, const double* sta
 }
 
 // ---------------------------------------------------------------------------------------------
-// fp32 CUDA-core GEMM: C[M][N] (+)= opA(A) opB(B) (+ bias[n]) with optional ELU.
+// fp32 CUDA-core GEMM: C[M][N] (+)= opA(A) opB(B) (+ bias[n]) with optional activation (Go1Activation `kind`, activation.cuh).
 //   TA == 0: A is [M][K] (lda), TA == 1: A is [K][M];  TB == 0: B is [K][N] (ldb), TB == 1: B is [N][K].
 // 128x128x8 tiles, 256 threads, 8x8 register micro-tiles; split-K over gridDim.z with atomicAdd.
 // ---------------------------------------------------------------------------------------------
-DI float elu1(float x) { return x > 0.f ? x : expm1f(x); }
+// The exact-fp32 kernels apply the activation per element inside unrolled loops: ELU stays inline (the configured default), the other
+// kinds share one out-of-line copy of their libm code.
+__device__ __noinline__ float act_exact_other(int kind, float v) {
+    GO1_ACT_SWITCH(kind, KD, return act_exact<KD>(v);)
+    return v;
+}
+DI float act_exact_rt(int kind, float v) { return kind == GO1_ACT_ELU ? act_exact<GO1_ACT_ELU>(v) : act_exact_other(kind, v); }
+DI float act_deriv_rt(int kind, float y) {
+    GO1_ACT_SWITCH(kind, KD, return act_deriv<KD>(y);)
+    return 1.0f;
+}
+// entry points that take a bare `int act`: mode in bits 0..7, Go1Activation above (GO1_ACT)
+static inline int act_mode(int act) { return act & 0xff; }
+static inline int act_kind(int act) { return act >> 8; }
 
 struct SgemmEp { const float* ex; const float* wex; const float* aux; int ldex, ldwex, nex, ldaux; };
 
 template <int TA, int TB>
 __global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
                                                     float* __restrict__ Cm, int ldc, const float* __restrict__ bias,
-                                                    int M, int N, int K, int act, int accumulate, int kchunk, const SgemmEp ep) {
+                                                    int M, int N, int K, int act, int kind, int accumulate, int kchunk, const SgemmEp ep) {
     constexpr int BM = 128, BN = 128, BK = 8;
     __shared__ float As[2][BK][BM + 4], Bs[2][BK][BN + 4];
     const int tid = threadIdx.x;
@@ -215,20 +229,20 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A,
             if (accumulate) v += *c;
             for (int t = 0; t < ep.nex; t++) v = fmaf(ep.ex[(size_t)gm * ep.ldex + t], ep.wex[(size_t)gn * ep.ldwex + t], v);
             if (bias) v += bias[gn];
-            if (act == 1) v = elu1(v);
-            else if (act == 2) { const float y = ep.aux[(size_t)gm * ep.ldaux + gn]; v *= (y > 0.f ? 1.0f : y + 1.0f); }
+            if (act == 1) v = act_exact_rt(kind, v);
+            else if (act == 2) { const float y = ep.aux[(size_t)gm * ep.ldaux + gn]; v *= act_deriv_rt(kind, y); }
             *c = v;
         }
     }
 }
 
-__global__ void bias_act_kernel(float* __restrict__ Cm, int ldc, const float* __restrict__ bias, int M, int N, int act) {
+__global__ void bias_act_kernel(float* __restrict__ Cm, int ldc, const float* __restrict__ bias, int M, int N, int act, int kind) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)M * N) return;
     const int m = (int)(i / N), n = (int)(i - (size_t)m * N);
     float v = Cm[(size_t)m * ldc + n];
     if (bias) v += bias[n];
-    if (act == 1) v = elu1(v);
+    if (act == 1) v = act_exact_rt(kind, v);
     Cm[(size_t)m * ldc + n] = v;
 }
 __global__ void zero_strided_kernel(float* __restrict__ Cm, int ldc, int M, int N) {
@@ -245,11 +259,13 @@ extern "C" int go1_gemm_ex(int transA, int transB, int M, int N, int K, const fl
                            float* Cm, int ldc, const Go1GemmEpilogue* epi, int impl, void* stream) {
     if (!A || !B || !Cm || !epi || M <= 0 || N <= 0 || K <= 0) return go1_set_error("go1_gemm: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
+    if (epi->act < 0 || epi->act > 2) return go1_set_error("go1_gemm_ex: act must be 0, 1 or 2");
+    if (!go1_act_kind_ok(epi->act_kind)) return go1_set_error("go1_gemm_ex: unknown activation kind (Go1Activation)");
     if (impl == 1) return go1_gemm_tf32(transA, transB, M, N, K, A, lda, B, ldb, Cm, ldc, epi, st);
     if (impl != 0) return go1_set_error("go1_gemm: unknown impl");
     if (epi->lead_cols > 0) return go1_set_error("go1_gemm_ex: lead_cols is implemented by impl 1 only");
     if (epi->colsum || epi->num_bwd_extra > 0) return go1_set_error("go1_gemm_ex: the fused column sum / trailing-input backward are implemented by impl 1 only");
-    const float* bias = epi->bias; const int act = epi->act, accumulate = epi->accumulate;
+    const float* bias = epi->bias; const int act = epi->act, kind = epi->act_kind, accumulate = epi->accumulate;
     SgemmEp ep; ep.ex = epi->extra; ep.wex = epi->w_extra; ep.aux = epi->dact_y; ep.ldex = epi->ld_extra; ep.ldwex = epi->ld_w_extra;
     ep.nex = epi->extra ? epi->num_extra : 0; ep.ldaux = epi->ld_dact_y;
     if (ep.nex < 0 || ep.nex > 4) return go1_set_error("go1_gemm_ex: num_extra must be 0..4");
@@ -265,13 +281,13 @@ extern "C" int go1_gemm_ex(int transA, int transB, int M, int N, int K, const fl
         const size_t tot = (size_t)M * N;
         zero_strided_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cm, ldc, M, N); go1_count_launch(1);
     }
-#define LAUNCH(TA, TB) sgemm_kernel<TA, TB><<<grid, 256, 0, st>>>(A, lda, B, ldb, Cm, ldc, bias, M, N, K, act, accumulate, kchunk, ep)
+#define LAUNCH(TA, TB) sgemm_kernel<TA, TB><<<grid, 256, 0, st>>>(A, lda, B, ldb, Cm, ldc, bias, M, N, K, act, kind, accumulate, kchunk, ep)
     if (!transA && !transB) LAUNCH(0, 0); else if (!transA && transB) LAUNCH(0, 1); else if (transA && !transB) LAUNCH(1, 0); else LAUNCH(1, 1);
     go1_count_launch(1);
 #undef LAUNCH
     if (splitk > 1 && (bias || act)) {
         const size_t tot = (size_t)M * N;
-        bias_act_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cm, ldc, bias, M, N, act); go1_count_launch(1);
+        bias_act_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cm, ldc, bias, M, N, act, kind); go1_count_launch(1);
     }
     return cuda_rc("go1_gemm");
 }
@@ -279,24 +295,17 @@ extern "C" int go1_gemm(int transA, int transB, int M, int N, int K, const float
                         float* Cm, int ldc, const float* bias, int act, int accumulate, int impl, void* stream) {
     Go1GemmEpilogue ep;
     memset(&ep, 0, sizeof ep);
-    ep.bias = bias; ep.act = act; ep.accumulate = accumulate;
+    if (act < 0) return go1_set_error("go1_gemm: bad act");
+    ep.bias = bias; ep.act = act_mode(act); ep.act_kind = act_kind(act); ep.accumulate = accumulate;
     return go1_gemm_ex(transA, transB, M, N, K, A, lda, B, ldb, Cm, ldc, &ep, impl, stream);
 }
 
-// ELU, branch-free (the same polynomial / ex2 split as the wgmma epilogue, gemm_tf32.cu: absolute error ~1e-7)
-__device__ __forceinline__ float elu_fast(float v) {
-    float p = fmaf(v, 1.f / 5040.f, 1.f / 720.f);
-    p = fmaf(p, v, 1.f / 120.f); p = fmaf(p, v, 1.f / 24.f); p = fmaf(p, v, 1.f / 6.f); p = fmaf(p, v, 0.5f);
-    p = fmaf(p * v, v, v);
-    float e;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(v * 1.4426950408889634f));
-    const float n = v > -0.35f ? p : e - 1.0f;
-    return v > 0.f ? v : n;
-}
 // y = act(y + extra . w_extra^T) in place: the deferred trailing-input term + activation of a first layer.
-// float4 variant (o % 4 == 0, 16-byte aligned rows): one thread = 4 consecutive columns, 4 row-strided elements in flight per thread.
+// float4 variant (o % 4 == 0, 16-byte aligned rows): one thread = 4 consecutive columns, 4 row-strided elements in flight per thread;
+// it finishes a wgmma product, so it uses the branch-free activations of that path (act_fast).  KIND < 0: no activation.
+template <int KIND>
 __global__ void __launch_bounds__(256) extra_fwd4_kernel(float* __restrict__ y, int ldy, const float* __restrict__ ex, int ldex, const float* __restrict__ wex, int ldw,
-                                                         int M, int o4, int E, int act, int rows_per_pass) {
+                                                         int M, int o4, int E, int rows_per_pass) {
     // blockDim.x = 256 threads = (256 / o4) rows x o4 column groups (o4 divides 256) or one row segment
     const int cg = threadIdx.x % o4, rsub = threadIdx.x / o4, rpb = blockDim.x / o4;
     float w[4][4];
@@ -325,7 +334,7 @@ __global__ void __launch_bounds__(256) extra_fwd4_kernel(float* __restrict__ y, 
                     float a = r[c];
 #pragma unroll
                     for (int t = 0; t < 4; t++) a = fmaf(e[u][t], w[c][t], a);
-                    r[c] = act == 1 ? elu_fast(a) : a;
+                    r[c] = KIND >= 0 ? act_fast<(KIND >= 0 ? KIND : 0)>(a) : a;
                 }
                 *reinterpret_cast<float4*>(y + (size_t)m * ldy + 4 * cg) = make_float4(r[0], r[1], r[2], r[3]);
             }
@@ -334,7 +343,7 @@ __global__ void __launch_bounds__(256) extra_fwd4_kernel(float* __restrict__ y, 
 }
 // generic variant: grid (column blocks of 256, row blocks of 8): each thread keeps its column's E weights in registers and walks 8 rows
 __global__ void __launch_bounds__(256) extra_fwd_kernel(float* __restrict__ y, int ldy, const float* __restrict__ ex, int ldex, const float* __restrict__ wex, int ldw,
-                                                        int M, int o, int E, int act) {
+                                                        int M, int o, int E, int act, int kind) {
     const int n = blockIdx.x * 256 + threadIdx.x;
     if (n >= o) return;
     float w[4] = {0.f, 0.f, 0.f, 0.f};
@@ -347,39 +356,50 @@ __global__ void __launch_bounds__(256) extra_fwd_kernel(float* __restrict__ y, i
 #pragma unroll
         for (int t = 0; t < 4; t++) if (t < E) acc = fmaf(__ldg(ex + (size_t)m * ldex + t), w[t], acc);
         float v = y[(size_t)m * ldy + n] + acc;
-        if (act == 1) v = v > 0.f ? v : expm1f(v);
+        if (act == 1) v = act_exact_rt(kind, v);
         y[(size_t)m * ldy + n] = v;
     }
 }
 extern "C" int go1_mlp_extra_forward(float* y, int ldy, const float* extra, int ldex, const float* w_extra, int ldw, int M, int o, int E, int act,
                                      void* stream) {
-    if (!y || !extra || !w_extra || M <= 0 || o <= 0 || E < 1 || E > 4 || act < 0 || act > 1) return go1_set_error("go1_mlp_extra_forward: bad arguments");
+    if (!y || !extra || !w_extra || M <= 0 || o <= 0 || E < 1 || E > 4 || act < 0 || act_mode(act) > 1) return go1_set_error("go1_mlp_extra_forward: bad arguments");
+    const int kind = act_kind(act);
+    act = act_mode(act);
+    if (!go1_act_kind_ok(kind)) return go1_set_error("go1_mlp_extra_forward: unknown activation kind (Go1Activation)");
     const int o4 = o / 4;
     if ((o & 3) == 0 && (ldy & 3) == 0 && (((uintptr_t)y) & 15) == 0 && o4 <= 256 && 256 % o4 == 0) {
         const int rpb = 256 / o4;
         int grid = (M + 4 * rpb - 1) / (4 * rpb);
         if (grid > 132 * 16) grid = 132 * 16;
-        extra_fwd4_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(y, ldy, extra, ldex, w_extra, ldw, M, o4, E, act, 4 * rpb); go1_count_launch(1);
+#define LAUNCH(KD) extra_fwd4_kernel<KD><<<grid, 256, 0, (cudaStream_t)stream>>>(y, ldy, extra, ldex, w_extra, ldw, M, o4, E, 4 * rpb)
+        if (act == 0) LAUNCH(-1);
+        else { GO1_ACT_SWITCH(kind, KD, LAUNCH(KD);) }
+#undef LAUNCH
+        go1_count_launch(1);
         return cuda_rc("go1_mlp_extra_forward");
     }
     dim3 grid((o + 255) / 256, (M + 7) / 8);
-    extra_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(y, ldy, extra, ldex, w_extra, ldw, M, o, E, act); go1_count_launch(1);
+    extra_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(y, ldy, extra, ldex, w_extra, ldw, M, o, E, act, kind); go1_count_launch(1);
     return cuda_rc("go1_mlp_extra_forward");
 }
 
-// dz = dy * ELU'(y) from the saved output y (alpha = 1: ELU' = 1 for y > 0 else y + 1)
-__global__ void elu_bwd_kernel(const float* __restrict__ y, int ldy, const float* __restrict__ dy, int lddy, float* __restrict__ dz, int lddz, int M, int N) {
+// dz = dy * f'(z) from the saved output y (act_deriv, activation.cuh; ELU, alpha = 1: 1 for y > 0 else y + 1)
+__global__ void act_bwd_kernel(const float* __restrict__ y, int ldy, const float* __restrict__ dy, int lddy, float* __restrict__ dz, int lddz, int M, int N, int kind) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (size_t)M * N) return;
     const int m = (int)(i / N), n = (int)(i - (size_t)m * N);
     const float yv = y[(size_t)m * ldy + n];
-    dz[(size_t)m * lddz + n] = dy[(size_t)m * lddy + n] * (yv > 0.f ? 1.0f : yv + 1.0f);
+    dz[(size_t)m * lddz + n] = dy[(size_t)m * lddy + n] * act_deriv_rt(kind, yv);
+}
+extern "C" int go1_act_backward(const float* y, int ldy, const float* dy, int lddy, float* dz, int lddz, int M, int N, int kind, void* stream) {
+    if (!y || !dy || !dz || M <= 0 || N <= 0) return go1_set_error("go1_act_backward: bad arguments");
+    if (!go1_act_kind_ok(kind)) return go1_set_error("go1_act_backward: unknown activation kind (Go1Activation)");
+    const size_t tot = (size_t)M * N;
+    act_bwd_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, (cudaStream_t)stream>>>(y, ldy, dy, lddy, dz, lddz, M, N, kind); go1_count_launch(1);
+    return cuda_rc("go1_act_backward");
 }
 extern "C" int go1_elu_backward(const float* y, int ldy, const float* dy, int lddy, float* dz, int lddz, int M, int N, void* stream) {
-    if (!y || !dy || !dz || M <= 0 || N <= 0) return go1_set_error("go1_elu_backward: bad arguments");
-    const size_t tot = (size_t)M * N;
-    elu_bwd_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, (cudaStream_t)stream>>>(y, ldy, dy, lddy, dz, lddz, M, N); go1_count_launch(1);
-    return cuda_rc("go1_elu_backward");
+    return go1_act_backward(y, ldy, dy, lddy, dz, lddz, M, N, GO1_ACT_ELU, stream);
 }
 
 // wgrad of a narrow (o <= 16) output layer: gW[j][k] (+)= sum_m dz[m][j] x[m][k].  One thread per input column k keeps the o
@@ -858,7 +878,7 @@ extern "C" int go1_gather_rows(const float* src, const int64_t* idx, float* dst,
 // ---------------------------------------------------------------------------------------------
 // skinny pieces of the MLP backward that are pure bandwidth (one pass over dz), kept off the GEMM kernels:
 //   extra columns of a first layer:  dextra[m][t] = sum_j dz[m][j] We[j][t];   gWe[j][t] (+)= sum_m dz[m][j] extra[m][t]
-//   dgrad through a <=4-wide output: dprev[m][c] = (sum_t dz[m][t] W[t][c]) * ELU'(y_prev[m][c])
+//   dgrad through a <=4-wide output: dprev[m][c] = (sum_t dz[m][t] W[t][c]) * f'(y_prev[m][c])   (f' from the saved output: act_deriv)
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) extra_dinput_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ We, int ldw,
                                                            float* __restrict__ dextra, int ldde, int M, int o, int E) {
@@ -913,21 +933,21 @@ extern "C" int go1_mlp_extra_backward(const float* dz, int lddz, const float* ex
     return cuda_rc("go1_mlp_extra_backward");
 }
 __global__ void skinny_dgrad_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ W, int ldw, const float* __restrict__ y, int ldy,
-                                    float* __restrict__ dprev, int lddp, int M, int o, int n) {
+                                    float* __restrict__ dprev, int lddp, int M, int o, int n, int kind) {
     const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (size_t)M * n) return;
     const int m = (int)(idx / n), c = (int)(idx - (size_t)m * n);
     float v = 0.f;
 #pragma unroll
     for (int t = 0; t < 16; t++) if (t < o) v = fmaf(__ldg(dz + (size_t)m * lddz + t), __ldg(W + (size_t)t * ldw + c), v);
-    if (y) { const float yy = y[(size_t)m * ldy + c]; v *= (yy > 0.f ? 1.0f : yy + 1.0f); }
+    if (y) { const float yy = y[(size_t)m * ldy + c]; v *= act_deriv_rt(kind, yy); }
     dprev[(size_t)m * lddp + c] = v;
 }
 // float4 variant: a warp owns rows (stride 8 inside the block's row slab), a lane owns 4 consecutive columns of a 128-column group and keeps
 // its O x 4 weights in registers; the row's o output gradients are fetched by the first o lanes and shuffle-broadcast.  Optionally the
 // column sums of the values written (= the bias gradient of the layer below) are reduced here as well: per-lane partial sums, one
 // shared-memory reduction per block, one set of atomics per block.
-template <int O>
+template <int O, int KIND>
 __global__ void __launch_bounds__(256) skinny_dgrad4_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ W, int ldw, const float* __restrict__ y, int ldy,
                                                             float* __restrict__ dprev, int lddp, float* __restrict__ colsum, int M, int o, int n, int rows_per_block) {
     __shared__ float4 s_sum[8][32];
@@ -953,7 +973,7 @@ __global__ void __launch_bounds__(256) skinny_dgrad4_kernel(const float* __restr
             const float d = __shfl_sync(0xffffffffu, dl, t);
             v0 = fmaf(d, wr[t][0], v0); v1 = fmaf(d, wr[t][1], v1); v2 = fmaf(d, wr[t][2], v2); v3 = fmaf(d, wr[t][3], v3);
         }
-        if (y) { v0 *= (yy.x > 0.f ? 1.0f : yy.x + 1.0f); v1 *= (yy.y > 0.f ? 1.0f : yy.y + 1.0f); v2 *= (yy.z > 0.f ? 1.0f : yy.z + 1.0f); v3 *= (yy.w > 0.f ? 1.0f : yy.w + 1.0f); }
+        if (y) { v0 *= act_deriv<KIND>(yy.x); v1 *= act_deriv<KIND>(yy.y); v2 *= act_deriv<KIND>(yy.z); v3 *= act_deriv<KIND>(yy.w); }
         if (col_ok) *reinterpret_cast<float4*>(dprev + (size_t)m * lddp + c) = make_float4(v0, v1, v2, v3);
         cs.x += v0; cs.y += v1; cs.z += v2; cs.w += v3;
     }
@@ -968,9 +988,10 @@ __global__ void __launch_bounds__(256) skinny_dgrad4_kernel(const float* __restr
         }
     }
 }
-extern "C" int go1_skinny_dgrad_ex(const float* dz, int lddz, const float* W, int ldw, const float* y_prev, int ldy, float* dprev, int lddp,
-                                   float* colsum, int M, int o, int n, void* stream) {
+extern "C" int go1_skinny_dgrad_act(const float* dz, int lddz, const float* W, int ldw, const float* y_prev, int ldy, float* dprev, int lddp,
+                                    float* colsum, int M, int o, int n, int kind, void* stream) {
     if (!dz || !W || !dprev || M <= 0 || o <= 0 || o > 16 || n <= 0) return go1_set_error("go1_skinny_dgrad: bad arguments");
+    if (!go1_act_kind_ok(kind)) return go1_set_error("go1_skinny_dgrad: unknown activation kind (Go1Activation)");
     cudaStream_t st = (cudaStream_t)stream;
     const bool vec = (n & 3) == 0 && (ldw & 3) == 0 && (lddp & 3) == 0 && (!y_prev || (ldy & 3) == 0) &&
                      ((((uintptr_t)W) | ((uintptr_t)dprev) | ((uintptr_t)(y_prev ? y_prev : W))) & 15) == 0;
@@ -979,16 +1000,20 @@ extern "C" int go1_skinny_dgrad_ex(const float* dz, int lddz, const float* W, in
         int rpb = (M * cb + 2 * 132 - 1) / (2 * 132);           // about two blocks per SM
         rpb = (rpb + 7) / 8 * 8; if (rpb < 8) rpb = 8;
         dim3 grid(cb, (M + rpb - 1) / rpb);
-        if (o <= 2) skinny_dgrad4_kernel<2><<<grid, 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, colsum, M, o, n, rpb);
-        else if (o <= 4) skinny_dgrad4_kernel<4><<<grid, 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, colsum, M, o, n, rpb);
-        else skinny_dgrad4_kernel<16><<<grid, 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, colsum, M, o, n, rpb);
+#define LAUNCH(O, KD) skinny_dgrad4_kernel<O, KD><<<grid, 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, colsum, M, o, n, rpb)
+        GO1_ACT_SWITCH(kind, KD, if (o <= 2) LAUNCH(2, KD); else if (o <= 4) LAUNCH(4, KD); else LAUNCH(16, KD);)
+#undef LAUNCH
         go1_count_launch(1);
         return cuda_rc("go1_skinny_dgrad");
     }
     if (colsum) return go1_set_error("go1_skinny_dgrad_ex: the fused column sum needs 16-byte aligned operands with n % 4 == 0");
     const size_t tot = (size_t)M * n;
-    skinny_dgrad_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, M, o, n); go1_count_launch(1);
+    skinny_dgrad_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, M, o, n, kind); go1_count_launch(1);
     return cuda_rc("go1_skinny_dgrad");
+}
+extern "C" int go1_skinny_dgrad_ex(const float* dz, int lddz, const float* W, int ldw, const float* y_prev, int ldy, float* dprev, int lddp,
+                                   float* colsum, int M, int o, int n, void* stream) {
+    return go1_skinny_dgrad_act(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, colsum, M, o, n, GO1_ACT_ELU, stream);
 }
 extern "C" int go1_skinny_dgrad(const float* dz, int lddz, const float* W, int ldw, const float* y_prev, int ldy, float* dprev, int lddp,
                                 int M, int o, int n, void* stream) {

@@ -109,17 +109,26 @@ class Go1CurriculumBuffers(C.Structure):
         "xr_send", "xr_events", "xr_ids", "xr_commands")]
 
 
+# enum Go1Activation (include/go1_b200.h), keyed by the names AC_Args.activation accepts (the reference maps crelu to nn.ReLU too)
+ACTIVATIONS = {"elu": 0, "selu": 1, "relu": 2, "crelu": 2, "lrelu": 3, "tanh": 4, "sigmoid": 5}
+
+
+def act_arg(kind, mode):
+    """GO1_ACT(kind, mode): the `act` argument of the entry points that take a bare int."""
+    return (kind << 8) | mode
+
+
 class Go1GemmEpilogue(C.Structure):
     _fields_ = [("bias", C.c_void_p), ("act", _i), ("accumulate", _i), ("extra", C.c_void_p), ("ld_extra", _i), ("w_extra", C.c_void_p),
                 ("ld_w_extra", _i), ("num_extra", _i), ("dact_y", C.c_void_p), ("ld_dact_y", _i), ("lead_cols", _i), ("colsum", C.c_void_p),
                 ("bwd_extra", C.c_void_p), ("bwd_w_extra", C.c_void_p), ("g_w_extra", C.c_void_p), ("d_extra", C.c_void_p),
-                ("ld_bwd_extra", _i), ("ld_bwd_w_extra", _i), ("ld_g_w_extra", _i), ("ld_d_extra", _i), ("num_bwd_extra", _i)]
+                ("ld_bwd_extra", _i), ("ld_bwd_w_extra", _i), ("ld_g_w_extra", _i), ("ld_d_extra", _i), ("num_bwd_extra", _i), ("act_kind", _i)]
 
 
 class Go1TailProblem(C.Structure):
     _fields_ = [("x", C.c_void_p), ("ldx", _i), ("W2", C.c_void_p), ("b2", C.c_void_p), ("y2", C.c_void_p), ("ldy2", _i),
                 ("W3", C.c_void_p), ("b3", C.c_void_p), ("y3", C.c_void_p), ("ldy3", _i), ("Wh", C.c_void_p), ("bh", C.c_void_p), ("nh", _i),
-                ("out", C.c_void_p), ("ldout", _i)]
+                ("out", C.c_void_p), ("ldout", _i), ("act_kind", _i)]
 
 
 class Go1CopySeg(C.Structure):
@@ -138,7 +147,8 @@ def copy_segments(pairs):
 
 class Go1TailBwdProblem(C.Structure):
     _fields_ = [("dout", C.c_void_p), ("lddout", _i), ("nh", _i), ("Wh", C.c_void_p), ("y3", C.c_void_p), ("ldy3", _i), ("W3", C.c_void_p),
-                ("y2", C.c_void_p), ("ldy2", _i), ("dz3", C.c_void_p), ("lddz3", _i), ("dz2", C.c_void_p), ("lddz2", _i), ("gb3", C.c_void_p), ("gb2", C.c_void_p)]
+                ("y2", C.c_void_p), ("ldy2", _i), ("dz3", C.c_void_p), ("lddz3", _i), ("dz2", C.c_void_p), ("lddz2", _i), ("gb3", C.c_void_p), ("gb2", C.c_void_p),
+                ("act_kind", _i)]
 
 
 class Go1Error(RuntimeError):
@@ -185,10 +195,12 @@ def lib():
         "go1_mlp_tail_forward": ([vp, ip, ip, ip, vp, vp, ip, vp, ip, vp, vp, ip, vp, ip, vp, vp, ip, vp, ip, vp], ip),
         "go1_transpose": ([vp, ip, vp, ip, ip, ip, vp], ip),
         "go1_elu_backward": ([vp, ip, vp, ip, vp, ip, ip, ip, vp], ip),
+        "go1_act_backward": ([vp, ip, vp, ip, vp, ip, ip, ip, ip, vp], ip),
         "go1_mlp_extra_forward": ([vp, ip, vp, ip, vp, ip, ip, ip, ip, ip, vp], ip),
         "go1_mlp_extra_backward": ([vp, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, ip, ip, vp], ip),
         "go1_skinny_dgrad": ([vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, ip, vp], ip),
         "go1_skinny_dgrad_ex": ([vp, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, vp], ip),
+        "go1_skinny_dgrad_act": ([vp, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, ip, vp], ip),
         "go1_skinny_wgrad_ex": ([vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, ip, vp], ip),
         "go1_gemm_grouped": ([ip, ip, ip, ip, ip, ip, C.POINTER(vp), ip, C.POINTER(vp), ip, C.POINTER(vp), ip, ip, vp], ip),
         "go1_copy_segments": ([C.POINTER(Go1CopySeg), ip, vp], ip),

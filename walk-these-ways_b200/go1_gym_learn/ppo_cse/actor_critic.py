@@ -7,7 +7,7 @@ the reference's names, .act / .evaluate / .act_student / .act_teacher / .get_act
   * all parameters are views into ONE flat fp32 buffer (adaptation module first), gradients into one flat
     gradient buffer -> one grad-norm, one Adam launch, one NCCL all-reduce per optimizer step;
   * forward and backward are explicit go1_gemm calls (fp32 CUDA-core or tcgen05 TF32) with fused
-    bias+ELU epilogues; cat(obs_history, latent) is never materialised (the 2 extra input columns are a
+    bias+activation epilogues (AC_Args.activation: every name of the reference's get_activation); cat(obs_history, latent) is never materialised (the 2 extra input columns are a
     second, K=2 GEMM accumulated into the first layer's pre-activation);
   * no autograd graph: the backward pass is written out (see `backward_ppo`, `backward_adaptation`).
 """
@@ -23,16 +23,16 @@ class AC_Args(PrefixProto, cli=False):
     init_noise_std = 1.0
     actor_hidden_dims = [512, 256, 128]
     critic_hidden_dims = [512, 256, 128]
-    activation = 'elu'  # only elu runs on the fused kernels
+    activation = 'elu'  # can be elu, relu, selu, crelu, lrelu, tanh, sigmoid (all run on the fused kernels; crelu is nn.ReLU, as in the reference)
     adaptation_module_branch_hidden_dims = [256, 128]
     use_decoder = False
     gemm_impl = 1       # 1 = tcgen05 TF32 tensor cores (default; torch 1.10, the reference's pin, also ran these matmuls in TF32), 0 = fp32 CUDA cores (exact)
 
 
-def _mlp(in_dim, hidden, out_dim):
+def _mlp(in_dim, hidden, out_dim, activation):
     layers, d = [], in_dim
     for h in hidden:
-        layers += [nn.Linear(d, h), nn.ELU()]
+        layers += [nn.Linear(d, h), get_activation(activation)]
         d = h
     layers.append(nn.Linear(d, out_dim))
     return nn.Sequential(*layers)
@@ -71,6 +71,7 @@ class _Net:
         self.acts = {}
         self._cache = {}
         self._ep = capi.Go1GemmEpilogue()
+        self.kind = self._ep.act_kind = owner.act_kind      # Go1Activation of the hidden layers, passed to every kernel that applies f or f'
 
     def _buf(self, key, M, width):
         t = self.acts.get(key)
@@ -193,6 +194,7 @@ class _Net:
         sp, flat = self.specs, self.flat
         ptr = lambda off: flat.data_ptr() + 4 * off
         q = capi.Go1TailProblem()
+        q.act_kind = self.kind
         (w2, b2, n2, k1) = sp[1]
         y2 = self._buf((tag, 1), M, n2)
         q.x, q.ldx, q.W2, q.b2, q.y2, q.ldy2 = self._p(x1), ldx1, ptr(w2), ptr(b2), y2.data_ptr(), y2.stride(0)
@@ -237,6 +239,7 @@ class _Net:
         capi.check(L.go1_skinny_wgrad_ex(capi.ptr(dout), dout.stride(0), capi.ptr(y3), y3.stride(0), gWh.data_ptr(), n3, gbh.data_ptr(), M, nh, n3, 1, st), "skinny_wgrad")
         dz3, dz2 = self._buf((tag, "d", 2), M, n3), self._buf((tag, "d", 1), M, n2)
         q = capi.Go1TailBwdProblem()
+        q.act_kind = self.kind
         q.dout, q.lddout, q.nh, q.Wh = dout.data_ptr(), dout.stride(0), nh, self.flat.data_ptr() + 4 * woh
         q.y3, q.ldy3, q.W3, q.y2, q.ldy2 = y3.data_ptr(), y3.stride(0), self.flat.data_ptr() + 4 * wo3, y2.data_ptr(), y2.stride(0)
         q.dz3, q.lddz3, q.dz2, q.lddz2 = dz3.data_ptr(), dz3.stride(0), dz2.data_ptr(), dz2.stride(0)
@@ -245,8 +248,8 @@ class _Net:
 
     def backward(self, x, ldx, K0, extra, outs, dout, M, impl, accumulate, want_dextra=False, tag="a", dz1_out=None, aug_first=False, pre=None):
         """dout: gradient w.r.t. the network output [M][out] (the last layer has no activation).  Writes weight/bias grads
-        into the flat grad buffer.  dz of every hidden layer comes out of the dgrad GEMM already multiplied by ELU'
-        (fused epilogue).  dz1_out: optional [M][o1] strided view; when given the first layer's dz is written there and its wgrad is
+        into the flat grad buffer.  dz of every hidden layer comes out of the dgrad GEMM already multiplied by the
+        activation's derivative, computed from the saved layer output (fused epilogue).  dz1_out: optional [M][o1] strided view; when given the first layer's dz is written there and its wgrad is
         left to the caller (ActorCritic fuses the three first-layer wgrads into one GEMM).  aug_first: the caller's fused wgrad also yields the first
         layer's bias gradient and trailing-input weight gradients (augmented input columns), so the dgrad epilogue that produces the first layer's
         dz reduces neither of them (only d(extra) if requested).  Returns d(extra) [M][E] if requested."""
@@ -298,7 +301,7 @@ class _Net:
                     dextra = self._buf((tag, "dextra"), M, E)
                 capi.check(L.go1_mlp_extra_backward(capi.ptr(dz), ldz, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i, gW.data_ptr() + 4 * K0, i,
                                                     capi.ptr(dextra) if want_dextra else None, E, M, o, E, accumulate, st), "extra_backward")
-            # ---- dgrad (+ fused ELU'): dz_prev[M][i] = (dz[M][o] W[o][i]) * ELU'(y_prev)
+            # ---- dgrad (+ fused activation derivative): dz_prev[M][i] = (dz[M][o] W[o][i]) * f'(y_prev)
             if pre is not None and li == n - 2:
                 dz, bias_done = pre[1], True            # produced (with its bias gradient) by the fused kernel
                 continue
@@ -345,8 +348,8 @@ class _Net:
                     if fuse and not accumulate and not self.owner.grads_prezeroed:
                         gb_prev.zero_()
                     # the bias gradient of layer li-1 (column sums of dprev) is reduced in the same pass
-                    capi.check(L.go1_skinny_dgrad_ex(capi.ptr(dz), ldz, capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(dprev), ldp,
-                                                     gb_prev.data_ptr() if fuse else None, M, o, i, st), "skinny_dgrad")
+                    capi.check(L.go1_skinny_dgrad_act(capi.ptr(dz), ldz, capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(dprev), ldp,
+                                                      gb_prev.data_ptr() if fuse else None, M, o, i, self.kind, st), "skinny_dgrad")
                     bias_done = bool(fuse)
                 else:
                     self._gemm(0, 0, M, i, o, dz, ldz, W, i, dprev, ldp, None, 2, 0, 0, dact_y=yprev)
@@ -363,12 +366,14 @@ class ActorCritic(nn.Module):
             print("ActorCritic.__init__ got unexpected arguments, which will be ignored: " + str([key for key in kwargs.keys()]))
         self.decoder = AC_Args.use_decoder
         super().__init__()
-        if AC_Args.activation != 'elu':
-            raise NotImplementedError("the fused MLP kernels implement ELU (the reference's configured activation)")
+        activation = AC_Args.activation
+        if activation not in capi.ACTIVATIONS:
+            raise ValueError(f"AC_Args.activation = {activation!r}: expected one of {sorted(capi.ACTIVATIONS)}")
+        self.act_kind = capi.ACTIVATIONS[activation]      # fixed per instance: it is baked into the captured CUDA graphs
         self.num_obs_history, self.num_privileged_obs, self.num_actions = num_obs_history, num_privileged_obs, num_actions
-        self.adaptation_module = _mlp(num_obs_history, AC_Args.adaptation_module_branch_hidden_dims, num_privileged_obs)
-        self.actor_body = _mlp(num_privileged_obs + num_obs_history, AC_Args.actor_hidden_dims, num_actions)
-        self.critic_body = _mlp(num_privileged_obs + num_obs_history, AC_Args.critic_hidden_dims, 1)
+        self.adaptation_module = _mlp(num_obs_history, AC_Args.adaptation_module_branch_hidden_dims, num_privileged_obs, activation)
+        self.actor_body = _mlp(num_privileged_obs + num_obs_history, AC_Args.actor_hidden_dims, num_actions, activation)
+        self.critic_body = _mlp(num_privileged_obs + num_obs_history, AC_Args.critic_hidden_dims, 1, activation)
         self.std = nn.Parameter(AC_Args.init_noise_std * torch.ones(num_actions))
         self.distribution = None
         self._flat = self._grad = None
@@ -501,9 +506,9 @@ class ActorCritic(nn.Module):
 
     def forward_all(self, observation_history, privileged_observations, tag="act"):
         """update_distribution + evaluate in one pass.  With the tensor-core path the first layers of the three MLPs --
-        which all read obs_history -- run as ONE product [M][256+512+512] = h Wcat^T: bias + ELU (+ the critic's two
+        which all read obs_history -- run as ONE product [M][256+512+512] = h Wcat^T: bias + activation (+ the critic's two
         privileged columns) ride in its epilogue for the adaptation/critic slices; the actor slice is finished
-        (latent columns + ELU) by go1_mlp_extra_forward once the adaptation module has produced the latent."""
+        (latent columns + activation) by go1_mlp_extra_forward once the adaptation module has produced the latent."""
         self.flatten()
         self._check_input(observation_history)
         h, priv = observation_history, privileged_observations.contiguous()
@@ -551,7 +556,7 @@ class ActorCritic(nn.Module):
         self._a_out = na.forward(h, h.stride(0), K0, None, M, impl, tag, first_out=ya)
         latent = self._latent = self._a_out[-1]
         capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(yp), yp.stride(0), capi.ptr(latent), latent.stride(0), Wp.data_ptr() + 4 * K0, K0 + E,
-                                                    M, op, E, 1, capi.stream_ptr()), "go1_mlp_extra_forward")
+                                                    M, op, E, capi.act_arg(self.act_kind, 1), capi.stream_ptr()), "go1_mlp_extra_forward")
         if pair:                    # the equal-shape tails of the actor and critic bodies in ONE grid
             qp, outs_p, shape = npol._tail_problem(yp, yp.stride(0), M, tag)
             qc, outs_c, _ = ncr._tail_problem(yc, yc.stride(0), M, tag)
@@ -759,8 +764,8 @@ class ActorCritic(nn.Module):
 
 
 def get_activation(act_name):
+    """The nn module of an AC_Args.activation name (reference actor_critic.py:149-166; an unknown name raises instead of returning None)."""
     table = {"elu": nn.ELU, "selu": nn.SELU, "relu": nn.ReLU, "crelu": nn.ReLU, "lrelu": nn.LeakyReLU, "tanh": nn.Tanh, "sigmoid": nn.Sigmoid}
     if act_name not in table:
-        print("invalid activation function!")
-        return None
+        raise ValueError(f"invalid activation function {act_name!r}: expected one of {sorted(table)}")
     return table[act_name]()
