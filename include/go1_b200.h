@@ -325,6 +325,10 @@ typedef struct Go1GemmEpilogue {
     const float* bwd_extra; const float* bwd_w_extra; float* g_w_extra; float* d_extra;
     int32_t ld_bwd_extra, ld_bwd_w_extra, ld_g_w_extra, ld_d_extra, num_bwd_extra;
     int32_t act_kind;    /* Go1Activation behind act 1 / 2 (0 = ELU) */
+    int32_t store_transposed;   /* impl 1: C is stored as its transpose, [N][M] with row stride ldc (the fused terms above still see
+                                 * C[m][n]); gives the next product a K-major operand: the first-layer dz of the weight-gradient product.
+                                 * Needs M >= 32, accumulate 0, a 16-byte aligned C and ldc % 4 == 0.  The TMA store writes whole 16-byte
+                                 * chunks: when M % 4 != 0, row padding columns M .. (M rounded up to 4) - 1 may be overwritten. */
 } Go1GemmEpilogue;
 int go1_gemm_ex(int transA, int transB, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
                 float* C, int ldc, const Go1GemmEpilogue* ep, int impl, void* stream);
@@ -364,8 +368,8 @@ int go1_mlp_tail_backward_grouped(const Go1TailBwdProblem* probs, int nprob, int
 int go1_gemm_timing(int on, double* total_ms, double* total_flop, long long* launches);
 /* number of kernels replayed through CUDA graphs, added to go1_kernel_launch_count() by the caller that replays them */
 void go1_kernel_launch_add(long long n);
-/* dst[c][r] = src[r][c] (rows x cols fp32, row strides lds/ldd).  Utility only: impl 1 reads operands in either major
- * (transA / transB as given), so the learner no longer stages transposed copies. */
+/* dst[c][r] = src[r][c] (rows x cols fp32, row strides lds/ldd).  impl 1 reads operands in either major, but an MN-major one is
+ * transposed on the SM every k-block: the learner stages the K-major copy of the minibatch history for its first-layer weight gradients. */
 int go1_transpose(const float* src, int lds, float* dst, int ldd, int rows, int cols, void* stream);
 /* dz = dy * ELU'(z) computed from the saved layer output y (autograd of nn.ELU). dz may alias dy. */
 int go1_elu_backward(const float* y, int ldy, const float* dy, int lddy, float* dz, int lddz, int M, int N, void* stream);

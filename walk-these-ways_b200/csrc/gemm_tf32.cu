@@ -6,7 +6,12 @@
 // dgrad (B = W as [K][N]) and wgrad (A = dz as [K][M], B = activations as [K][N]) have MN-major operands, and TF32 wgmma
 // multiplies K-major shared-memory tiles only: their TMA boxes ([32 k-rows][tile width], unswizzled) are transposed by the
 // consumer warps from shared memory to shared memory (into the 128B-swizzled K-major form, double-buffered so that the
-// transposition of k-block i + 1 overlaps the tensor-core work on k-block i); no transposed copy exists in HBM.
+// transposition of k-block i + 1 overlaps the tensor-core work on k-block i).  That costs 64 KB of shared-memory traffic per
+// 128 x 128 k-block on top of 80 KB of TMA writes and wgmma reads, plus a wait and a barrier per k-block.  The two largest
+// wgrads, the first layers' (1280 x 2105 and 256 x 2101 over M = 24576), read K-major copies instead: the history transposed once
+// per update (go1_transpose, [2105][24576] per minibatch: 207 MB each, 830 MB for the four minibatches at 4096 envs) and dz stored
+// transposed by the dgrad epilogue that produces it (store_transposed).  On an H100 SXM (700 W): 1299 -> 565 us and
+// 206 -> 137 us per launch.  The dgrads' W and the layer-2/3 wgrads are still transposed on the SM.
 // Structure (persistent CTAs, one per SM, 384 threads, walking 128 x BN output tiles):
 //   warps 0-7   two consumer warpgroups, 64 rows x BN columns each: wgmma.mma_async m64nBNk8 (4 per k-block) with the accumulator
 //               in registers, then the epilogue: accumulator -> swizzled shared memory -> one 32 x 32 block per warp at a time,
@@ -108,6 +113,7 @@ struct GemmArgs {
     int ldex, ldwex, nex, ldaux;
     int lead;                // > 0: extra columns + activation only for output columns < lead
     int amn, bmn;            // operand is MN-major in HBM (A given as [K][M], B given as [K][N]); persistent kernel only
+    int ct;                  // C is stored transposed, element (m, n) at C[n * ldc + m]: staged epilogue only (tma_store)
     float* colsum;           // optional [N]: += column sums of the values written (bias gradient fused into the dgrad epilogue)
     const float* bx; const float* bwx; float* gwx; float* dx;     // fused trailing-input backward (see Go1GemmEpilogue)
     int ldbx, ldbwx, ldgwx, lddx, nbx;
@@ -288,14 +294,22 @@ __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const C
         }
     }
     if (es.out) {           // warp-uniform: all 32 lanes stage their row (rows / columns beyond M / N are clipped by the TMA store)
-        uint8_t* srow = es.out + lane * 128;
+        if (g.ct) {         // the block of C^T: this lane's row becomes column `lane`; store j writes row j of the block, 32 lanes x 4 bytes of
+            __syncwarp();   // one 128-byte row (swizzled chunk (lane / 4) ^ (j % 8): conflict-free).  Every lane has read its row of the block.
 #pragma unroll
-        for (int j = 0; j < 8; j++)
-            *reinterpret_cast<float4*>(srow + ((j ^ (lane & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+            for (int j = 0; j < 32; j++)
+                *reinterpret_cast<float*>(es.out + j * 128 + ((((lane >> 2) ^ (j & 7)) << 4) | ((lane & 3) << 2))) = v[j];
+        } else {
+            uint8_t* srow = es.out + lane * 128;
+#pragma unroll
+            for (int j = 0; j < 8; j++)
+                *reinterpret_cast<float4*>(srow + ((j ^ (lane & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
+        }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes -> visible to the TMA (async proxy) read
         __syncwarp();
         if (lane == 0) {
-            tma_store_2d(es.mapC, es.out, col0, row);                    // lane 0's row is the block's first row
+            if (g.ct) tma_store_2d(es.mapC, es.out, row, col0);          // lane 0's row is the block's first row (the map is over C^T)
+            else tma_store_2d(es.mapC, es.out, col0, row);
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         }
         return;
@@ -535,6 +549,23 @@ int make_map_uncached(CUtensorMap* map, const float* ptr, int rows, int cols, in
                           swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { char b[96]; snprintf(b, sizeof b, "cuTensorMapEncodeTiled failed (%d)", (int)r); return go1_set_error(b); }
     return 0;
+}
+
+// Split count of a plain product: the s (with at least min_kb k-blocks per split) that minimises the wave-quantised makespan
+// ceil(tiles s / SMs) x (ceil(num_kb / s) + SPLIT_TILE_KB) in k-block times, where a tile costs about SPLIT_TILE_KB k-blocks besides its
+// main loop (pipeline fill, accumulator staging, the reduction into C).  Ties go to the smaller s (less reduction traffic).  The fused
+// first-layer weight gradient (170 tiles x 768 k-blocks) gets s = 3: 510 tiles, 3.86 of 4 waves, where s = 1 ran 1.29 waves as 2.
+int split_count(int tiles, int num_kb, int min_kb, int sms) {
+    constexpr int SPLIT_TILE_KB = 4;
+    int best = 1;
+    long long best_cost = -1;
+    for (int s = 1; s <= num_kb / (min_kb > 0 ? min_kb : 1); s++) {
+        const int kb = (num_kb + s - 1) / s;
+        if ((num_kb + kb - 1) / kb != s) continue;                  // some split would be empty
+        const long long cost = (long long)(((long long)tiles * s + sms - 1) / sms) * (kb + SPLIT_TILE_KB);
+        if (best_cost < 0 || cost < best_cost) { best = s; best_cost = cost; }
+    }
+    return best;
 }
 
 __global__ void zero_strided(float* C, int ldc, int M, int N) {
@@ -1089,27 +1120,23 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     g.C = Cm; g.bias = bias; g.M = M; g.N = N; g.K = K; g.ldc = ldc; g.act = act; g.kind = ep->act_kind; g.accumulate = accumulate;
     g.ex = ep->extra; g.ldex = ep->ld_extra; g.wex = ep->w_extra; g.ldwex = ep->ld_w_extra; g.nex = ep->extra ? ep->num_extra : 0;
     g.aux = ep->dact_y; g.ldaux = ep->ld_dact_y;
-    g.amn = amn; g.bmn = bmn; g.lead = ep->lead_cols; g.colsum = ep->colsum;
+    g.amn = amn; g.bmn = bmn; g.lead = ep->lead_cols; g.colsum = ep->colsum; g.ct = ep->store_transposed ? 1 : 0;
     g.nbx = ep->num_bwd_extra; g.bx = ep->bwd_extra; g.bwx = ep->bwd_w_extra; g.gwx = ep->g_w_extra; g.dx = ep->d_extra;
     g.ldbx = ep->ld_bwd_extra; g.ldbwx = ep->ld_bwd_w_extra; g.ldgwx = ep->ld_g_w_extra; g.lddx = ep->ld_d_extra;
     if (g.nbx < 0 || g.nbx > 4 || (g.nbx > 0 && ((g.gwx && !g.bx) || (!g.gwx && !g.dx) || (g.dx && !g.bwx)))) return go1_set_error("go1_gemm_ex: bad fused trailing-input backward arguments");
     if (g.nex < 0 || g.nex > 4) return go1_set_error("go1_gemm_ex: num_extra must be 0..4");
     if (act == 2 && !g.aux) return go1_set_error("go1_gemm_ex: act 2 needs dact_y");
+    if (g.ct && (nprob != 1 || accumulate || M < 32 || (ldc & 3) || (((uintptr_t)Cm) & 15)))      // the transposed blocks leave by TMA store only
+        return go1_set_error("go1_gemm_ex: store_transposed needs M >= 32, no accumulate and a 16-byte aligned C with ldc a multiple of 4");
     const int num_kb = (K + BK - 1) / BK;
-    // Tile selection: 128 x BN tiles, BN = the smallest of 32 / 64 / 128 that covers N (128 beyond).  Products whose tiles do not fill the SMs
-    // and whose reduction is long are split along K (partial tiles meet in C by vector reductions).
-    static const int split_ctas = getenv("GO1_TF32_SPLIT_CTAS") ? atoi(getenv("GO1_TF32_SPLIT_CTAS")) : 2 * sm_count();
+    // Tile selection: 128 x BN tiles, BN = the smallest of 32 / 64 / 128 that covers N (128 beyond).  Plain products (no fused epilogue) with a
+    // long reduction are split along K (partial tiles meet in C by vector reductions).
     static const int split_min_kb = getenv("GO1_TF32_SPLIT_MINKB") ? atoi(getenv("GO1_TF32_SPLIT_MINKB")) : 16;
     const int BN = (N > 64) ? 128 : (N > 32 ? 64 : 32);
     const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * nprob;
-    int splits = 1;
-    if (tiles < sm_count() && num_kb >= split_min_kb && g.nex == 0 && act != 2 && g.lead <= 0 && !g.colsum && g.nbx == 0) {      // split-K: about two CTA-units per SM, >= 16 k-blocks each
-        splits = (nprob > 1 ? sm_count() : split_ctas) / tiles;      // grouped: one CTA-unit per SM (fewer, longer partial sums: less same-address red traffic)
-        if (splits > num_kb / split_min_kb) splits = num_kb / split_min_kb;
-        if (splits < 1) splits = 1;
-    }
+    const bool plain = g.nex == 0 && act != 2 && g.lead <= 0 && !g.colsum && g.nbx == 0 && !g.ct;
+    const int splits = plain ? split_count(tiles, num_kb, split_min_kb, sm_count()) : 1;
     g.kb_per_split = (num_kb + splits - 1) / splits;
-    splits = (num_kb + g.kb_per_split - 1) / g.kb_per_split;
     GemmMaps gm;
     // K-major: rows = M (or N), cols = K, box BK x tile rows.  MN-major: rows = K, cols = M (or N), box tile width x BK k-rows.
     for (int p = 0; p < nprob; p++) {
@@ -1134,8 +1161,8 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     static const int use_staged = getenv("GO1_TF32_STAGED") ? atoi(getenv("GO1_TF32_STAGED")) : 1;
     CUtensorMap mc = ma, my = ma;
     g.tma_store = g.tma_aux = 0;
-    if (use_staged && nprob == 1 && splits == 1 && !accumulate && N >= 32 && (ldc & 3) == 0 && (((uintptr_t)Cm) & 15) == 0) {
-        if (int e2 = make_map(&mc, Cm, M, N, ldc, 32)) return e2;
+    if ((use_staged || g.ct) && nprob == 1 && splits == 1 && !accumulate && (g.ct ? M : N) >= 32 && (ldc & 3) == 0 && (((uintptr_t)Cm) & 15) == 0) {
+        if (int e2 = g.ct ? make_map(&mc, Cm, N, M, ldc, 32) : make_map(&mc, Cm, M, N, ldc, 32)) return e2;
         g.tma_store = 1;
         if (g.act == 2 && (g.ldaux & 3) == 0 && (((uintptr_t)g.aux) & 15) == 0) {
             if (int e2 = make_map(&my, g.aux, M, N, g.ldaux, 32)) return e2;

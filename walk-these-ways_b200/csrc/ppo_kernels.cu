@@ -265,6 +265,7 @@ extern "C" int go1_gemm_ex(int transA, int transB, int M, int N, int K, const fl
     if (impl != 0) return go1_set_error("go1_gemm: unknown impl");
     if (epi->lead_cols > 0) return go1_set_error("go1_gemm_ex: lead_cols is implemented by impl 1 only");
     if (epi->colsum || epi->num_bwd_extra > 0) return go1_set_error("go1_gemm_ex: the fused column sum / trailing-input backward are implemented by impl 1 only");
+    if (epi->store_transposed) return go1_set_error("go1_gemm_ex: store_transposed is implemented by impl 1 only");
     const float* bias = epi->bias; const int act = epi->act, kind = epi->act_kind, accumulate = epi->accumulate;
     SgemmEp ep; ep.ex = epi->extra; ep.wex = epi->w_extra; ep.aux = epi->dact_y; ep.ldex = epi->ld_extra; ep.ldwex = epi->ld_w_extra;
     ep.nex = epi->extra ? epi->num_extra : 0; ep.ldaux = epi->ld_dact_y;

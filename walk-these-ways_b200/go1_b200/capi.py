@@ -122,7 +122,8 @@ class Go1GemmEpilogue(C.Structure):
     _fields_ = [("bias", C.c_void_p), ("act", _i), ("accumulate", _i), ("extra", C.c_void_p), ("ld_extra", _i), ("w_extra", C.c_void_p),
                 ("ld_w_extra", _i), ("num_extra", _i), ("dact_y", C.c_void_p), ("ld_dact_y", _i), ("lead_cols", _i), ("colsum", C.c_void_p),
                 ("bwd_extra", C.c_void_p), ("bwd_w_extra", C.c_void_p), ("g_w_extra", C.c_void_p), ("d_extra", C.c_void_p),
-                ("ld_bwd_extra", _i), ("ld_bwd_w_extra", _i), ("ld_g_w_extra", _i), ("ld_d_extra", _i), ("num_bwd_extra", _i), ("act_kind", _i)]
+                ("ld_bwd_extra", _i), ("ld_bwd_w_extra", _i), ("ld_g_w_extra", _i), ("ld_d_extra", _i), ("num_bwd_extra", _i), ("act_kind", _i),
+                ("store_transposed", _i)]
 
 
 class Go1TailProblem(C.Structure):

@@ -45,6 +45,19 @@ def _empty(*shape, device):
         return torch.empty(*shape, device=device)
 
 
+def history_kmajor(h, priv, out):
+    """The first layers' input transposed, K-major for their weight-gradient products: out[K0 + 1 + 2E][>= M] (row pitch a multiple of
+    4 floats) gets h's K0 columns as rows 0..K0-1, ones in row K0 and priv's E columns in rows K0 + 1.. (priv None: only K0 + 1 rows).
+    Rows K0 + 1 + E.. are left for the latent, which ActorCritic.backward_ppo writes for each minibatch."""
+    M, K0 = h.shape[0], h.shape[1]
+    L, st = capi.lib(), capi.stream_ptr()
+    capi.check(L.go1_transpose(capi.ptr(h), h.stride(0), capi.ptr(out), out.stride(0), M, K0, st), "transpose")
+    out[K0, :M].fill_(1.0)
+    if priv is not None:
+        capi.check(L.go1_transpose(capi.ptr(priv), priv.stride(0), capi.ptr(out[K0 + 1:]), out.stride(0), M, priv.shape[1], st), "transpose")
+    return out
+
+
 def _aligned(t_or_ptr, ld):
     p = t_or_ptr if isinstance(t_or_ptr, int) else t_or_ptr.data_ptr()
     return (p & 15) == 0 and (ld & 3) == 0
@@ -55,9 +68,9 @@ class _Net:
 
     impl 0: every product is one fp32 CUDA-core go1_gemm.  impl 1: the large products run on the tcgen05 TF32 kernel,
     which reads its operands through TMA (16-byte aligned rows) in either major: forward K-major, dgrad with W as an
-    MN-major B operand, wgrad with dz and the layer input as MN-major A and B operands -- no transposed copies.  Only
-    the first-layer weight block W[:, :K0] (row stride 2102 floats) is packed to a TMA-readable copy, cached per
-    weight version."""
+    MN-major B operand, wgrad with dz and the layer input as MN-major A and B operands -- except the first layers' wgrad, which
+    ActorCritic runs K-major on transposed copies (history_kmajor, dz1T).  Only the first-layer weight block W[:, :K0] (row
+    stride 2102 floats) is packed to a TMA-readable copy, cached per weight version."""
 
     def __init__(self, seq, flat, grad, offsets, owner):
         self.linears = [m for m in seq if isinstance(m, nn.Linear)]
@@ -104,9 +117,10 @@ class _Net:
         return x.data_ptr() if torch.is_tensor(x) else x
 
     def _gemm(self, ta, tb, M, N, K, A, lda, B, ldb, Cm, ldc, bias=None, act=0, acc=0, impl=0, extra=None, w_extra=0, ld_w_extra=0, dact_y=None, lead_cols=0,
-              colsum=None, bwd_extra=None):
+              colsum=None, bwd_extra=None, store_transposed=0):
         ep = self._ep
         ep.lead_cols = lead_cols
+        ep.store_transposed = store_transposed
         ep.colsum = self._p(colsum) if colsum is not None else None
         if bwd_extra is not None:      # (extra [M][E], w_extra ptr, ld, g_w_extra ptr, ld, dextra [M][E] or None)
             ex, wex, ldw, gw, ldg, dex = bwd_extra
@@ -246,13 +260,13 @@ class _Net:
         q.gb3, q.gb2 = self.grad.data_ptr() + 4 * bo3, self.grad.data_ptr() + 4 * bo2
         return q, dz3, dz2
 
-    def backward(self, x, ldx, K0, extra, outs, dout, M, impl, accumulate, want_dextra=False, tag="a", dz1_out=None, aug_first=False, pre=None):
+    def backward(self, x, ldx, K0, extra, outs, dout, M, impl, accumulate, want_dextra=False, tag="a", dz1T=None, pre=None):
         """dout: gradient w.r.t. the network output [M][out] (the last layer has no activation).  Writes weight/bias grads
         into the flat grad buffer.  dz of every hidden layer comes out of the dgrad GEMM already multiplied by the
-        activation's derivative, computed from the saved layer output (fused epilogue).  dz1_out: optional [M][o1] strided view; when given the first layer's dz is written there and its wgrad is
-        left to the caller (ActorCritic fuses the three first-layer wgrads into one GEMM).  aug_first: the caller's fused wgrad also yields the first
-        layer's bias gradient and trailing-input weight gradients (augmented input columns), so the dgrad epilogue that produces the first layer's
-        dz reduces neither of them (only d(extra) if requested).  Returns d(extra) [M][E] if requested."""
+        activation's derivative, computed from the saved layer output (fused epilogue).  dz1T: optional [o1][M] strided view; when given the
+        first layer's dz is stored there transposed (K-major for the weight-gradient product) and that layer's wgrad, bias gradient and
+        trailing-input weight gradients are left to the caller (ActorCritic._first_layer_wgrad: augmented rows of the transposed input), so
+        the dgrad epilogue that produces it reduces neither of them (only d(extra) if requested).  Returns d(extra) [M][E] if requested."""
         L, st = capi.lib(), capi.stream_ptr()
         n = len(self.specs)
         dz = dout
@@ -272,7 +286,7 @@ class _Net:
             else:
                 inp, ld_in, K = outs[li - 1], outs[li - 1].stride(0), i
             prez = 1 if (accumulate or self.owner.grads_prezeroed) else 0      # the caller zeroed the gradient buffer: accumulate, no memsets
-            skinny_w = not (li == 0 and dz1_out is not None) and o <= 16 and K >= 32
+            skinny_w = not (li == 0 and dz1T is not None) and o <= 16 and K >= 32
             if not bias_done and skinny_w and K % 4 == 0 and self._tma_ok(inp, ld_in):
                 # the narrow heads: weight AND bias gradient in one bandwidth-bound pass over the layer input
                 capi.check(L.go1_skinny_wgrad_ex(capi.ptr(dz), ldz, capi.ptr(inp), ld_in, gW.data_ptr(), i, gb.data_ptr(), M, o, K, prez, st), "skinny_wgrad")
@@ -281,7 +295,7 @@ class _Net:
                 capi.check(L.go1_colsum(capi.ptr(dz), ldz, capi.ptr(gb), M, o, accumulate, st), "colsum")
             bias_done = False
             # ---- wgrad: dW[o][K] = dz^T[o][M] inp[M][K]
-            if li == 0 and dz1_out is not None:
+            if li == 0 and dz1T is not None:
                 pass                                    # fused by the caller
             elif o <= 16 and K >= 32:   # the narrow heads: one bandwidth-bound pass instead of a padded GEMM tile
                 if skinny_w:
@@ -306,7 +320,8 @@ class _Net:
                 dz, bias_done = pre[1], True            # produced (with its bias gradient) by the fused kernel
                 continue
             if li > 0:
-                dprev = dz1_out if (li == 1 and dz1_out is not None) else self._buf((tag, "d", li - 1), M, i)
+                aug = dz1T is not None and li == 1
+                dprev = dz1T if aug else self._buf((tag, "d", li - 1), M, i)
                 ldp = dprev.stride(0)
                 yprev = outs[li - 1]
                 if impl == 1 and self._tma_ok(dz, ldz) and self._tma_ok(W, i) and M >= 64:      # (the 12-wide actor head included: 19 us here, 22 us on the skinny pass)
@@ -317,7 +332,6 @@ class _Net:
                     if fuse and not accumulate and not self.owner.grads_prezeroed:
                         gb_prev.zero_()
                     bx = None
-                    aug = aug_first and li == 1
                     if aug:
                         # the first layer's bias and trailing-input weight gradients come out of the caller's fused wgrad; only d(extra) is left
                         if extra is not None and want_dextra:
@@ -337,10 +351,11 @@ class _Net:
                             dextra.zero_()
                         bx = (extra, Wp.data_ptr() + 4 * K0, pi, gWp.data_ptr() + 4 * K0, pi, dextra if want_dextra else None)
                         extra_done = True
-                    self._gemm(0, 0, M, i, o, dz, ldz, W, i, dprev, ldp, None, 2, 0, 1, dact_y=yprev, colsum=gb_prev if (fuse and not aug) else None, bwd_extra=bx)
+                    self._gemm(0, 0, M, i, o, dz, ldz, W, i, dprev, ldp, None, 2, 0, 1, dact_y=yprev, colsum=gb_prev if (fuse and not aug) else None, bwd_extra=bx,
+                               store_transposed=1 if aug else 0)
                     bias_done = bool(fuse) or aug
-                elif aug_first and li == 1:
-                    raise capi.Go1Error("augmented first-layer wgrad: the dgrad that produces the first layer's dz must be a tcgen05 product")
+                elif aug:
+                    raise capi.Go1Error("transposed first-layer dz: the dgrad that produces it must be a tensor-core product")
                 elif o <= 16:
                     pwo, pbo, po, pi = self.specs[li - 1]
                     gb_prev = self.grad[pbo:pbo + po]
@@ -687,29 +702,56 @@ class ActorCritic(nn.Module):
                 Cc = (C.c_void_p * n)(*[it[8].data_ptr() for it in chunk])
                 capi.check(L.go1_gemm_grouped(1, 0, o, K, M, n, A, ldz, B, ld_in, Cc, i, 1, st), "go1_gemm_grouped")
 
-    def backward_ppo(self, h, priv, dmean, dvalue, dstd, aug=False):
+    def _first_layers_fusable(self, h, priv):
+        """The first layers of the three nets can run their backward as one K-major product over hT (history_kmajor)."""
+        nets, K0, E = self._nets, self.num_obs_history, self.num_privileged_obs
+        return self._impl() == 1 and h.shape[0] >= 64 and _Net._tma_ok(h, h.stride(0)) and 1 <= E <= 4 and priv.shape[1] == E and \
+            nets["actor"].specs[0][3] == K0 + E and nets["critic"].specs[0][3] == K0 + E and nets["adapt"].specs[0][3] == K0
+
+    def _first_layer_wgrad(self, names, dz1T, hT, M, tag):
+        """Weight gradients of the listed nets' first layers as ONE tensor-core product with both operands K-major,
+        gcat[sum o][KA] = dz1T[sum o][M] hT[KA][M]^T (dz1T: the first-layer dz of the nets, stacked in `names` order, transposed by the
+        dgrad epilogues that made it).  The augmented rows of hT make column K0 the bias gradient and columns K0 + 1.. the trailing-input
+        weight gradients of the critic (priv) and the actor (latent); they are copied into the flat gradient buffer (overwriting)."""
+        nets, K0, E = self._nets, self.num_obs_history, self.num_privileged_obs
+        KA = hT.shape[0]
+        KP = (KA + 31) // 32 * 32
+        n0 = nets["adapt"]
+        gcat = n0._buf((tag, "gWcat"), dz1T.shape[0], KP)
+        n0._gemm(0, 1, dz1T.shape[0], KA, M, dz1T, dz1T.stride(0), hT, hT.stride(0), gcat, KP, None, 0, 0, 1)
+        row, pairs = 0, []
+        for name in names:
+            xcol = {"adapt": None, "actor": K0 + 1 + E, "critic": K0 + 1}[name]
+            wo, bo, o, i = nets[name].specs[0]
+            gW = self._grad[wo:wo + o * i].view(o, i)
+            pairs.append((gW[:, :K0], gcat[row:row + o, :K0]))
+            pairs.append((self._grad[bo:bo + o].view(o, 1), gcat[row:row + o, K0:K0 + 1]))
+            if xcol is not None:
+                pairs.append((gW[:, K0:K0 + E], gcat[row:row + o, xcol:xcol + E]))
+            row += o
+        capi.copy_segments(pairs)
+
+    def backward_ppo(self, h, priv, dmean, dvalue, dstd, aug=False, hT=None):
         """Gradients of the PPO loss into flat_grads (overwrites). h/priv are the minibatch inputs of the forward
         pass just run with tag='train'; dmean [M,A], dvalue [M,1], dstd [A].
-        aug: h is a view of a row buffer with spare columns behind the K0 history columns that the caller has filled with
-        [1 | priv (E) | anything (E)] (RolloutStorage.mini_batch_generator does).  The latent is copied into the last E and the fused
-        first-layer wgrad runs over K0 + 1 + 2E input columns: its extra output columns ARE the three first-layer bias gradients and the
-        trailing-input weight gradients of the critic (priv columns) and the actor (latent columns), for free on the tensor core, so the
-        dgrad epilogues that produce the first-layer dz skip those reductions."""
-        M, K0, impl = h.shape[0], self.num_obs_history, self._impl()
+        hT: history_kmajor(h, priv) if the caller keeps one (RolloutStorage builds it once per update); built here otherwise.  Its latent
+        rows are written here.  aug: h is a view of a row buffer with spare columns [1 | priv | latent] behind the K0 history columns;
+        the latent is copied there as well."""
+        M, K0 = h.shape[0], self.num_obs_history
         nets = self._nets
-        if impl == 1 and M >= 64 and _Net._tma_ok(h, h.stride(0)):
-            # the three first layers share their input: ONE dz [M][o_a+o_p+o_c] and ONE tensor-core wgrad
-            # dWcat[1280][2100] = dzcat^T h instead of three (the first-layer dz of each net is written straight into its
-            # column slice of `dz1` by that net's layer-2 dgrad)
+        if self._first_layers_fusable(h, priv):
+            # the three first layers share their input: ONE transposed dz [o_a+o_p+o_c][M] (each net's layer-2 dgrad stores its
+            # first-layer dz into its row slice) and ONE tensor-core wgrad with K-major operands (_first_layer_wgrad)
             oa, op, oc = nets["adapt"].specs[0][2], nets["actor"].specs[0][2], nets["critic"].specs[0][2]
-            dz1 = nets["adapt"]._buf(("train", "dz1cat"), M, oa + op + oc)
             E = self.num_privileged_obs
-            aug = bool(aug) and self.fuse_bias_grad and self.grads_prezeroed and h.stride(0) >= K0 + 1 + 2 * E and 1 <= E <= 4 and \
-                nets["actor"].specs[0][3] == K0 + E and nets["critic"].specs[0][3] == K0 + E and priv.shape[1] == E
-            KA = K0 + 1 + 2 * E if aug else K0          # input columns of the fused wgrad
-            if aug:
-                h_ext = h.as_strided((M, KA), (h.stride(0), 1))
-                capi.copy_segments([(h_ext[:, K0 + 1 + E:], self._latent)])
+            if hT is None:
+                hT = history_kmajor(h, priv, nets["adapt"]._buf(("train", "hT"), K0 + 1 + 2 * E, (M + 31) // 32 * 32))
+            L, st = capi.lib(), capi.stream_ptr()
+            capi.check(L.go1_transpose(capi.ptr(self._latent), self._latent.stride(0), capi.ptr(hT[K0 + 1 + E:]), hT.stride(0), M, E, st), "transpose")
+            if aug and h.stride(0) >= K0 + 1 + 2 * E:
+                capi.copy_segments([(h.as_strided((M, E), (h.stride(0), 1), h.storage_offset() + K0 + 1 + E), self._latent)])
+            dz1 = nets["adapt"]._buf(("train", "dz1catT"), oa + op + oc, hT.stride(0))
+            impl = 1
             if self.group_wgrads and self.grads_prezeroed:
                 self._wgrad_queue = []
             pre_p = pre_c = None
@@ -723,40 +765,38 @@ class ActorCritic(nn.Module):
             if side is not None:    # critic chain beside actor -> adaptation chain
                 self._fork(side)
                 with torch.cuda.stream(side):
-                    nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, 0, tag="train", dz1_out=dz1[:, oa + op:], aug_first=aug, pre=pre_c)
-            dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, impl, 0, want_dextra=True, tag="train", dz1_out=dz1[:, oa:oa + op],
-                                          aug_first=aug, pre=pre_p)
+                    nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, 0, tag="train", dz1T=dz1[oa + op:], pre=pre_c)
+            dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, impl, 0, want_dextra=True, tag="train", dz1T=dz1[oa:oa + op],
+                                          pre=pre_p)
             if side is None:
-                nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, 0, tag="train", dz1_out=dz1[:, oa + op:], aug_first=aug, pre=pre_c)
-            nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, 0, tag="train", dz1_out=dz1[:, :oa], aug_first=aug)
+                nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, 0, tag="train", dz1T=dz1[oa + op:], pre=pre_c)
+            nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, 0, tag="train", dz1T=dz1[:oa])
             if side is not None:
                 self._join(side)
             if self._wgrad_queue is not None:
                 self._flush_wgrads()
-            n0 = nets["adapt"]
-            KP = (KA + 31) // 32 * 32
-            gcat = n0._buf(("train", "gWcat"), oa + op + oc, KP)
-            n0._gemm(1, 0, oa + op + oc, KA, M, dz1, dz1.stride(0), h_ext if aug else h, h.stride(0), gcat, KP, None, 0, 0, 1)
-            row, pairs = 0, []
-            for name, xcol in (("adapt", None), ("actor", K0 + 1 + E), ("critic", K0 + 1)):
-                wo, bo, o, i = nets[name].specs[0]
-                gW = self._grad[wo:wo + o * i].view(o, i)
-                pairs.append((gW[:, :K0], gcat[row:row + o, :K0]))
-                if aug:     # column K0: the bias gradient; columns xcol..xcol+E: the trailing-input weight gradient of this net
-                    pairs.append((self._grad[bo:bo + o].view(o, 1), gcat[row:row + o, K0:K0 + 1]))
-                    if xcol is not None:
-                        pairs.append((gW[:, K0:K0 + E], gcat[row:row + o, xcol:xcol + E]))
-                row += o
-            capi.copy_segments(pairs)
+            self._first_layer_wgrad(("adapt", "actor", "critic"), dz1, hT, M, "train")
         else:
+            impl = self._impl()
             dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, impl, 0, want_dextra=True, tag="train")
             nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, 0, tag="train")
             nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, 0, tag="train")
         self._grad[self.std_offset:self.std_offset + self.num_actions].copy_(dstd)
 
-    def backward_adaptation(self, h, outs, dpred):
+    def backward_adaptation(self, h, outs, dpred, hT=None):
+        """Gradients of the adaptation module (overwrites its part of flat_grads).  hT: history_kmajor(h, ..) if the caller keeps one
+        (built here otherwise); the first layer's weight and bias gradients are the K-major product over its first K0 + 1 rows."""
         M, K0 = h.shape[0], self.num_obs_history
-        self._nets["adapt"].backward(h, h.stride(0), K0, None, outs, dpred, M, self._impl(), 0, tag="adapt")
+        net = self._nets["adapt"]
+        if self._impl() == 1 and M >= 64 and _Net._tma_ok(h, h.stride(0)) and net.specs[0][3] == K0:
+            if hT is None:
+                hT = history_kmajor(h, None, net._buf(("adapt", "hT"), K0 + 1, (M + 31) // 32 * 32))
+            oa = net.specs[0][2]
+            dz1 = net._buf(("adapt", "dz1T"), oa, hT.stride(0))
+            net.backward(h, h.stride(0), K0, None, outs, dpred, M, 1, 0, tag="adapt", dz1T=dz1)
+            self._first_layer_wgrad(("adapt",), dz1, hT[:K0 + 1], M, "adapt")
+        else:
+            net.backward(h, h.stride(0), K0, None, outs, dpred, M, self._impl(), 0, tag="adapt")
 
     def adaptation_forward(self, h):
         self.flatten()

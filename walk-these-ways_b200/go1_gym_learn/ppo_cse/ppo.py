@@ -222,7 +222,7 @@ class PPO:
                                       capi.ptr(dmean), ac.num_actions, capi.ptr(dvalue), capi.ptr(self._dstd), capi.ptr(self._scalars), M, ac.num_actions,
                                       PPO_Args.clip_param, PPO_Args.value_loss_coef, PPO_Args.entropy_coef, int(PPO_Args.use_clipped_value_loss),
                                       1.0 / (M * world), st()), "ppo_loss")
-            ac.backward_ppo(hist_b, priv_b, dmean, dvalue, self._dstd, aug=getattr(hist_b, "aug", False))
+            ac.backward_ppo(hist_b, priv_b, dmean, dvalue, self._dstd, hT=getattr(hist_b, "hT", None))
             # ONE collective per optimizer step: gradients (already scaled by 1/global batch) + the 8 loss scalars in the buffer head
             self._allreduce(ac.flat_grads)
             if PPO_Args.desired_kl is not None and PPO_Args.schedule == 'adaptive':   # ppo.py:118-132, on the device, from the global KL
@@ -239,7 +239,7 @@ class PPO:
                 capi.check(L.go1_ppo_mse(capi.ptr(pred), pred.stride(0), capi.ptr(priv_b), priv_b.stride(0), capi.ptr(dpred), dpred.stride(0),
                                          capi.ptr(self._mse_scalars), M, num_train, pred.shape[1], st()), "mse")
                 ac.flat_grads[ac.HEAD:ac.n_adapt_params].zero_()
-                ac.backward_adaptation(hist_b, outs, dpred)
+                ac.backward_adaptation(hist_b, outs, dpred, hT=getattr(hist_b, "hT", None))
                 if self.process_group is not None:      # adaptation gradients + the MSE pair (buffer head) in one averaging all-reduce
                     import torch.distributed as dist
                     dist.all_reduce(ac.flat_grads[:ac.n_adapt_params], op=dist.ReduceOp.AVG, group=self.process_group)

@@ -28,8 +28,9 @@ def main():
     flush = torch.empty(256 * 1024 * 1024 // 4, device="cuda")
     print(f"{'shape':>24s} {'note':>26s} {'impl0 us':>10s} {'TF/s':>7s} {'impl1 us':>10s} {'TF/s':>7s}")
     for M, N, K, note in SHAPES:
-        # operand majors as the learner issues them: wgrad reads dz / activations as [K][M] / [K][N], dgrad reads W as [K][N]
-        ta, tb = (1, 0) if "wgrad" in note else ((0, 0) if "dgrad" in note else (0, 1))
+        # operand majors as the learner issues them: wgrad reads dz / activations as [K][M] / [K][N] (the first layers' read transposed
+        # copies, K-major), dgrad reads W as [K][N]
+        ta, tb = (1, 0) if ("wgrad" in note and "L1" not in note) else ((0, 0) if "dgrad" in note else (0, 1))
         if os.environ.get("GEMM_BENCH_KMAJOR"):
             ta, tb = 0, 1
         pad = lambda n: (n + 3) // 4 * 4
