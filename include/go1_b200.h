@@ -340,28 +340,18 @@ int go1_gemm_grouped(int transA, int transB, int M, int N, int K, int nprob, con
  *   y2 = ELU(x W2^T + b2) [M][N2];   y3 = ELU(y2 W3^T + b3) [M][N3]  (N3 = 0: skipped);   out = y_last Wh^T + bh [M][nh], nh <= 16.
  * x is the first layer's activated output (K1 columns, row stride ldx); W* are torch nn.Linear weights [out][in], contiguous; y2 / y3 are
  * kept for the backward pass.  Supported tails: K1-N2-N3 = 512-256-128 (actor / critic bodies of scripts/train.py) and 256-128-0
- * (adaptation module); the activations between the layers never leave the SM (TMEM -> registers -> shared memory -> tensor core). */
+ * (adaptation module); the activations between the layers never leave the SM (wgmma accumulators in registers -> shared memory -> tensor core). */
 int go1_mlp_tail_forward(const float* x, int ldx, int M, int K1, const float* W2, const float* b2, int N2, float* y2, int ldy2,
                          const float* W3, const float* b3, int N3, float* y3, int ldy3, const float* Wh, const float* bh, int nh,
                          float* out, int ldout, void* stream);
-/* The same (ELU, or the problems' act_kind) for up to two problems of equal shape in ONE grid (the actor and critic bodies: 2 x 192 row blocks fill the 148 SMs in 3 even
- * rounds instead of 2 x 2 ragged ones).  nh <= 12 per problem. */
+/* The same (ELU, or the problems' act_kind) for up to two problems of equal shape in ONE grid (the actor and critic bodies: one CTA per SM
+ * walks the 64-row blocks of both problems, instead of two launches that each end in a partly filled round).  nh <= 12 per problem. */
 typedef struct Go1TailProblem {
     const float* x; int32_t ldx; const float* W2; const float* b2; float* y2; int32_t ldy2;
     const float* W3; const float* b3; float* y3; int32_t ldy3; const float* Wh; const float* bh; int32_t nh; float* out; int32_t ldout;
     int32_t act_kind;    /* Go1Activation in place of ELU (0 = ELU); the problems of one launch share it */
 } Go1TailProblem;
 int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int nprob, int M, int K1, int N2, int N3, void* stream);
-/* Backward of the same bodies, first half, for up to two problems in one grid (nn.Linear / nn.ELU autograd of actor_critic.py:38-77):
- *   dz3 = (dout Wh) * ELU'(y3) [M][N3];  dz2 = (dz3 W3) * ELU'(y2) [M][N2];  gb3 += colsum(dz3);  gb2 += colsum(dz2)   (N3 = 128, N2 = 256, nh <= 12)
- * dout is the gradient of the head's output [M][nh], Wh [nh][N3] and W3 [N3][N2] the nn.Linear weights, y3 / y2 the saved activations;
- * dz3 never leaves the SM between the CUDA-core product and the wgmma product.  gb3 / gb2 are accumulated with atomics. */
-typedef struct Go1TailBwdProblem {
-    const float* dout; int32_t lddout, nh; const float* Wh; const float* y3; int32_t ldy3; const float* W3; const float* y2; int32_t ldy2;
-    float* dz3; int32_t lddz3; float* dz2; int32_t lddz2; float* gb3; float* gb2;
-    int32_t act_kind;    /* Go1Activation whose derivative stands in for ELU' (0 = ELU); the problems of one launch share it */
-} Go1TailBwdProblem;
-int go1_mlp_tail_backward_grouped(const Go1TailBwdProblem* probs, int nprob, int M, int N3, int N2, void* stream);
 
 /* Per-launch timing of the impl-1 (wgmma) products for the roofline report: on = 1 starts collecting (CUDA events on the launch
  * stream around every call that is not being graph-captured), on = 0 stops and returns the summed kernel time, flops and count. */

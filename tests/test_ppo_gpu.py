@@ -411,9 +411,10 @@ def test_fused_first_layer_epilogue_lead_cols_and_extra_forward():
 
 @pytest.mark.parametrize("M", [512, 2304, 1000, 24576 + 300])      # the last one: several row blocks per CTA and a change of problem inside a CTA's sequence
 def test_fused_backward_epilogues_match_separate_kernels(M):
-    """The bias gradients (column sums of dz) and the trailing-input gradients of the first layers (go1_mlp_extra_backward) reduced
-    inside the dgrad GEMM epilogues must equal the separate bandwidth kernels: same flat gradient buffer up to the fp32 rounding of
-    a different summation order (atomics), checked against an fp64 torch-autograd gradient of the same loss as well."""
+    """The bias gradients (column sums of dz) reduced inside the dgrad epilogues (GEMM atomics, or the skinny dgrad behind a narrow
+    head) must equal the separate column-sum kernel over the dz buffer they were reduced from, up to the fp32 rounding of a different
+    summation order; the whole flat gradient buffer is checked against an fp64 torch-autograd gradient of the same loss as well."""
+    from go1_b200 import capi
     from go1_gym_learn.ppo_cse import ActorCritic
     from go1_gym_learn.ppo_cse.actor_critic import AC_Args
     AC_Args.gemm_impl = 1
@@ -426,44 +427,32 @@ def test_fused_backward_epilogues_match_separate_kernels(M):
     dmean = torch.randn(M, NA, device="cuda") / M
     dvalue = torch.randn(M, 1, device="cuda") / M
     dstd = torch.randn(NA, device="cuda")
-    grads = {}
-    for fuse in (False, True):
-        ac.fuse_bias_grad = fuse
-        ac.flat_grads.zero_(); ac.grads_prezeroed = True
-        mean, value = ac.forward_all(h, priv, tag="train")
-        ac.backward_ppo(h, priv, dmean, dvalue, dstd)
-        torch.cuda.synchronize()
-        grads[fuse] = ac.flat_grads.clone()
-        ac.grads_prezeroed = False
-    a, b = grads[False], grads[True]
+    ac.flat_grads.zero_()
+    ac.forward_all(h, priv, tag="train")
+    ac.backward_ppo(h, priv, dmean, dvalue, dstd)
+    torch.cuda.synchronize()
+    a = ac.flat_grads.clone()
     scale = a.abs().max()
-    assert float((a - b).abs().max()) <= 2e-5 * float(scale) + 1e-7, float((a - b).abs().max())
-    # augmented input columns: bias and trailing-input weight gradients of the first layers out of the fused first-layer wgrad
-    # (h lives in a row buffer with spare columns [1 | priv | latent slot] behind the history, as RolloutStorage builds it)
+    L = capi.lib()
+    for name in ("adapt", "actor", "critic"):
+        net = ac._nets[name]
+        for k in range(1, len(net.specs) - 1):          # the hidden layers behind the first one: their dz stays in a buffer of _Net
+            dz = net.acts[("train", "d", k)][:M]
+            _, bo, o, _ = net.specs[k]
+            want = torch.empty(o, device="cuda")
+            capi.check(L.go1_colsum(capi.ptr(dz), dz.stride(0), capi.ptr(want), M, o, 0, capi.stream_ptr()), "colsum")
+            err = float((a[bo:bo + o] - want).abs().max())
+            assert err <= 2e-5 * float(scale) + 1e-7, (name, k, err)
+    # h as a view of a row buffer with a 2112-float pitch, the minibatch layout of RolloutStorage: same products, another order of the atomic sums
     hb = torch.zeros(M, NH + 12, device="cuda")
-    hb[:, :NH] = h; hb[:, NH] = 1.0; hb[:, NH + 1:NH + 1 + NP] = priv
+    hb[:, :NH] = h
     h2 = hb[:, :NH]
-    ac.fuse_bias_grad = True
-    ac.flat_grads.zero_(); ac.grads_prezeroed = True
+    ac.flat_grads.zero_()
     ac.forward_all(h2, priv, tag="train")
-    ac.backward_ppo(h2, priv, dmean, dvalue, dstd, aug=True)
+    ac.backward_ppo(h2, priv, dmean, dvalue, dstd)
     torch.cuda.synchronize()
-    c = ac.flat_grads.clone()
-    ac.grads_prezeroed = False
-    assert torch.equal(hb[:, NH + 1 + NP:NH + 1 + 2 * NP], ac._latent)          # the latent slot was filled
-    # TF32 products instead of fp32 reductions for these few gradients: compare at TF32 accuracy against the fp32-reduced ones
-    assert float((a - c).abs().max()) <= 3e-3 * float(scale) + 1e-7, float((a - c).abs().max())
-    # first half of the bodies' backward tails in one launch (go1_mlp_tail_backward_grouped): same operands, same products -> same gradients
-    # up to the order of the atomic bias-gradient sums
-    ac.fuse_tail_bwd = True
-    ac.flat_grads.zero_(); ac.grads_prezeroed = True
-    ac.forward_all(h2, priv, tag="train")
-    ac.backward_ppo(h2, priv, dmean, dvalue, dstd, aug=True)
-    torch.cuda.synchronize()
-    d = ac.flat_grads.clone()
-    ac.grads_prezeroed = False; ac.fuse_tail_bwd = False
-    assert float((c - d).abs().max()) <= 2e-5 * float(scale) + 1e-7, float((c - d).abs().max())
-    b = d
+    b = ac.flat_grads.clone()
+    assert float((a - b).abs().max()) <= 3e-3 * float(scale) + 1e-7, float((a - b).abs().max())
     # fp64 autograd of sum(mean * dmean) + sum(value * dvalue) through plain torch modules holding the same weights
     import copy
     ref = {k: copy.deepcopy(getattr(ac, k)).double() for k in ("adaptation_module", "actor_body", "critic_body")}

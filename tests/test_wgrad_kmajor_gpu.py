@@ -84,11 +84,10 @@ def test_kmajor_first_layer_wgrad_matches_autograd(M):
     priv = torch.randn(M, NP, device="cuda")
     hT = history_kmajor(h, priv, torch.empty(NH + 1 + 2 * NP, (M + 31) // 32 * 32, device="cuda"))
     dmean, dvalue, dstd = torch.randn(M, NA, device="cuda") / M, torch.randn(M, 1, device="cuda") / M, torch.randn(NA, device="cuda")
-    ac.flat_grads.zero_(); ac.grads_prezeroed = True
     ac.forward_all(h, priv, tag="train")
+    ac.flat_grads.fill_(3.0)                                     # overwritten, not accumulated into
     ac.backward_ppo(h, priv, dmean, dvalue, dstd, hT=hT)
     torch.cuda.synchronize()
-    ac.grads_prezeroed = False
     g = ac.flat_grads.clone()
     assert torch.equal(hT[NH + 1 + NP:, :M].t(), ac._latent)     # the latent rows were written
     ref = {k: copy.deepcopy(getattr(ac, k)).double() for k in ("adaptation_module", "actor_body", "critic_body")}

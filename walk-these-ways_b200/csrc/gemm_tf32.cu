@@ -117,7 +117,7 @@ struct GemmArgs {
     float* colsum;           // optional [N]: += column sums of the values written (bias gradient fused into the dgrad epilogue)
     const float* bx; const float* bwx; float* gwx; float* dx;     // fused trailing-input backward (see Go1GemmEpilogue)
     int ldbx, ldbwx, ldgwx, lddx, nbx;
-    int tma_store, tma_aux;  // staged epilogue (persistent kernel, STAGED): C blocks leave / derivative operand blocks arrive through shared memory by TMA
+    int tma_store, tma_aux;  // staged epilogue: C blocks leave / derivative operand blocks arrive through shared memory by TMA
     // grouped launch (persistent kernel): nprob problems of the same shape and operand strides in one grid; tile t belongs to problem
     // t / tiles_per_prob, whose operands are maps.a/b[p] and whose output is Cg[p] (no per-problem epilogue operands: split-K wgrads)
     float* Cg[4]; int nprob, tiles_per_prob;
@@ -166,6 +166,22 @@ __device__ __forceinline__ void epilogue_dact(const D dact, const GemmArgs& g, f
 #pragma unroll
         for (int j = 0; j < 32; j++) if (j < ncols) v[j] *= dact(__ldg(arow + j));
     }
+}
+
+// Column sums of a 32 x 32 block held one row per lane (sred[j] = column j; overwritten) by a transpose-reduce: 31 shuffles for 32
+// columns (each halving step trades half of the columns for the partner's partial sums).  Lane l ends up with column l.
+__device__ __forceinline__ float transpose_reduce32(float (&sred)[32], const int lane) {
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) {
+        const bool upper = (lane & off) != 0;
+#pragma unroll
+        for (int j = 0; j < off; j++) {
+            const float send = upper ? sred[j] : sred[j + off];
+            const float keep = upper ? sred[j + off] : sred[j];
+            sred[j] = keep + __shfl_xor_sync(0xffffffffu, send, off);
+        }
+    }
+    return sred[0];
 }
 
 // Epilogue of one 32-column chunk held in registers (thread = output row, r[j] = column col0 + j).  Called by all 32 lanes
@@ -245,21 +261,12 @@ __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const C
         else epilogue_dact([](float y) { return act_deriv<GO1_ACT_ELU>(y); }, g, v, row, col0, ncols, lane, ypre, have_pre, es);
     }
     }
-    if (g.colsum) {         // warp-uniform.  Column sums over the warp's 32 rows by a transpose-reduce: 31 shuffles for 32 columns
-        float sred[32];     // (each halving step trades half of the columns for the partner's partial sums), then one atomic per lane
+    if (g.colsum) {         // warp-uniform.  Column sums over the warp's 32 rows, then one atomic per lane
+        float sred[32];
 #pragma unroll
         for (int j = 0; j < 32; j++) sred[j] = (row_ok && j < ncols) ? v[j] : 0.f;
-#pragma unroll
-        for (int off = 16; off >= 1; off >>= 1) {
-            const bool upper = (lane & off) != 0;
-#pragma unroll
-            for (int j = 0; j < off; j++) {
-                const float send = upper ? sred[j] : sred[j + off];
-                const float keep = upper ? sred[j + off] : sred[j];
-                sred[j] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-            }
-        }
-        if (lane < ncols) atomicAdd(g.colsum + col0 + lane, sred[0]);      // lane l ends up with column col0 + l
+        const float s = transpose_reduce32(sred, lane);
+        if (lane < ncols) atomicAdd(g.colsum + col0 + lane, s);
     }
     if (g.nbx > 0) {        // warp-uniform.  C is the dz of a first layer with nbx trailing inputs: their weight gradient (column sums weighted by the
         const int cjx = col0 + lane;                     // row's trailing inputs) and input gradient (row dots with the trailing-input weights)
@@ -271,17 +278,8 @@ __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const C
                 float sred[32];
 #pragma unroll
                 for (int j = 0; j < 32; j++) sred[j] = (row_ok && j < ncols) ? v[j] * e : 0.f;
-#pragma unroll
-                for (int off = 16; off >= 1; off >>= 1) {
-                    const bool upper = (lane & off) != 0;
-#pragma unroll
-                    for (int j = 0; j < off; j++) {
-                        const float send = upper ? sred[j] : sred[j + off];
-                        const float keep = upper ? sred[j + off] : sred[j];
-                        sred[j] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-                    }
-                }
-                if (lane < ncols) atomicAdd(g.gwx + (size_t)cjx * g.ldgwx + t, sred[0]);
+                const float s = transpose_reduce32(sred, lane);
+                if (lane < ncols) atomicAdd(g.gwx + (size_t)cjx * g.ldgwx + t, s);
                 }
                 if (g.dx) {
                     const float wl = lane < ncols ? __ldg(g.bwx + (size_t)cjx * g.ldbwx + t) : 0.f;
@@ -341,7 +339,7 @@ __device__ __forceinline__ bool epilogue_prefetch(const GemmArgs& g, const int r
 // as the accumulator / output staging (32 KB per warpgroup).
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int X_BYTES = 65536;
-template <int BN, bool STAGED, bool ANYKIND>
+template <int BN, bool ANYKIND>
 __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __grid_constant__ GemmMaps gm,
                                                                       const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
                                                                       const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
@@ -353,7 +351,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
     uint8_t* ring = base;
     uint8_t* xreg = base + (size_t)stages * STAGE_BYTES;
     uint8_t* stage_aux = xreg + X_BYTES;
-    uint64_t* full = (uint64_t*)(stage_aux + ((STAGED && g.tma_aux) ? NCONS * 4096 : 0));
+    uint64_t* full = (uint64_t*)(stage_aux + (g.tma_aux ? NCONS * 4096 : 0));
     uint64_t* empty = full + MAX_STAGES;
     uint64_t* aux_bar = empty + MAX_STAGES;      // [NCONS]
 
@@ -365,8 +363,8 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
             asm volatile("prefetch.tensormap [%0];" ::"l"(&gm.a[p]) : "memory");
             asm volatile("prefetch.tensormap [%0];" ::"l"(&gm.b[p]) : "memory");
         }
-        if (STAGED && g.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"(&mapC) : "memory");
-        if (STAGED && g.tma_aux) asm volatile("prefetch.tensormap [%0];" ::"l"(&mapY) : "memory");
+        if (g.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"(&mapC) : "memory");
+        if (g.tma_aux) asm volatile("prefetch.tensormap [%0];" ::"l"(&mapY) : "memory");
         for (int s = 0; s < stages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], NCONS); }
         for (int w = 0; w < NCONS; w++) mbar_init(&aux_bar[w], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -412,7 +410,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
     const int q = 2 * wgi + (w & 1), grp = w >> 1;      // epilogue: 32-row block q of the tile, column group grp
     const bool tr = g.amn || g.bmn;
     const bool split = g.kb_per_split < num_kb_total;
-    const bool st_out = STAGED && g.tma_store, st_aux = STAGED && g.tma_aux;
+    const bool st_out = g.tma_store, st_aux = g.tma_aux;
     uint8_t* xwg = xreg + wgi * (X_BYTES / 2);          // this warpgroup's accumulator staging: [chunk][64 rows][128 B]
     uint8_t* my_aux = stage_aux + warp * 4096;
     uint64_t* my_bar = &aux_bar[warp];
@@ -583,10 +581,10 @@ __global__ void bias_act_strided(float* C, int ldc, const float* bias, int M, in
     *c = v;
 }
 
-template <int BN, bool STAGED, bool ANYKIND>
+template <int BN, bool ANYKIND>
 int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st) {
     constexpr int STAGE_BYTES = (BM + BN) * BK * 4;
-    const size_t staging = X_BYTES + ((STAGED && g.tma_aux) ? (size_t)NCONS * 4096 : 0);
+    const size_t staging = X_BYTES + (g.tma_aux ? (size_t)NCONS * 4096 : 0);
     const size_t fixed = staging + (2 * 8 + NCONS) * 8 + 16 + 1024;
     const size_t budget = 227 * 1024;
     int stages = (int)((budget - fixed) / STAGE_BYTES);
@@ -595,7 +593,7 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
     const size_t smem = (size_t)stages * STAGE_BYTES + fixed;
     static bool configured = false;
     if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tf32_wgmma<BN, STAGED, ANYKIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget);
+        cudaError_t e = cudaFuncSetAttribute(gemm_tf32_wgmma<BN, ANYKIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget);
         if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
         configured = true;
     }
@@ -604,7 +602,7 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
     const int total = g.tiles_per_prob * (g.nprob > 1 ? g.nprob : 1);
     const int sms = sm_count();
     const int grid = total < sms ? total : sms;          // one CTA per SM (the ring and the staging fill its shared memory)
-    gemm_tf32_wgmma<BN, STAGED, ANYKIND><<<grid, 32 * NCONS + 128, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages);
+    gemm_tf32_wgmma<BN, ANYKIND><<<grid, 32 * NCONS + 128, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages);
     go1_count_launch(1);
     return 0;
 }
@@ -860,211 +858,6 @@ int launch_tail(const TailMaps& maps, const TailArgs& g, cudaStream_t st) {
     return 0;
 }
 
-// ---------------------------------------------------------------------------------------------------------------
-// Fused MLP tail, backward (first half): for the bodies 512-256-128-head (actor_critic.py:38-77), from the gradient of the head's output,
-//     dz3 = (dout Wh) * f'(y3)     [M][128]     CUDA cores: K = nh <= 12
-//     dz2 = (dz3 W3) * f'(y2)      [M][256]     tensor core: A = the dz3 tile the consumer warps laid out in shared memory, B = W3 (resident)
-// plus the bias gradients gb3 = colsum(dz3), gb2 = colsum(dz2), for up to two problems (actor + critic) in one grid.  This replaces, per
-// body, a skinny dgrad launch and a 24576 x 256 x 128 dgrad launch (which re-reads dz3 from memory and whose tiles are too short to hide
-// their epilogue): dz3 never leaves the SM between the two products.  The wgrads (dz3^T y2, dz2^T y1) and the last dgrad (dz1) stay
-// separate products.  One CTA (384 threads) per 64-row block:
-//   warp 8      loads W3 ([K = 128][N = 256], MN-major) as four unswizzled [32][256] boxes whenever the CTA meets a new problem
-//   warps 0-7   transpose those boxes into the resident K-major operand (128 KB); per block: E0, warp = (32-row half, 32-column chunk),
-//               builds a dz3 chunk from dout, Wh (shared memory) and y3, writes it swizzled into the A tile and sends it to global memory
-//               by TMA; then warpgroup g multiplies the tile by columns [128 g, 128 g + 128) of W3 (16 wgmma) and E1 multiplies the
-//               accumulator fragments by f'(y2) and stores dz2 from registers.
-// Column sums meet in shared memory (atomics) and are flushed once per CTA.
-// ---------------------------------------------------------------------------------------------------------------
-struct TailBwdProb { const float* dout; const float* Wh; const float* y3; const float* y2; float* dz2; float* gb3; float* gb2; int lddout, nh, ldy3, ldy2, lddz2; };
-struct TailBwdArgs { TailBwdProb p[TAIL_MAXP]; int nprob, M, tiles_per_prob, tiles, kind; };
-struct TailBwdMaps { CUtensorMap w3[TAIL_MAXP], dz3[TAIL_MAXP]; };
-constexpr int TB_N3 = 128, TB_N2 = 256;
-constexpr int TB_W3_BYTES = TB_N3 * TB_N2 * 4;                 // 128 KB: 4 k-blocks x [256 n][32 k]
-constexpr int TB_RAW_BYTES = BK * TB_N2 * 4;                   // 32 KB: one box [32 k][256 n]
-constexpr int TB_Z3_BYTES = TAIL_BM * TB_N3 * 4;               // 32 KB: 4 k-blocks x [64 rows][32 floats]
-constexpr int TB_SMEM = TB_W3_BYTES + TB_RAW_BYTES + TB_Z3_BYTES + (TAIL_MAXP * TAIL_HPW * TB_N3 + TAIL_MAXP * (TB_N3 + TB_N2)) * 4 + 2 * 8 + 16 + 1024;
-
-// column sums of a 32 x 32 block held one row per lane (v[j] = column j): 31 shuffles; lane l ends up with column l
-__device__ __forceinline__ float warp_colsum32(const float (&v)[32], const int lane) {
-    float sred[32];
-#pragma unroll
-    for (int j = 0; j < 32; j++) sred[j] = v[j];
-#pragma unroll
-    for (int off = 16; off >= 1; off >>= 1) {
-        const bool upper = (lane & off) != 0;
-#pragma unroll
-        for (int j = 0; j < off; j++) {
-            const float send = upper ? sred[j] : sred[j + off];
-            const float keep = upper ? sred[j + off] : sred[j];
-            sred[j] = keep + __shfl_xor_sync(0xffffffffu, send, off);
-        }
-    }
-    return sred[0];
-}
-
-template <typename D>
-__device__ __forceinline__ void mlp_tail_bwd_body(const TailBwdMaps& maps, const TailBwdArgs& g, const D dact) {
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t* base = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-    uint8_t* w3s = base;                                     // B operand: [4 k-blocks][256 n][32 k], 128B-swizzled
-    uint8_t* raw = base + TB_W3_BYTES;                       // one W3 box as TMA delivers it
-    uint8_t* z3 = raw + TB_RAW_BYTES;                        // A operand: [4 k-blocks][64 rows][32 floats], 128B-swizzled
-    float* s_wh = (float*)(z3 + TB_Z3_BYTES);                // [MAXP][HPW][128]
-    float* s_cs = s_wh + TAIL_MAXP * TAIL_HPW * TB_N3;       // [MAXP][128 + 256] column sums (bias gradients)
-    uint64_t* raw_full = (uint64_t*)(s_cs + TAIL_MAXP * (TB_N3 + TB_N2));
-    uint64_t* raw_free = raw_full + 1;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (threadIdx.x == 0) {
-        for (int p = 0; p < g.nprob; p++) {
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.w3[p]) : "memory");
-            asm volatile("prefetch.tensormap [%0];" ::"l"(&maps.dz3[p]) : "memory");
-        }
-        mbar_init(raw_full, 1); mbar_init(raw_free, NCONS);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    for (int i = threadIdx.x; i < TAIL_MAXP * TAIL_HPW * TB_N3; i += blockDim.x) {
-        const int p = i / (TAIL_HPW * TB_N3), r = (i / TB_N3) % TAIL_HPW, k = i % TB_N3;
-        s_wh[i] = (p < g.nprob && r < g.p[p].nh) ? __ldg(g.p[p].Wh + (size_t)r * TB_N3 + k) : 0.f;
-    }
-    for (int i = threadIdx.x; i < TAIL_MAXP * (TB_N3 + TB_N2); i += blockDim.x) s_cs[i] = 0.f;
-    __syncthreads();
-
-    if (warp == NCONS) {
-        // ===== W3 loader: one box at a time, for every new problem among this CTA's blocks (the consumers follow the same sequence) =====
-        if (elect_one()) {
-            int cur = -1, nbox = 0;
-            for (int t = blockIdx.x; t < g.tiles; t += gridDim.x) {
-                const int p = t / g.tiles_per_prob;
-                if (p == cur) continue;
-                cur = p;
-                for (int kb = 0; kb < TB_N3 / BK; kb++, nbox++) {
-                    mbar_wait(raw_free, (nbox & 1) ^ 1);
-                    mbar_expect_tx(raw_full, TB_RAW_BYTES);
-                    tma_load_2d(&maps.w3[p], raw_full, raw, 0, kb * BK);
-                }
-            }
-        }
-        return;
-    }
-    if (warp > NCONS) return;
-
-    // ===== consumers =====
-    const int wgi = warp >> 2, w = warp & 3, ctid = threadIdx.x;
-    const int h = warp & 1, cg = warp >> 1;                             // E0: rows 32 h .. 32 h + 31 of the block, dz3 columns 32 cg .. 32 cg + 31
-    uint8_t* myblk = z3 + (size_t)cg * (TAIL_BM * 128) + h * 4096;
-    const int rA = 16 * w + (lane >> 2);                                // E1: this thread's fragment rows rA and rA + 8
-    int cur = -1, nbox = 0;
-    for (int t = blockIdx.x; t < g.tiles; t += gridDim.x) {
-        const int p = t / g.tiles_per_prob, m0 = (t - p * g.tiles_per_prob) * TAIL_BM;
-        const TailBwdProb& pr = g.p[p];
-        float* cs = s_cs + p * (TB_N3 + TB_N2);
-        if (p != cur) {      // the previous problem's products are complete (end-of-block barrier): bring this problem's W3 into K-major form
-            cur = p;
-            for (int kb = 0; kb < TB_N3 / BK; kb++, nbox++) {
-                mbar_wait(raw_full, nbox & 1);
-                transpose_tile<TB_N2>((const float*)raw, w3s + (size_t)kb * (TB_N2 * 128), ctid);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(raw_free);
-            }
-        }
-        // ---- E0: dz3 chunk cg = (dout Wh)[.., 32 cg ..] * f'(y3)
-        {
-            const int row = m0 + 32 * h + lane;
-            const bool row_ok = row < g.M;
-            float4 y[8];
-            const float4* yrow = reinterpret_cast<const float4*>(pr.y3 + (size_t)(row_ok ? row : 0) * pr.ldy3 + 32 * cg);
-#pragma unroll
-            for (int j = 0; j < 8; j++) y[j] = __ldg(yrow + j);
-            float d[TAIL_HPW];
-#pragma unroll
-            for (int n = 0; n < TAIL_HPW; n++) d[n] = (row_ok && n < pr.nh) ? __ldg(pr.dout + (size_t)row * pr.lddout + n) : 0.f;
-            float v[32];
-#pragma unroll
-            for (int j = 0; j < 32; j++) v[j] = 0.f;
-            const float* wh = s_wh + (size_t)p * TAIL_HPW * TB_N3 + 32 * cg;
-#pragma unroll
-            for (int n = 0; n < TAIL_HPW; n++) {
-                if (n < pr.nh) {
-                    const float4* wv = reinterpret_cast<const float4*>(wh + n * TB_N3);
-#pragma unroll
-                    for (int j = 0; j < 8; j++) {
-                        const float4 ww = wv[j];
-                        v[4 * j] = fmaf(d[n], ww.x, v[4 * j]); v[4 * j + 1] = fmaf(d[n], ww.y, v[4 * j + 1]);
-                        v[4 * j + 2] = fmaf(d[n], ww.z, v[4 * j + 2]); v[4 * j + 3] = fmaf(d[n], ww.w, v[4 * j + 3]);
-                    }
-                }
-            }
-#pragma unroll
-            for (int j = 0; j < 8; j++) {
-                v[4 * j] *= dact(y[j].x); v[4 * j + 1] *= dact(y[j].y);
-                v[4 * j + 2] *= dact(y[j].z); v[4 * j + 3] *= dact(y[j].w);
-            }
-            if (!row_ok) {
-#pragma unroll
-                for (int j = 0; j < 32; j++) v[j] = 0.f;
-            }
-            const float c3 = warp_colsum32(v, lane);
-            atomicAdd(cs + 32 * cg + lane, c3);
-            uint8_t* trow = myblk + (size_t)lane * 128;
-#pragma unroll
-            for (int j = 0; j < 8; j++)
-                *reinterpret_cast<float4*>(trow + ((j ^ (lane & 7)) << 4)) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-            fence_async_smem();
-            __syncwarp();
-            if (lane == 0) {
-                tma_store_2d(&maps.dz3[p], myblk, 32 * cg, m0 + 32 * h);
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            }
-        }
-        cons_sync();                                                    // the dz3 tile (and, for a new problem, W3) is in shared memory
-        // ---- the product and E1: dz2 columns [128 wgi, 128 wgi + 128) = accumulator * f'(y2)
-        {
-            float acc[64];
-            wg::fence();
-#pragma unroll
-            for (int kb = 0; kb < TB_N3 / BK; kb++)
-                wg::mma_kblock<128>(acc, z3 + (size_t)kb * (TAIL_BM * 128), w3s + (size_t)kb * (TB_N2 * 128) + (size_t)wgi * 128 * 128, kb > 0);
-            wg::commit();
-            wg::wait<0>();
-            const bool ok0 = m0 + rA < g.M, ok1 = m0 + rA + 8 < g.M;
-            const float* y0 = pr.y2 + (size_t)(ok0 ? m0 + rA : 0) * pr.ldy2;
-            const float* y1 = pr.y2 + (size_t)(ok1 ? m0 + rA + 8 : 0) * pr.ldy2;
-#pragma unroll
-            for (int j = 0; j < 16; j++) {
-                const int col = 128 * wgi + 8 * j + 2 * (lane & 3);
-                const float2 ya = __ldg(reinterpret_cast<const float2*>(y0 + col)), yb = __ldg(reinterpret_cast<const float2*>(y1 + col));
-                float2 va = make_float2(acc[4 * j] * dact(ya.x), acc[4 * j + 1] * dact(ya.y));
-                float2 vb = make_float2(acc[4 * j + 2] * dact(yb.x), acc[4 * j + 3] * dact(yb.y));
-                if (!ok0) va = make_float2(0.f, 0.f);
-                if (!ok1) vb = make_float2(0.f, 0.f);
-                if (ok0) *reinterpret_cast<float2*>(pr.dz2 + (size_t)(m0 + rA) * pr.lddz2 + col) = va;
-                if (ok1) *reinterpret_cast<float2*>(pr.dz2 + (size_t)(m0 + rA + 8) * pr.lddz2 + col) = vb;
-                float sx = va.x + vb.x, sy = va.y + vb.y;              // column sums over the warp's 16 rows: lanes with equal lane % 4 share columns
-#pragma unroll
-                for (int off = 4; off <= 16; off <<= 1) { sx += __shfl_xor_sync(0xffffffffu, sx, off); sy += __shfl_xor_sync(0xffffffffu, sy, off); }
-                if (lane < 4) { atomicAdd(cs + TB_N3 + col, sx); atomicAdd(cs + TB_N3 + col + 1, sy); }
-            }
-        }
-        // the dz3 tile is rewritten by the next block: its TMA stores have read it, both warpgroups' products are complete
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-        cons_sync();
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    cons_sync();
-    // bias gradients: one set of atomics per CTA
-    for (int i = ctid; i < g.nprob * (TB_N3 + TB_N2); i += 32 * NCONS) {
-        const int p = i / (TB_N3 + TB_N2), c = i - p * (TB_N3 + TB_N2);
-        const float vsum = s_cs[p * (TB_N3 + TB_N2) + c];
-        if (vsum != 0.f) atomicAdd(c < TB_N3 ? g.p[p].gb3 + c : g.p[p].gb2 + (c - TB_N3), vsum);
-    }
-}
-template <bool ANYKIND>
-__global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_bwd_kernel(const __grid_constant__ TailBwdMaps maps, const TailBwdArgs g) {
-    if (ANYKIND) mlp_tail_bwd_body(maps, g, act_deriv_coefficients(g.kind));
-    else mlp_tail_bwd_body(maps, g, [](float y) { return act_deriv<GO1_ACT_ELU>(y); });
-}
-
 }  // namespace
 
 // ---- optional per-launch timing of the tensor-core GEMM (bench.py's roofline): CUDA events on the launch stream around every
@@ -1094,7 +887,7 @@ extern "C" int go1_gemm_timing(int on, double* total_ms, double* total_flop, lon
         if (csv && i / 2 < g_time_recs.size()) {
             const TimeRec& r = g_time_recs[i / 2];
             fprintf(csv, "%d,%d,%d,%d,%d,%d,%d,%d,%s,%d,%.2f\n", r.M, r.N, r.K, r.amn, r.bmn, r.act, r.nex, r.splits,
-                    r.kern >= 1000 ? (r.kern == 1004 ? "tailbwd" : (r.kern == 1003 ? "tail3" : "tail2")) : (r.kern == 128 ? "p128" : (r.kern == 64 ? "p64" : "p32")), r.colsum, 1e3 * t);
+                    r.kern >= 1000 ? (r.kern == 1003 ? "tail3" : "tail2") : (r.kern == 128 ? "p128" : (r.kern == 64 ? "p64" : "p32")), r.colsum, 1e3 * t);
         }
     }
     if (csv) fclose(csv);
@@ -1131,11 +924,11 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     const int num_kb = (K + BK - 1) / BK;
     // Tile selection: 128 x BN tiles, BN = the smallest of 32 / 64 / 128 that covers N (128 beyond).  Plain products (no fused epilogue) with a
     // long reduction are split along K (partial tiles meet in C by vector reductions).
-    static const int split_min_kb = getenv("GO1_TF32_SPLIT_MINKB") ? atoi(getenv("GO1_TF32_SPLIT_MINKB")) : 16;
+    constexpr int SPLIT_MIN_KB = 16;          // least k-blocks per split
     const int BN = (N > 64) ? 128 : (N > 32 ? 64 : 32);
     const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * nprob;
     const bool plain = g.nex == 0 && act != 2 && g.lead <= 0 && !g.colsum && g.nbx == 0 && !g.ct;
-    const int splits = plain ? split_count(tiles, num_kb, split_min_kb, sm_count()) : 1;
+    const int splits = plain ? split_count(tiles, num_kb, SPLIT_MIN_KB, sm_count()) : 1;
     g.kb_per_split = (num_kb + splits - 1) / splits;
     GemmMaps gm;
     // K-major: rows = M (or N), cols = K, box BK x tile rows.  MN-major: rows = K, cols = M (or N), box tile width x BK k-rows.
@@ -1157,11 +950,11 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
         g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, BN, g.colsum ? 1 : 0});
     }
     int e;
-    // staged epilogue: C blocks leave the accumulator staging by TMA store, the derivative operand arrives through TMA loads
-    static const int use_staged = getenv("GO1_TF32_STAGED") ? atoi(getenv("GO1_TF32_STAGED")) : 1;
+    // staged epilogue: C blocks leave the accumulator staging by TMA store, the derivative operand arrives through TMA loads.  The direct
+    // row-per-lane stores serve the rest: split-K partial tiles, accumulate, grouped launches, N < 32 and a misaligned C.
     CUtensorMap mc = ma, my = ma;
     g.tma_store = g.tma_aux = 0;
-    if ((use_staged || g.ct) && nprob == 1 && splits == 1 && !accumulate && (g.ct ? M : N) >= 32 && (ldc & 3) == 0 && (((uintptr_t)Cm) & 15) == 0) {
+    if (nprob == 1 && splits == 1 && !accumulate && (g.ct ? M : N) >= 32 && (ldc & 3) == 0 && (((uintptr_t)Cm) & 15) == 0) {
         if (int e2 = g.ct ? make_map(&mc, Cm, N, M, ldc, 32) : make_map(&mc, Cm, M, N, ldc, 32)) return e2;
         g.tma_store = 1;
         if (g.act == 2 && (g.ldaux & 3) == 0 && (((uintptr_t)g.aux) & 15) == 0) {
@@ -1170,9 +963,9 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
         }
     }
     const bool any = g.act != 0 && g.kind != GO1_ACT_ELU;
-    if (BN == 128) e = any ? launch_gemm<128, true, true>(gm, mc, my, g, splits, st) : launch_gemm<128, true, false>(gm, mc, my, g, splits, st);
-    else if (BN == 64) e = any ? launch_gemm<64, true, true>(gm, mc, my, g, splits, st) : launch_gemm<64, true, false>(gm, mc, my, g, splits, st);
-    else e = any ? launch_gemm<32, true, true>(gm, mc, my, g, splits, st) : launch_gemm<32, true, false>(gm, mc, my, g, splits, st);
+    if (BN == 128) e = any ? launch_gemm<128, true>(gm, mc, my, g, splits, st) : launch_gemm<128, false>(gm, mc, my, g, splits, st);
+    else if (BN == 64) e = any ? launch_gemm<64, true>(gm, mc, my, g, splits, st) : launch_gemm<64, false>(gm, mc, my, g, splits, st);
+    else e = any ? launch_gemm<32, true>(gm, mc, my, g, splits, st) : launch_gemm<32, false>(gm, mc, my, g, splits, st);
     if (e) return e;
     if (splits > 1 && (bias || act))
         for (int p = 0; p < nprob; p++) { const size_t tot = (size_t)M * N; bias_act_strided<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cs[p], ldc, bias, M, N, act, ep->act_kind); go1_count_launch(1); }
@@ -1277,55 +1070,4 @@ extern "C" int go1_mlp_tail_forward(const float* x, int ldx, int M, int K1, cons
     Go1TailProblem q = {};
     q.x = x; q.ldx = ldx; q.W2 = W2; q.b2 = b2; q.y2 = y2; q.ldy2 = ldy2; q.W3 = W3; q.b3 = b3; q.y3 = y3; q.ldy3 = ldy3; q.Wh = Wh; q.bh = bh; q.nh = nh; q.out = out; q.ldout = ldout;
     return go1_mlp_tail_forward_grouped(&q, 1, M, K1, N2, N3, stream);
-}
-
-// ---- fused MLP tail (backward, first half), see mlp_tail_bwd_kernel
-extern "C" int go1_mlp_tail_backward_grouped(const Go1TailBwdProblem* probs, int nprob, int M, int N3, int N2, void* stream) {
-    cudaStream_t st = (cudaStream_t)stream;
-    if (!probs || nprob < 1 || nprob > TAIL_MAXP || M <= 0) return go1_set_error("go1_mlp_tail_backward: 1 or 2 problems of the same shape");
-    if (N3 != TB_N3 || N2 != TB_N2) return go1_set_error("go1_mlp_tail_backward: the supported tail is ...-256-128-head");
-    TailBwdMaps maps;
-    TailBwdArgs g;
-    g.nprob = nprob; g.M = M; g.tiles_per_prob = (M + TAIL_BM - 1) / TAIL_BM; g.tiles = g.tiles_per_prob * nprob;
-    g.kind = probs[0].act_kind;
-    if (!go1_act_kind_ok(g.kind)) return go1_set_error("go1_mlp_tail_backward: unknown activation kind (Go1Activation)");
-    for (int p = 0; p < nprob; p++) {
-        const Go1TailBwdProblem& q = probs[p];
-        if (q.act_kind != g.kind) return go1_set_error("go1_mlp_tail_backward: the problems of one launch share their activation kind");
-        if (!q.dout || !q.Wh || !q.y3 || !q.W3 || !q.y2 || !q.dz3 || !q.dz2 || !q.gb3 || !q.gb2 || q.nh < 1 || q.nh > TAIL_HPW || q.lddout < q.nh)
-            return go1_set_error("go1_mlp_tail_backward: bad arguments (head width 1..12)");
-        if ((q.ldy3 & 3) || (q.ldy2 & 3) || (q.lddz3 & 3) || (q.lddz2 & 3) ||
-            ((((uintptr_t)q.y3 | (uintptr_t)q.y2 | (uintptr_t)q.W3 | (uintptr_t)q.dz3 | (uintptr_t)q.dz2) & 15) != 0))
-            return go1_set_error("go1_mlp_tail_backward: operands must be 16-byte aligned with row strides that are multiples of 4 floats");
-        if (int e = make_map_mn(&maps.w3[p], q.W3, N3, N2, N2, N2)) return e;
-        if (int e = make_map(&maps.dz3[p], q.dz3, M, N3, q.lddz3, 32)) return e;
-        TailBwdProb& d = g.p[p];
-        d.dout = q.dout; d.Wh = q.Wh; d.y3 = q.y3; d.y2 = q.y2; d.dz2 = q.dz2; d.lddz2 = q.lddz2; d.gb3 = q.gb3; d.gb2 = q.gb2; d.lddout = q.lddout; d.nh = q.nh; d.ldy3 = q.ldy3; d.ldy2 = q.ldy2;
-    }
-    for (int p = nprob; p < TAIL_MAXP; p++) { maps.w3[p] = maps.w3[0]; maps.dz3[p] = maps.dz3[0]; g.p[p] = g.p[0]; }
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(mlp_tail_bwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TB_SMEM);
-        if (e == cudaSuccess) e = cudaFuncSetAttribute(mlp_tail_bwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TB_SMEM);
-        if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
-        configured = true;
-    }
-    const int sms = sm_count();
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    const bool timed = g_time_on && cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone;
-    if (timed) {
-        cudaEventRecord(timing_event(), st);
-        double fl = 0.0;
-        for (int p = 0; p < nprob; p++) fl += 2.0 * (double)M * ((double)N3 * N2 + (double)probs[p].nh * N3);
-        g_time_flop += fl;
-        g_time_recs.push_back({M * nprob, N2, N3, 0, 1, 2, 0, 1, 1004, 1});
-    }
-    const int grid = g.tiles < sms ? g.tiles : sms;
-    if (g.kind == GO1_ACT_ELU) mlp_tail_bwd_kernel<false><<<grid, 32 * NCONS + 128, TB_SMEM, st>>>(maps, g);
-    else mlp_tail_bwd_kernel<true><<<grid, 32 * NCONS + 128, TB_SMEM, st>>>(maps, g);
-    go1_count_launch(1);
-    if (timed) cudaEventRecord(timing_event(), st);
-    cudaError_t ce = cudaGetLastError();
-    if (ce != cudaSuccess) return go1_set_error(cudaGetErrorString(ce));
-    return 0;
 }

@@ -146,12 +146,6 @@ def copy_segments(pairs):
     check(lib().go1_copy_segments(arr, n, stream_ptr()), "go1_copy_segments")
 
 
-class Go1TailBwdProblem(C.Structure):
-    _fields_ = [("dout", C.c_void_p), ("lddout", _i), ("nh", _i), ("Wh", C.c_void_p), ("y3", C.c_void_p), ("ldy3", _i), ("W3", C.c_void_p),
-                ("y2", C.c_void_p), ("ldy2", _i), ("dz3", C.c_void_p), ("lddz3", _i), ("dz2", C.c_void_p), ("lddz2", _i), ("gb3", C.c_void_p), ("gb2", C.c_void_p),
-                ("act_kind", _i)]
-
-
 class Go1Error(RuntimeError):
     pass
 
@@ -191,7 +185,6 @@ def lib():
         "go1_ppo_normalize_advantages": ([vp, vp, i64, i64, vp], ip),
         "go1_gemm": ([ip, ip, ip, ip, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, vp], ip),
         "go1_gemm_ex": ([ip, ip, ip, ip, ip, vp, ip, vp, ip, vp, ip, C.POINTER(Go1GemmEpilogue), ip, vp], ip),
-        "go1_mlp_tail_backward_grouped": ([C.POINTER(Go1TailBwdProblem), ip, ip, ip, ip, vp], ip),
         "go1_mlp_tail_forward_grouped": ([C.POINTER(Go1TailProblem), ip, ip, ip, ip, ip, vp], ip),
         "go1_mlp_tail_forward": ([vp, ip, ip, ip, vp, vp, ip, vp, ip, vp, vp, ip, vp, ip, vp, vp, ip, vp, ip, vp], ip),
         "go1_transpose": ([vp, ip, vp, ip, ip, ip, vp], ip),

@@ -238,11 +238,8 @@ class Runner:
                     graph = torch.cuda.CUDAGraph()
                     ac.ensure_packed()
                     n0 = L.go1_kernel_launch_count()
-                    try:
-                        with torch.cuda.graph(graph):
-                            actions = self._graph_step_body(sg)
-                    finally:
-                        ac.force_repack = False
+                    with torch.cuda.graph(graph):
+                        actions = self._graph_step_body(sg)
                     n_kernels = L.go1_kernel_launch_count() - n0
                     L.go1_kernel_launch_add(-n_kernels)
                     env._cur = p; env.obs_history = env._bufs[p]       # capture ran the host half of _roll without executing anything

@@ -6,7 +6,7 @@ the reference's names, .act / .evaluate / .act_student / .act_teacher / .get_act
 .action_std / .entropy), but:
   * all parameters are views into ONE flat fp32 buffer (adaptation module first), gradients into one flat
     gradient buffer -> one grad-norm, one Adam launch, one NCCL all-reduce per optimizer step;
-  * forward and backward are explicit go1_gemm calls (fp32 CUDA-core or tcgen05 TF32) with fused
+  * forward and backward are explicit go1_gemm calls (fp32 CUDA-core or wgmma TF32) with fused
     bias+activation epilogues (AC_Args.activation: every name of the reference's get_activation); cat(obs_history, latent) is never materialised (the 2 extra input columns are a
     second, K=2 GEMM accumulated into the first layer's pre-activation);
   * no autograd graph: the backward pass is written out (see `backward_ppo`, `backward_adaptation`).
@@ -26,7 +26,7 @@ class AC_Args(PrefixProto, cli=False):
     activation = 'elu'  # can be elu, relu, selu, crelu, lrelu, tanh, sigmoid (all run on the fused kernels; crelu is nn.ReLU, as in the reference)
     adaptation_module_branch_hidden_dims = [256, 128]
     use_decoder = False
-    gemm_impl = 1       # 1 = tcgen05 TF32 tensor cores (default; torch 1.10, the reference's pin, also ran these matmuls in TF32), 0 = fp32 CUDA cores (exact)
+    gemm_impl = 1       # 1 = wgmma TF32 tensor cores (default; torch 1.10, the reference's pin, also ran these matmuls in TF32), 0 = fp32 CUDA cores (exact)
 
 
 def _mlp(in_dim, hidden, out_dim, activation):
@@ -58,15 +58,10 @@ def history_kmajor(h, priv, out):
     return out
 
 
-def _aligned(t_or_ptr, ld):
-    p = t_or_ptr if isinstance(t_or_ptr, int) else t_or_ptr.data_ptr()
-    return (p & 15) == 0 and (ld & 3) == 0
-
-
 class _Net:
     """Forward/backward of one MLP whose first layer reads [x (K0 columns) | extra (E columns)].
 
-    impl 0: every product is one fp32 CUDA-core go1_gemm.  impl 1: the large products run on the tcgen05 TF32 kernel,
+    impl 0: every product is one fp32 CUDA-core go1_gemm.  impl 1: the large products run on the wgmma TF32 kernel,
     which reads its operands through TMA (16-byte aligned rows) in either major: forward K-major, dgrad with W as an
     MN-major B operand, wgrad with dz and the layer input as MN-major A and B operands -- except the first layers' wgrad, which
     ActorCritic runs K-major on transposed copies (history_kmajor, dz1T).  Only the first-layer weight block W[:, :K0] (row
@@ -234,49 +229,20 @@ class _Net:
         capi.check(capi.lib().go1_mlp_tail_forward_grouped(arr, 1, M, k1, n2, n3, capi.stream_ptr()), "go1_mlp_tail_forward")
         return outs
 
-    def tail_bwd_ok(self, outs, dout):
-        """This body is a ...-256-128-head one whose backward first half go1_mlp_tail_backward_grouped supports (launches nothing)."""
-        sp = self.specs
-        if len(sp) != 4 or sp[2][2] != 128 or sp[2][3] != 256 or sp[1][2] != 256 or sp[3][2] > 12 or not self.owner.grads_prezeroed:
-            return False
-        y3, y2 = outs[2], outs[1]
-        return self._tma_ok(y3, y3.stride(0)) and self._tma_ok(y2, y2.stride(0)) and ((self.flat.data_ptr() + 4 * sp[2][0]) & 15) == 0 and dout.stride(1) == 1
-
-    def tail_bwd_problem(self, outs, dout, M, tag):
-        """Launches the head's wgrad (+ bias gradient) of this body and returns (Go1TailBwdProblem, dz3, dz2) for the fused backward first
-        half (go1_mlp_tail_backward_grouped).  Call only if tail_bwd_ok()."""
-        sp = self.specs
-        (wo3, bo3, n3, n2), (woh, boh, nh, _), (wo2, bo2, _, _) = sp[2], sp[3], sp[1]
-        y3, y2 = outs[2], outs[1]
+    def backward(self, x, ldx, K0, extra, outs, dout, M, impl, want_dextra=False, tag="a", dz1T=None, wgrads=None):
+        """dout: gradient w.r.t. the network output [M][out] (the last layer has no activation).  Adds the weight and bias gradients into
+        the flat grad buffer, which the caller has zeroed (ActorCritic.backward_ppo / backward_adaptation): split-K partial tiles and the
+        bias gradients reduced in epilogues are atomic sums.  dz of every hidden layer comes out of the dgrad GEMM already multiplied by
+        the activation's derivative, computed from the saved layer output (fused epilogue).  dz1T: optional [o1][M] strided view; when
+        given the first layer's dz is stored there transposed (K-major for the weight-gradient product) and that layer's wgrad, bias
+        gradient and trailing-input weight gradients are left to the caller (ActorCritic._first_layer_wgrad: augmented rows of the
+        transposed input).  wgrads: optional list that collects the tensor-core wgrads instead of launching them (ActorCritic._flush_wgrads
+        launches equal shapes as grouped products).  Returns d(extra) [M][E] if requested."""
         L, st = capi.lib(), capi.stream_ptr()
-        gWh, gbh = self.grad[woh:woh + nh * n3], self.grad[boh:boh + nh]
-        capi.check(L.go1_skinny_wgrad_ex(capi.ptr(dout), dout.stride(0), capi.ptr(y3), y3.stride(0), gWh.data_ptr(), n3, gbh.data_ptr(), M, nh, n3, 1, st), "skinny_wgrad")
-        dz3, dz2 = self._buf((tag, "d", 2), M, n3), self._buf((tag, "d", 1), M, n2)
-        q = capi.Go1TailBwdProblem()
-        q.act_kind = self.kind
-        q.dout, q.lddout, q.nh, q.Wh = dout.data_ptr(), dout.stride(0), nh, self.flat.data_ptr() + 4 * woh
-        q.y3, q.ldy3, q.W3, q.y2, q.ldy2 = y3.data_ptr(), y3.stride(0), self.flat.data_ptr() + 4 * wo3, y2.data_ptr(), y2.stride(0)
-        q.dz3, q.lddz3, q.dz2, q.lddz2 = dz3.data_ptr(), dz3.stride(0), dz2.data_ptr(), dz2.stride(0)
-        q.gb3, q.gb2 = self.grad.data_ptr() + 4 * bo3, self.grad.data_ptr() + 4 * bo2
-        return q, dz3, dz2
-
-    def backward(self, x, ldx, K0, extra, outs, dout, M, impl, accumulate, want_dextra=False, tag="a", dz1T=None, pre=None):
-        """dout: gradient w.r.t. the network output [M][out] (the last layer has no activation).  Writes weight/bias grads
-        into the flat grad buffer.  dz of every hidden layer comes out of the dgrad GEMM already multiplied by the
-        activation's derivative, computed from the saved layer output (fused epilogue).  dz1T: optional [o1][M] strided view; when given the
-        first layer's dz is stored there transposed (K-major for the weight-gradient product) and that layer's wgrad, bias gradient and
-        trailing-input weight gradients are left to the caller (ActorCritic._first_layer_wgrad: augmented rows of the transposed input), so
-        the dgrad epilogue that produces it reduces neither of them (only d(extra) if requested).  Returns d(extra) [M][E] if requested."""
-        L, st = capi.lib(), capi.stream_ptr()
-        n = len(self.specs)
-        dz = dout
-        dextra = None
-        bias_done = False      # this layer's bias gradient was already reduced in the epilogue of the dgrad product that made its dz
-        extra_done = False     # likewise the trailing-input gradients of the first layer
-        start = n - 1
-        if pre is not None:    # (dz of layer n-2, dz of layer n-3) from go1_mlp_tail_backward_grouped, which also reduced their bias gradients;
-            dz, start, bias_done = pre[0], n - 2, True      # the head's wgrad was launched by tail_bwd_problem
-        for li in range(start, -1, -1):
+        dz, dextra = dout, None
+        bias_done = False      # this layer's bias gradient was reduced by the dgrad that made its dz, or is left to the caller
+        extra_done = False     # likewise the first layer's trailing-input gradients
+        for li in range(len(self.specs) - 1, -1, -1):
             wo, bo, o, i = self.specs[li]
             W = self.flat[wo:wo + o * i]
             gW, gb = self.grad[wo:wo + o * i], self.grad[bo:bo + o]
@@ -285,91 +251,67 @@ class _Net:
                 inp, ld_in, K = x, ldx, (K0 if extra is not None else i)
             else:
                 inp, ld_in, K = outs[li - 1], outs[li - 1].stride(0), i
-            prez = 1 if (accumulate or self.owner.grads_prezeroed) else 0      # the caller zeroed the gradient buffer: accumulate, no memsets
-            skinny_w = not (li == 0 and dz1T is not None) and o <= 16 and K >= 32
-            if not bias_done and skinny_w and K % 4 == 0 and self._tma_ok(inp, ld_in):
-                # the narrow heads: weight AND bias gradient in one bandwidth-bound pass over the layer input
-                capi.check(L.go1_skinny_wgrad_ex(capi.ptr(dz), ldz, capi.ptr(inp), ld_in, gW.data_ptr(), i, gb.data_ptr(), M, o, K, prez, st), "skinny_wgrad")
-                skinny_w, bias_done = False, True
+            wgrad_done = li == 0 and dz1T is not None       # made by the caller
+            skinny = not wgrad_done and o <= 16 and K >= 32  # the narrow heads: one bandwidth-bound pass instead of a padded GEMM tile
+            # ---- 1. bias gradient: reduced by the dgrad that made dz, by the skinny wgrad, or by go1_colsum
             if not bias_done:
-                capi.check(L.go1_colsum(capi.ptr(dz), ldz, capi.ptr(gb), M, o, accumulate, st), "colsum")
-            bias_done = False
-            # ---- wgrad: dW[o][K] = dz^T[o][M] inp[M][K]
-            if li == 0 and dz1T is not None:
-                pass                                    # fused by the caller
-            elif o <= 16 and K >= 32:   # the narrow heads: one bandwidth-bound pass instead of a padded GEMM tile
-                if skinny_w:
-                    capi.check(L.go1_skinny_wgrad(capi.ptr(dz), ldz, capi.ptr(inp), ld_in, gW.data_ptr(), i, M, o, K, prez, st), "skinny_wgrad")
-            else:       # impl 1: both operands MN-major, read in place by the tcgen05 kernel
+                if skinny and K % 4 == 0 and self._tma_ok(inp, ld_in):
+                    # weight AND bias gradient in one pass over the layer input
+                    capi.check(L.go1_skinny_wgrad_ex(capi.ptr(dz), ldz, capi.ptr(inp), ld_in, gW.data_ptr(), i, gb.data_ptr(), M, o, K, 1, st), "skinny_wgrad")
+                    wgrad_done = True
+                else:
+                    capi.check(L.go1_colsum(capi.ptr(dz), ldz, capi.ptr(gb), M, o, 0, st), "colsum")
+            # ---- 2. wgrad: dW[o][K] = dz^T[o][M] inp[M][K]
+            if wgrad_done:
+                pass
+            elif skinny:
+                capi.check(L.go1_skinny_wgrad(capi.ptr(dz), ldz, capi.ptr(inp), ld_in, gW.data_ptr(), i, M, o, K, 1, st), "skinny_wgrad")
+            else:       # impl 1: both operands MN-major, read in place by the wgmma kernel; split-K partial tiles add into the zeroed gradient
                 tc = impl == 1 and M >= 64 and K >= 8 and self._tma_ok(dz, ldz) and self._tma_ok(inp, ld_in)
-                # into a gradient buffer the caller has already zeroed the split-K partial tiles can accumulate directly (no zeroing pass)
-                acc_w = 1 if (accumulate or (tc and self.owner.grads_prezeroed)) else 0
-                q = self.owner._wgrad_queue
-                if q is not None and tc and acc_w:      # deferred: ActorCritic launches the equal-shape wgrads of its MLPs as grouped products
-                    q.append((o, K, M, ldz, ld_in, i, dz, inp, gW))
+                if tc and wgrads is not None:
+                    wgrads.append((o, K, M, ldz, ld_in, i, dz, inp, gW))
                 else:
-                    self._gemm(1, 0, o, K, M, dz, ldz, inp, ld_in, gW, i, None, 0, acc_w, 1 if tc else 0)
-            if li == 0 and extra is not None and not extra_done:
-                E = i - K0
-                if want_dextra:
-                    dextra = self._buf((tag, "dextra"), M, E)
-                capi.check(L.go1_mlp_extra_backward(capi.ptr(dz), ldz, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i, gW.data_ptr() + 4 * K0, i,
-                                                    capi.ptr(dextra) if want_dextra else None, E, M, o, E, accumulate, st), "extra_backward")
-            # ---- dgrad (+ fused activation derivative): dz_prev[M][i] = (dz[M][o] W[o][i]) * f'(y_prev)
-            if pre is not None and li == n - 2:
-                dz, bias_done = pre[1], True            # produced (with its bias gradient) by the fused kernel
-                continue
-            if li > 0:
-                aug = dz1T is not None and li == 1
-                dprev = dz1T if aug else self._buf((tag, "d", li - 1), M, i)
-                ldp = dprev.stride(0)
-                yprev = outs[li - 1]
-                if impl == 1 and self._tma_ok(dz, ldz) and self._tma_ok(W, i) and M >= 64:      # (the 12-wide actor head included: 19 us here, 22 us on the skinny pass)
-                    # W read MN-major in place; the bias gradient of layer li-1 (column sums of dprev) rides in the epilogue
-                    pwo, pbo, po, pi = self.specs[li - 1]
-                    gb_prev = self.grad[pbo:pbo + po]
-                    fuse = self.owner.fuse_bias_grad
-                    if fuse and not accumulate and not self.owner.grads_prezeroed:
-                        gb_prev.zero_()
-                    bx = None
-                    if aug:
-                        # the first layer's bias and trailing-input weight gradients come out of the caller's fused wgrad; only d(extra) is left
-                        if extra is not None and want_dextra:
-                            E0 = pi - K0
-                            Wp = self.flat[pwo:pwo + po * pi]
-                            dextra = self._buf((tag, "dextra"), M, E0)
-                            dextra.zero_()
-                            bx = (extra, Wp.data_ptr() + 4 * K0, pi, None, 0, dextra)
-                        extra_done = True
-                    elif fuse and li == 1 and extra is not None and self.owner.grads_prezeroed and not accumulate and 1 <= pi - K0 <= 4:
-                        # dprev is the first layer's dz: its trailing-input weight gradient (and d(extra)) are reduced in this epilogue too
-                        E0 = pi - K0
-                        Wp = self.flat[pwo:pwo + po * pi]
-                        gWp = self.grad[pwo:pwo + po * pi]
-                        if want_dextra:
-                            dextra = self._buf((tag, "dextra"), M, E0)
-                            dextra.zero_()
-                        bx = (extra, Wp.data_ptr() + 4 * K0, pi, gWp.data_ptr() + 4 * K0, pi, dextra if want_dextra else None)
-                        extra_done = True
-                    self._gemm(0, 0, M, i, o, dz, ldz, W, i, dprev, ldp, None, 2, 0, 1, dact_y=yprev, colsum=gb_prev if (fuse and not aug) else None, bwd_extra=bx,
-                               store_transposed=1 if aug else 0)
-                    bias_done = bool(fuse) or aug
-                elif aug:
-                    raise capi.Go1Error("transposed first-layer dz: the dgrad that produces it must be a tensor-core product")
-                elif o <= 16:
-                    pwo, pbo, po, pi = self.specs[li - 1]
-                    gb_prev = self.grad[pbo:pbo + po]
-                    fuse = impl == 1 and self.owner.fuse_bias_grad and i % 4 == 0 and self._tma_ok(W, i) and self._tma_ok(dprev, ldp) and self._tma_ok(yprev, yprev.stride(0))
-                    if fuse and not accumulate and not self.owner.grads_prezeroed:
-                        gb_prev.zero_()
-                    # the bias gradient of layer li-1 (column sums of dprev) is reduced in the same pass
-                    capi.check(L.go1_skinny_dgrad_act(capi.ptr(dz), ldz, capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(dprev), ldp,
-                                                      gb_prev.data_ptr() if fuse else None, M, o, i, self.kind, st), "skinny_dgrad")
-                    bias_done = bool(fuse)
-                else:
-                    self._gemm(0, 0, M, i, o, dz, ldz, W, i, dprev, ldp, None, 2, 0, 0, dact_y=yprev)
-                dz = dprev
-        return dextra
+                    self._gemm(1, 0, o, K, M, dz, ldz, inp, ld_in, gW, i, None, 0, 1 if tc else 0, 1 if tc else 0)
+            if li == 0:
+                if extra is not None and not extra_done:
+                    E = i - K0
+                    if want_dextra:
+                        dextra = self._buf((tag, "dextra"), M, E)
+                    capi.check(L.go1_mlp_extra_backward(capi.ptr(dz), ldz, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i, gW.data_ptr() + 4 * K0, i,
+                                                        capi.ptr(dextra) if want_dextra else None, E, M, o, E, 0, st), "extra_backward")
+                return dextra
+            # ---- 3. dgrad (+ fused activation derivative): dz_prev[M][i] = (dz[M][o] W[o][i]) * f'(y_prev)
+            pwo, pbo, po, pi = self.specs[li - 1]
+            gb_prev, yprev = self.grad[pbo:pbo + po], outs[li - 1]
+            to_T = li == 1 and dz1T is not None
+            dprev = dz1T if to_T else self._buf((tag, "d", li - 1), M, i)
+            ldp = dprev.stride(0)
+            if impl == 1 and self._tma_ok(dz, ldz) and self._tma_ok(W, i) and M >= 64:      # (the 12-wide actor head included: 19 us here, 22 us on the skinny pass)
+                # W read MN-major in place; the bias gradient of layer li-1 (column sums of dprev) rides in the epilogue
+                bx = None
+                if li == 1 and extra is not None and (to_T or 1 <= pi - K0 <= 4):
+                    # dprev is the first layer's dz: d(extra), and the trailing-input weight gradient unless _first_layer_wgrad makes it,
+                    # are reduced in this epilogue too
+                    extra_done = True
+                    if want_dextra:
+                        dextra = self._buf((tag, "dextra"), M, pi - K0).zero_()
+                    gwx = None if to_T else self.grad.data_ptr() + 4 * (pwo + K0)
+                    if dextra is not None or gwx is not None:
+                        bx = (extra, self.flat.data_ptr() + 4 * (pwo + K0), pi, gwx, pi, dextra)
+                self._gemm(0, 0, M, i, o, dz, ldz, W, i, dprev, ldp, None, 2, 0, 1, dact_y=yprev, colsum=None if to_T else gb_prev, bwd_extra=bx,
+                           store_transposed=1 if to_T else 0)
+                bias_done = True
+            elif to_T:
+                raise capi.Go1Error("transposed first-layer dz: the dgrad that produces it must be a tensor-core product")
+            elif o <= 16:
+                # the bias gradient of layer li-1 (column sums of dprev) is reduced in the same pass where the operands allow it
+                bias_done = impl == 1 and i % 4 == 0 and self._tma_ok(W, i) and self._tma_ok(dprev, ldp) and self._tma_ok(yprev, yprev.stride(0))
+                capi.check(L.go1_skinny_dgrad_act(capi.ptr(dz), ldz, capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(dprev), ldp,
+                                                  gb_prev.data_ptr() if bias_done else None, M, o, i, self.kind, st), "skinny_dgrad")
+            else:
+                self._gemm(0, 0, M, i, o, dz, ldz, W, i, dprev, ldp, None, 2, 0, 0, dact_y=yprev)
+                bias_done = False
+            dz = dprev
 
 
 class ActorCritic(nn.Module):
@@ -395,20 +337,14 @@ class ActorCritic(nn.Module):
         self._mean = self._value = self._logp = None
         self._sample_counter = 0
         self._counter_dev = None
-        self.force_repack = False     # (kept for callers that set it; packing is never part of a graph any more, see ensure_packed)
         self._packed_version = -1
-        self._wgrad_queue = None      # list while backward_ppo collects the tensor-core wgrads of the layers behind the first ones
         self.sample_seed = 0
         self.injected_eps = None      # parity tests inject the N(0,1) draws
         self.weights_version = 0      # bumped by every optimizer step / load: invalidates the packed first-layer weight copies
         import os
-        self.group_wgrads = os.environ.get("GO1_GROUP_WGRADS", "1") != "0"          # equal-shape wgrads of the three MLPs as grouped products
-        self.fuse_tail_bwd = os.environ.get("GO1_FUSE_TAIL_BWD", "0") != "0"        # first half of the bodies' backward tails in one launch (go1_mlp_tail_backward_grouped)
-        self.fuse_bias_grad = os.environ.get("GO1_FUSE_BIAS_GRAD", "1") != "0"     # bias gradients reduced in the dgrad GEMM epilogues
         self.update_streams = os.environ.get("GO1_UPDATE_STREAMS", "1") != "0"     # critic chain on a second stream during the update (measured -1.3 ms / iteration)
         self._side = None
-        self.fuse_tail = os.environ.get("GO1_FUSE_TAIL", "1") != "0"     # layers behind a first layer in one tcgen05 launch (go1_mlp_tail_forward_grouped: actor + critic bodies in one grid)
-        self.grads_prezeroed = False  # PPO.update zeroes the flat gradient buffer once per optimizer step (one fill instead of one per layer)
+        self.fuse_tail = os.environ.get("GO1_FUSE_TAIL", "1") != "0"     # layers behind a first layer in one wgmma launch (go1_mlp_tail_forward_grouped: actor + critic bodies in one grid)
 
     # ------------------------------------------------------------------ flat storage
     def _ordered_params(self):
@@ -684,13 +620,12 @@ class ActorCritic(nn.Module):
         return self._nets["adapt"].forward(h, h.stride(0), self.num_obs_history, None, h.shape[0], self._impl(), "latent")[-1]
 
     # ------------------------------------------------------------------ explicit backward passes (ppo.py:154-189)
-    def _flush_wgrads(self):
-        """Launch the queued wgrads: equal shapes (same M, N, K and operand strides) as ONE grouped product (go1_gemm_grouped: up to four
-        problems in one grid), the rest one by one.  All of them accumulate into the pre-zeroed flat gradient buffer."""
+    def _flush_wgrads(self, wgrads):
+        """Launch the collected wgrads: equal shapes (same M, N, K and operand strides) as ONE grouped product (go1_gemm_grouped: up to
+        four problems in one grid), the rest one by one.  All of them accumulate into the zeroed flat gradient buffer."""
         import ctypes as C
-        q, self._wgrad_queue = self._wgrad_queue, None
         groups = {}
-        for it in q:
+        for it in wgrads:
             groups.setdefault(it[:6], []).append(it)
         L, st = capi.lib(), capi.stream_ptr()
         for (o, K, M, ldz, ld_in, i), items in groups.items():
@@ -731,14 +666,14 @@ class ActorCritic(nn.Module):
             row += o
         capi.copy_segments(pairs)
 
-    def backward_ppo(self, h, priv, dmean, dvalue, dstd, aug=False, hT=None):
-        """Gradients of the PPO loss into flat_grads (overwrites). h/priv are the minibatch inputs of the forward
-        pass just run with tag='train'; dmean [M,A], dvalue [M,1], dstd [A].
+    def backward_ppo(self, h, priv, dmean, dvalue, dstd, hT=None):
+        """Gradients of the PPO loss into flat_grads[HEAD:] (overwrites; the loss scalars in the head are left alone). h/priv are the
+        minibatch inputs of the forward pass just run with tag='train'; dmean [M,A], dvalue [M,1], dstd [A].
         hT: history_kmajor(h, priv) if the caller keeps one (RolloutStorage builds it once per update); built here otherwise.  Its latent
-        rows are written here.  aug: h is a view of a row buffer with spare columns [1 | priv | latent] behind the K0 history columns;
-        the latent is copied there as well."""
+        rows are written here."""
         M, K0 = h.shape[0], self.num_obs_history
         nets = self._nets
+        self._grad[self.HEAD:].zero_()      # one fill; every kernel below adds into it (atomics in the epilogues and split-K products)
         if self._first_layers_fusable(h, priv):
             # the three first layers share their input: ONE transposed dz [o_a+o_p+o_c][M] (each net's layer-2 dgrad stores its
             # first-layer dz into its row slice) and ONE tensor-core wgrad with K-major operands (_first_layer_wgrad)
@@ -748,55 +683,45 @@ class ActorCritic(nn.Module):
                 hT = history_kmajor(h, priv, nets["adapt"]._buf(("train", "hT"), K0 + 1 + 2 * E, (M + 31) // 32 * 32))
             L, st = capi.lib(), capi.stream_ptr()
             capi.check(L.go1_transpose(capi.ptr(self._latent), self._latent.stride(0), capi.ptr(hT[K0 + 1 + E:]), hT.stride(0), M, E, st), "transpose")
-            if aug and h.stride(0) >= K0 + 1 + 2 * E:
-                capi.copy_segments([(h.as_strided((M, E), (h.stride(0), 1), h.storage_offset() + K0 + 1 + E), self._latent)])
             dz1 = nets["adapt"]._buf(("train", "dz1catT"), oa + op + oc, hT.stride(0))
             impl = 1
-            if self.group_wgrads and self.grads_prezeroed:
-                self._wgrad_queue = []
-            pre_p = pre_c = None
-            if self.fuse_tail_bwd:      # first half of both bodies' backward tails in ONE grid (dz3, dz2 and their bias gradients)
-                if nets["actor"].tail_bwd_ok(self._p_out, dmean) and nets["critic"].tail_bwd_ok(self._c_out, dvalue):
-                    tp, tc = nets["actor"].tail_bwd_problem(self._p_out, dmean, M, "train"), nets["critic"].tail_bwd_problem(self._c_out, dvalue, M, "train")
-                    arr = (capi.Go1TailBwdProblem * 2)(tp[0], tc[0])
-                    capi.check(capi.lib().go1_mlp_tail_backward_grouped(arr, 2, M, 128, 256, capi.stream_ptr()), "go1_mlp_tail_backward")
-                    pre_p, pre_c = tp[1:], tc[1:]
+            wgrads = []             # the tensor-core wgrads behind the first layers, launched as grouped products once all dz exist
             side = self._side_stream(M)
             if side is not None:    # critic chain beside actor -> adaptation chain
                 self._fork(side)
                 with torch.cuda.stream(side):
-                    nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, 0, tag="train", dz1T=dz1[oa + op:], pre=pre_c)
-            dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, impl, 0, want_dextra=True, tag="train", dz1T=dz1[oa:oa + op],
-                                          pre=pre_p)
+                    nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, tag="train", dz1T=dz1[oa + op:], wgrads=wgrads)
+            dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, impl, want_dextra=True, tag="train", dz1T=dz1[oa:oa + op],
+                                          wgrads=wgrads)
             if side is None:
-                nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, 0, tag="train", dz1T=dz1[oa + op:], pre=pre_c)
-            nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, 0, tag="train", dz1T=dz1[:oa])
+                nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, tag="train", dz1T=dz1[oa + op:], wgrads=wgrads)
+            nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, tag="train", dz1T=dz1[:oa], wgrads=wgrads)
             if side is not None:
                 self._join(side)
-            if self._wgrad_queue is not None:
-                self._flush_wgrads()
+            self._flush_wgrads(wgrads)
             self._first_layer_wgrad(("adapt", "actor", "critic"), dz1, hT, M, "train")
         else:
             impl = self._impl()
-            dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, impl, 0, want_dextra=True, tag="train")
-            nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, 0, tag="train")
-            nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, 0, tag="train")
+            dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, impl, want_dextra=True, tag="train")
+            nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, tag="train")
+            nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, tag="train")
         self._grad[self.std_offset:self.std_offset + self.num_actions].copy_(dstd)
 
     def backward_adaptation(self, h, outs, dpred, hT=None):
-        """Gradients of the adaptation module (overwrites its part of flat_grads).  hT: history_kmajor(h, ..) if the caller keeps one
-        (built here otherwise); the first layer's weight and bias gradients are the K-major product over its first K0 + 1 rows."""
+        """Gradients of the adaptation module (overwrites its part of flat_grads, [HEAD:n_adapt_params]).  hT: history_kmajor(h, ..) if the
+        caller keeps one (built here otherwise); the first layer's weight and bias gradients are the K-major product over its first K0 + 1 rows."""
         M, K0 = h.shape[0], self.num_obs_history
         net = self._nets["adapt"]
+        self._grad[self.HEAD:self.n_adapt_params].zero_()
         if self._impl() == 1 and M >= 64 and _Net._tma_ok(h, h.stride(0)) and net.specs[0][3] == K0:
             if hT is None:
                 hT = history_kmajor(h, None, net._buf(("adapt", "hT"), K0 + 1, (M + 31) // 32 * 32))
             oa = net.specs[0][2]
             dz1 = net._buf(("adapt", "dz1T"), oa, hT.stride(0))
-            net.backward(h, h.stride(0), K0, None, outs, dpred, M, 1, 0, tag="adapt", dz1T=dz1)
+            net.backward(h, h.stride(0), K0, None, outs, dpred, M, 1, tag="adapt", dz1T=dz1)
             self._first_layer_wgrad(("adapt",), dz1, hT[:K0 + 1], M, "adapt")
         else:
-            net.backward(h, h.stride(0), K0, None, outs, dpred, M, self._impl(), 0, tag="adapt")
+            net.backward(h, h.stride(0), K0, None, outs, dpred, M, self._impl(), tag="adapt")
 
     def adaptation_forward(self, h):
         self.flatten()

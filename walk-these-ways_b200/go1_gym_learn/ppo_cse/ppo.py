@@ -131,11 +131,8 @@ class PPO:
             ac.ensure_packed()                                    # the graph reads the packed weight copies, it does not build them
             L = capi.lib()
             n0 = L.go1_kernel_launch_count()
-            try:
-                with torch.cuda.graph(graph):
-                    outs = self._act_eager(h_in, p_in)
-            finally:
-                ac.force_repack = False
+            with torch.cuda.graph(graph):
+                outs = self._act_eager(h_in, p_in)
             n_kernels = L.go1_kernel_launch_count() - n0          # this library's kernels inside the graph
             L.go1_kernel_launch_add(-n_kernels)                   # capture launched nothing
             g = st[key] = (graph, h_in, p_in, outs, (ac._mean, ac._logp, ac._last_actions, ac._value, ac._latent), inplace, n_kernels)
@@ -212,8 +209,6 @@ class PPO:
             bi = it_mb % len(batches)
             (obs_b, critic_obs_b, priv_b, hist_b, actions_b, target_values_b, adv_b, returns_b, old_logp_b, old_mu_b, old_sigma_b, masks_b, env_bins_b) = batches[bi]
             M = hist_b.shape[0]
-            ac.flat_grads.zero_()           # the fused bias-gradient epilogues accumulate with atomics; the loss scalars land in the head afterwards
-            ac.grads_prezeroed = True
             mean_b, value_b = ac.forward_all(hist_b, priv_b, tag="train")
             dmean = ac._nets["actor"]._buf(("train", "dmean"), M, ac.num_actions)
             dvalue = ac._nets["critic"]._buf(("train", "dvalue"), M, 1)
@@ -238,7 +233,6 @@ class PPO:
                 dpred = ac._nets["adapt"]._buf(("adapt", "dpred"), M, pred.shape[1])
                 capi.check(L.go1_ppo_mse(capi.ptr(pred), pred.stride(0), capi.ptr(priv_b), priv_b.stride(0), capi.ptr(dpred), dpred.stride(0),
                                          capi.ptr(self._mse_scalars), M, num_train, pred.shape[1], st()), "mse")
-                ac.flat_grads[ac.HEAD:ac.n_adapt_params].zero_()
                 ac.backward_adaptation(hist_b, outs, dpred, hT=getattr(hist_b, "hT", None))
                 if self.process_group is not None:      # adaptation gradients + the MSE pair (buffer head) in one averaging all-reduce
                     import torch.distributed as dist
@@ -246,7 +240,6 @@ class PPO:
                 self.adaptation_module_optimizer.step()
                 self._acc[2:4] += self._mse_scalars
             n_updates += 1
-        ac.grads_prezeroed = False
 
         acc = self._acc.tolist()                      # the only host sync of the update
         self.learning_rate = float(self._lr_dev.item())
