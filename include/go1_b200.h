@@ -307,8 +307,9 @@ typedef enum Go1Activation { GO1_ACT_ELU = 0, GO1_ACT_SELU, GO1_ACT_RELU, GO1_AC
 int go1_gemm(int transA, int transB, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
              float* C, int ldc, const float* bias, int act, int accumulate, int impl, void* stream);
 /* Same product with the full fused epilogue, applied in this order to each output element v = sum_k a*b:
- *   v += C_old (accumulate);  v += sum_e extra[m][e] * w_extra[n][e]  (num_extra <= 4: the 2 trailing input columns of
- *   the actor/critic first layer, i.e. cat(obs_history, latent) without the cat);  v += bias[n];
+ *   v += C_old (accumulate);  v += sum_e extra[m][e] * w_extra[n][e]  (num_extra <= 4: the E trailing input columns of
+ *   the actor/critic first layer, i.e. cat(obs_history, latent) without the cat; a wider E is added after the product by
+ *   go1_mlp_extra_forward);  v += bias[n];
  *   act 1: v = f(v);  act 2: v *= f'(z) computed from the saved activation dact_y[m][n] (the autograd of the activation module
  *   fused into the dgrad GEMM);  f = the Go1Activation act_kind (0 = ELU). */
 typedef struct Go1GemmEpilogue {
@@ -319,7 +320,8 @@ typedef struct Go1GemmEpilogue {
                           * bias only): lets several first layers that share their input run as ONE product (impl 1) */
     float* colsum;       /* optional [N] (impl 1): colsum[n] += sum_m C[m][n] of the FINAL values this call writes -- the bias gradient
                           * of the layer whose dz this dgrad product produces, reduced in the epilogue (atomic adds: zero it first) */
-    /* optional (impl 1): C is the dz of a first layer with `num_bwd_extra` (<= 4) trailing inputs (go1_mlp_extra_backward's job done in
+    /* optional (impl 1): C is the dz of a first layer with `num_bwd_extra` (<= 4; a wider E goes through go1_mlp_extra_backward) trailing
+     * inputs (go1_mlp_extra_backward's job done in
      * this epilogue, atomic adds into zeroed outputs):  g_w_extra[n][t] += sum_m C[m][n] bwd_extra[m][t];
      * d_extra[m][t] += sum_n C[m][n] bwd_w_extra[n][t]  (d_extra may be NULL; g_w_extra may be NULL when d_extra is given) */
     const float* bwd_extra; const float* bwd_w_extra; float* g_w_extra; float* d_extra;
@@ -366,14 +368,18 @@ int go1_elu_backward(const float* y, int ldy, const float* dy, int lddy, float* 
 /* The same for any Go1Activation: dz = dy * f'(z) from the saved output y (go1_elu_backward is kind GO1_ACT_ELU of this kernel). */
 int go1_act_backward(const float* y, int ldy, const float* dy, int lddy, float* dz, int lddz, int M, int N, int kind, void* stream);
 /* Finishes a first layer whose trailing-input term was left out of the product: y = act(y + extra[m][:E] . w_extra[n][:E])
- * in place (E <= 4; act 0 / 1 / GO1_ACT(kind, 1)). */
+ * in place (1 <= E <= 64, the privileged-observation widths: at most 45; act 0 / 1 / GO1_ACT(kind, 1)).  Row strides: ldy >= o,
+ * ldex >= E, ldw >= E.  A bad argument returns non-zero before any launch. */
 int go1_mlp_extra_forward(float* y, int ldy, const float* extra, int ldex, const float* w_extra, int ldw, int M, int o, int E, int act,
                           void* stream);
-/* Backward of the E (<= 4) trailing input columns of a first layer (the `latent` / privileged columns of
- * cat(obs_history, .), actor_critic.py:115,143), one bandwidth-bound pass over dz [M][o]:
- *   g_w_extra[j][t] (+)= sum_m dz[m][j] extra[m][t];   dextra[m][t] = sum_j dz[m][j] w_extra[j][t] (if dextra != NULL). */
-int go1_mlp_extra_backward(const float* dz, int lddz, const float* extra, int ldex, const float* w_extra, int ldw, float* g_w_extra, int ldgw,
-                           float* dextra, int ldde, int M, int o, int E, int accumulate, void* stream);
+/* Backward of the E (1..64) trailing input columns of a first layer (the `latent` / privileged columns of
+ * cat(obs_history, .), actor_critic.py:115,143), bandwidth-bound passes over dz:
+ *   g_w_extra[j][t] (+)= sum_m dz[m][j] extra[m][t]  (if g_w_extra != NULL; needs dz_transposed 0);
+ *   dextra[m][t] = sum_j dz[m][j] w_extra[j][t]      (if dextra != NULL).
+ * dz_transposed 0: dz is [M][o] (lddz >= o);  1: dz is stored as [o][M] (lddz >= M), the first-layer dz a store_transposed dgrad
+ * epilogue writes.  At least one output; a bad argument returns non-zero before any launch. */
+int go1_mlp_extra_backward(const float* dz, int lddz, int dz_transposed, const float* extra, int ldex, const float* w_extra, int ldw,
+                           float* g_w_extra, int ldgw, float* dextra, int ldde, int M, int o, int E, int accumulate, void* stream);
 /* Forward of a narrow (o <= 16) output layer, the 12 / 2 / 1-wide heads of ActorCritic (actor_critic.py:52,64,76):
  *   out[m][t] = b[t] + sum_k x[m][k] W[t][k]   (W row-major [o][K], K % 4 == 0, x rows 16-byte aligned; b may be NULL). */
 int go1_skinny_forward(const float* x, int ldx, const float* W, int ldw, const float* b, float* out, int ldo, int M, int o, int K, void* stream);

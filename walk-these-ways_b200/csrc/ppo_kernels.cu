@@ -361,12 +361,90 @@ __global__ void __launch_bounds__(256) extra_fwd_kernel(float* __restrict__ y, i
         y[(size_t)m * ldy + n] = v;
     }
 }
+// Wide variant (4 < E <= 64, the privileged-observation widths): the CTA stages its 128-column tile of w_extra, transposed to [E][128],
+// in shared memory once, and copies of its 32-row chunks of extra.  A warp walks rows (4 in flight), a lane owns 4 consecutive columns and
+// reads the row's E extra values as shared-memory broadcasts.  VEC: float4 rows and act_fast, as extra_fwd4_kernel; otherwise scalar
+// accesses and the libm forms, as extra_fwd_kernel.  KIND < 0: no activation.
+constexpr int XWIDE_MAX_E = 64, XWIDE_COLS = 128, XWIDE_ROWS = 32;
+template <int KIND, bool VEC>
+__global__ void __launch_bounds__(256) extra_fwd_wide_kernel(float* __restrict__ y, int ldy, const float* __restrict__ ex, int ldex, const float* __restrict__ wex,
+                                                             int ldw, int M, int o, int E) {
+    __shared__ __align__(16) float ws[XWIDE_MAX_E][XWIDE_COLS];
+    __shared__ float xs[XWIDE_ROWS][XWIDE_MAX_E + 1];
+    const int n0 = blockIdx.x * XWIDE_COLS, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int i = threadIdx.x; i < E * XWIDE_COLS; i += blockDim.x) {
+        const int c = i / E, t = i - c * E;         // consecutive threads read consecutive t of one w_extra row
+        ws[t][c] = n0 + c < o ? __ldg(wex + (size_t)(n0 + c) * ldw + t) : 0.f;
+    }
+    const int c0 = n0 + 4 * lane;
+    for (int r0 = blockIdx.y * XWIDE_ROWS; r0 < M; r0 += gridDim.y * XWIDE_ROWS) {
+        const int rows = min(XWIDE_ROWS, M - r0);
+        __syncthreads();                            // ws complete / the previous chunk's xs consumed
+        for (int i = threadIdx.x; i < rows * E; i += blockDim.x) {
+            const int r = i / E, t = i - r * E;
+            xs[r][t] = __ldg(ex + (size_t)(r0 + r) * ldex + t);
+        }
+        __syncthreads();
+        if (c0 >= o) continue;
+        float a[4][4];
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            const int r = warp + 8 * u;
+            if (r < rows) {
+                const float* yr = y + (size_t)(r0 + r) * ldy + c0;
+                if (VEC) {
+                    const float4 v = *reinterpret_cast<const float4*>(yr);
+                    a[u][0] = v.x; a[u][1] = v.y; a[u][2] = v.z; a[u][3] = v.w;
+                } else {
+#pragma unroll
+                    for (int c = 0; c < 4; c++) a[u][c] = c0 + c < o ? yr[c] : 0.f;
+                }
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < 4; u++) {
+            const int r = warp + 8 * u;
+            if (r >= rows) continue;
+#pragma unroll 4
+            for (int t = 0; t < E; t++) {
+                const float e = xs[r][t];
+                const float4 w = *reinterpret_cast<const float4*>(&ws[t][4 * lane]);
+                a[u][0] = fmaf(e, w.x, a[u][0]); a[u][1] = fmaf(e, w.y, a[u][1]); a[u][2] = fmaf(e, w.z, a[u][2]); a[u][3] = fmaf(e, w.w, a[u][3]);
+            }
+            constexpr int K = KIND >= 0 ? KIND : 0;
+#pragma unroll
+            for (int c = 0; c < 4; c++) a[u][c] = KIND < 0 ? a[u][c] : (VEC ? act_fast<K>(a[u][c]) : act_exact<K>(a[u][c]));
+            float* yr = y + (size_t)(r0 + r) * ldy + c0;
+            if (VEC) {
+                *reinterpret_cast<float4*>(yr) = make_float4(a[u][0], a[u][1], a[u][2], a[u][3]);
+            } else {
+#pragma unroll
+                for (int c = 0; c < 4; c++) if (c0 + c < o) yr[c] = a[u][c];
+            }
+        }
+    }
+}
 extern "C" int go1_mlp_extra_forward(float* y, int ldy, const float* extra, int ldex, const float* w_extra, int ldw, int M, int o, int E, int act,
                                      void* stream) {
-    if (!y || !extra || !w_extra || M <= 0 || o <= 0 || E < 1 || E > 4 || act < 0 || act_mode(act) > 1) return go1_set_error("go1_mlp_extra_forward: bad arguments");
+    if (!y || !extra || !w_extra || M <= 0 || o <= 0 || act < 0 || act_mode(act) > 1) return go1_set_error("go1_mlp_extra_forward: bad arguments");
+    if (E < 1 || E > XWIDE_MAX_E) return go1_set_error("go1_mlp_extra_forward: E (trailing input columns) must be 1..64");
+    if (ldy < o || ldex < E || ldw < E) return go1_set_error("go1_mlp_extra_forward: row strides must be >= o (y) and >= E (extra, w_extra)");
     const int kind = act_kind(act);
     act = act_mode(act);
     if (!go1_act_kind_ok(kind)) return go1_set_error("go1_mlp_extra_forward: unknown activation kind (Go1Activation)");
+    if (E > 4) {
+        const bool vec = (o & 3) == 0 && (ldy & 3) == 0 && (((uintptr_t)y) & 15) == 0;
+        const int gx = (o + XWIDE_COLS - 1) / XWIDE_COLS;
+        const int gy = min((M + XWIDE_ROWS - 1) / XWIDE_ROWS, max(1, (132 * 4 + gx - 1) / gx));
+        const dim3 grid(gx, gy);
+#define LAUNCH(KD, V) extra_fwd_wide_kernel<KD, V><<<grid, 256, 0, (cudaStream_t)stream>>>(y, ldy, extra, ldex, w_extra, ldw, M, o, E)
+        if (act == 0) { if (vec) LAUNCH(-1, true); else LAUNCH(-1, false); }
+        else if (vec) { GO1_ACT_SWITCH(kind, KD, LAUNCH(KD, true);) }
+        else { GO1_ACT_SWITCH(kind, KD, LAUNCH(KD, false);) }
+#undef LAUNCH
+        go1_count_launch(1);
+        return cuda_rc("go1_mlp_extra_forward");
+    }
     const int o4 = o / 4;
     if ((o & 3) == 0 && (ldy & 3) == 0 && (((uintptr_t)y) & 15) == 0 && o4 <= 256 && 256 % o4 == 0) {
         const int rpb = 256 / o4;
@@ -919,18 +997,116 @@ __global__ void zero_small_kernel(float* p, int ld, int rows, int cols) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < rows * cols) p[(size_t)(i / cols) * ld + (i % cols)] = 0.f;
 }
-extern "C" int go1_mlp_extra_backward(const float* dz, int lddz, const float* extra, int ldex, const float* w_extra, int ldw, float* g_w_extra, int ldgw,
-                                      float* dextra, int ldde, int M, int o, int E, int accumulate, void* stream) {
-    if (!dz || !extra || !g_w_extra || M <= 0 || o <= 0 || E <= 0 || E > 4) return go1_set_error("go1_mlp_extra_backward: bad arguments");
-    cudaStream_t st = (cudaStream_t)stream;
-    if (dextra) {
-        if (!w_extra) return go1_set_error("go1_mlp_extra_backward: dextra needs w_extra");
-        extra_dinput_kernel<<<(M * 32 + 255) / 256, 256, 0, st>>>(dz, lddz, w_extra, ldw, dextra, ldde, M, o, E); go1_count_launch(1);
+// Wide variants (E up to EB = 8 / 16 / 32 / 64; also every E of a transposed dz).
+// d(extra): one thread per row m with its EB sums in registers; w_extra is staged in shared memory 64 rows at a time (zero beyond E) and
+// read as broadcasts.  DZT: dz is [o][M] (the transposed first-layer dz the dgrad epilogue stores; coalesced along m), else [M][o].
+template <int EB, bool DZT>
+__global__ void __launch_bounds__(128) extra_dinput_wide_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ We, int ldw,
+                                                                float* __restrict__ dextra, int ldde, int M, int o, int E) {
+    __shared__ __align__(16) float ws[64][EB];
+    const int m = blockIdx.x * blockDim.x + threadIdx.x;
+    float acc[EB];
+#pragma unroll
+    for (int t = 0; t < EB; t++) acc[t] = 0.f;
+    for (int j0 = 0; j0 < o; j0 += 64) {
+        const int nj = min(64, o - j0);
+        __syncthreads();
+        for (int i = threadIdx.x; i < 64 * EB; i += blockDim.x) {
+            const int jj = i / EB, t = i - jj * EB;
+            ws[jj][t] = jj < nj && t < E ? __ldg(We + (size_t)(j0 + jj) * ldw + t) : 0.f;
+        }
+        __syncthreads();
+        if (m >= M) continue;
+        const float* p = DZT ? dz + (size_t)j0 * lddz + m : dz + (size_t)m * lddz + j0;
+        const size_t step = DZT ? (size_t)lddz : 1;
+#pragma unroll 4
+        for (int jj = 0; jj < nj; jj++, p += step) {
+            const float d = *p;
+#pragma unroll
+            for (int t = 0; t < EB; t += 4) {
+                const float4 w = *reinterpret_cast<const float4*>(&ws[jj][t]);
+                acc[t] = fmaf(d, w.x, acc[t]); acc[t + 1] = fmaf(d, w.y, acc[t + 1]); acc[t + 2] = fmaf(d, w.z, acc[t + 2]); acc[t + 3] = fmaf(d, w.w, acc[t + 3]);
+            }
+        }
     }
-    if (!accumulate) { zero_small_kernel<<<(o * E + 255) / 256, 256, 0, st>>>(g_w_extra, ldgw, o, E); go1_count_launch(1); }
-    const int rpb = 64;
-    dim3 grid((o + 255) / 256, (M + rpb - 1) / rpb);
-    extra_wgrad_kernel<<<grid, 256, 0, st>>>(dz, lddz, extra, ldex, g_w_extra, ldgw, M, o, E, rpb); go1_count_launch(1);
+    if (m >= M) return;
+#pragma unroll
+    for (int t = 0; t < EB; t++) if (t < E) dextra[(size_t)m * ldde + t] = acc[t];
+}
+// weight gradient: one thread per column j with its EB sums in registers over the CTA's row slab; the slab's extra rows are staged in
+// shared memory 32 at a time (zero beyond E) and read as broadcasts; E atomics per thread at the end.
+template <int EB>
+__global__ void __launch_bounds__(128) extra_wgrad_wide_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ extra, int ldex,
+                                                               float* __restrict__ gWe, int ldgw, int M, int o, int E, int rows_per_block) {
+    __shared__ __align__(16) float xs[32][EB];
+    const int r0 = blockIdx.y * rows_per_block, r1 = min(M, r0 + rows_per_block);
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    float acc[EB];
+#pragma unroll
+    for (int t = 0; t < EB; t++) acc[t] = 0.f;
+    for (int m0 = r0; m0 < r1; m0 += 32) {
+        const int nr = min(32, r1 - m0);
+        __syncthreads();
+        for (int i = threadIdx.x; i < 32 * EB; i += blockDim.x) {
+            const int r = i / EB, t = i - r * EB;
+            xs[r][t] = r < nr && t < E ? __ldg(extra + (size_t)(m0 + r) * ldex + t) : 0.f;
+        }
+        __syncthreads();
+        if (j >= o) continue;
+#pragma unroll 4
+        for (int r = 0; r < nr; r++) {
+            const float d = dz[(size_t)(m0 + r) * lddz + j];
+#pragma unroll
+            for (int t = 0; t < EB; t += 4) {
+                const float4 x = *reinterpret_cast<const float4*>(&xs[r][t]);
+                acc[t] = fmaf(d, x.x, acc[t]); acc[t + 1] = fmaf(d, x.y, acc[t + 1]); acc[t + 2] = fmaf(d, x.z, acc[t + 2]); acc[t + 3] = fmaf(d, x.w, acc[t + 3]);
+            }
+        }
+    }
+    if (j >= o) return;
+#pragma unroll
+    for (int t = 0; t < EB; t++) if (t < E) atomicAdd(gWe + (size_t)j * ldgw + t, acc[t]);
+}
+#define XWIDE_EB_SWITCH(E, EBV, ...)                                                   \
+    if ((E) <= 8) { constexpr int EBV = 8; __VA_ARGS__ }                               \
+    else if ((E) <= 16) { constexpr int EBV = 16; __VA_ARGS__ }                        \
+    else if ((E) <= 32) { constexpr int EBV = 32; __VA_ARGS__ }                        \
+    else { constexpr int EBV = 64; __VA_ARGS__ }
+extern "C" int go1_mlp_extra_backward(const float* dz, int lddz, int dz_transposed, const float* extra, int ldex, const float* w_extra, int ldw,
+                                      float* g_w_extra, int ldgw, float* dextra, int ldde, int M, int o, int E, int accumulate, void* stream) {
+    if (!dz || M <= 0 || o <= 0) return go1_set_error("go1_mlp_extra_backward: bad arguments");
+    if (E < 1 || E > XWIDE_MAX_E) return go1_set_error("go1_mlp_extra_backward: E (trailing input columns) must be 1..64");
+    if (!g_w_extra && !dextra) return go1_set_error("go1_mlp_extra_backward: nothing to compute (g_w_extra and dextra are NULL)");
+    if (dextra && (!w_extra || ldw < E || ldde < E)) return go1_set_error("go1_mlp_extra_backward: dextra needs w_extra, ldw >= E and ldde >= E");
+    if (g_w_extra && (!extra || ldex < E || ldgw < E)) return go1_set_error("go1_mlp_extra_backward: g_w_extra needs extra, ldex >= E and ldgw >= E");
+    if (g_w_extra && dz_transposed) return go1_set_error("go1_mlp_extra_backward: the weight gradient takes dz as [M][o] (dz_transposed 0)");
+    if (lddz < (dz_transposed ? M : o)) return go1_set_error("go1_mlp_extra_backward: lddz must be >= o ([M][o] dz) or >= M ([o][M] dz)");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (E <= 4 && !dz_transposed) {
+        if (dextra) { extra_dinput_kernel<<<(M * 32 + 255) / 256, 256, 0, st>>>(dz, lddz, w_extra, ldw, dextra, ldde, M, o, E); go1_count_launch(1); }
+        if (g_w_extra) {
+            if (!accumulate) { zero_small_kernel<<<(o * E + 255) / 256, 256, 0, st>>>(g_w_extra, ldgw, o, E); go1_count_launch(1); }
+            const int rpb = 64;
+            dim3 grid((o + 255) / 256, (M + rpb - 1) / rpb);
+            extra_wgrad_kernel<<<grid, 256, 0, st>>>(dz, lddz, extra, ldex, g_w_extra, ldgw, M, o, E, rpb); go1_count_launch(1);
+        }
+        return cuda_rc("go1_mlp_extra_backward");
+    }
+    if (dextra) {
+        const unsigned grid = (unsigned)((M + 127) / 128);
+        if (dz_transposed) { XWIDE_EB_SWITCH(E, EB, extra_dinput_wide_kernel<EB, true><<<grid, 128, 0, st>>>(dz, lddz, w_extra, ldw, dextra, ldde, M, o, E);) }
+        else { XWIDE_EB_SWITCH(E, EB, extra_dinput_wide_kernel<EB, false><<<grid, 128, 0, st>>>(dz, lddz, w_extra, ldw, dextra, ldde, M, o, E);) }
+        go1_count_launch(1);
+    }
+    if (g_w_extra) {
+        if (!accumulate) { zero_small_kernel<<<(o * E + 255) / 256, 256, 0, st>>>(g_w_extra, ldgw, o, E); go1_count_launch(1); }
+        const int gx = (o + 127) / 128;
+        const int gy = min((M + 31) / 32, max(1, (132 * 4 + gx - 1) / gx));     // ~4 CTAs per SM; fewer slabs, fewer atomics
+        const int rpb = ((M + gy - 1) / gy + 31) / 32 * 32;
+        const dim3 grid(gx, (M + rpb - 1) / rpb);
+        XWIDE_EB_SWITCH(E, EB, extra_wgrad_wide_kernel<EB><<<grid, 128, 0, st>>>(dz, lddz, extra, ldex, g_w_extra, ldgw, M, o, E, rpb);)
+        go1_count_launch(1);
+    }
     return cuda_rc("go1_mlp_extra_backward");
 }
 __global__ void skinny_dgrad_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ W, int ldw, const float* __restrict__ y, int ldy,

@@ -191,7 +191,7 @@ def lib():
         "go1_elu_backward": ([vp, ip, vp, ip, vp, ip, ip, ip, vp], ip),
         "go1_act_backward": ([vp, ip, vp, ip, vp, ip, ip, ip, ip, vp], ip),
         "go1_mlp_extra_forward": ([vp, ip, vp, ip, vp, ip, ip, ip, ip, ip, vp], ip),
-        "go1_mlp_extra_backward": ([vp, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, ip, ip, vp], ip),
+        "go1_mlp_extra_backward": ([vp, ip, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, ip, ip, vp], ip),
         "go1_skinny_dgrad": ([vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, ip, vp], ip),
         "go1_skinny_dgrad_ex": ([vp, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, vp], ip),
         "go1_skinny_dgrad_act": ([vp, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, ip, vp], ip),

@@ -7,8 +7,9 @@ the reference's names, .act / .evaluate / .act_student / .act_teacher / .get_act
   * all parameters are views into ONE flat fp32 buffer (adaptation module first), gradients into one flat
     gradient buffer -> one grad-norm, one Adam launch, one NCCL all-reduce per optimizer step;
   * forward and backward are explicit go1_gemm calls (fp32 CUDA-core or wgmma TF32) with fused
-    bias+activation epilogues (AC_Args.activation: every name of the reference's get_activation); cat(obs_history, latent) is never materialised (the 2 extra input columns are a
-    second, K=2 GEMM accumulated into the first layer's pre-activation);
+    bias+activation epilogues (AC_Args.activation: every name of the reference's get_activation); cat(obs_history, latent) is never materialised (the E = num_privileged_obs trailing
+    input columns are added to the first layer's pre-activation: in the GEMM epilogue for E <= 4, by go1_mlp_extra_forward after
+    the product for 4 < E <= 64);
   * no autograd graph: the backward pass is written out (see `backward_ppo`, `backward_adaptation`).
 """
 import torch
@@ -176,7 +177,11 @@ class _Net:
                     ldw = KPk
                 else:
                     tc = False
-            if first_extra:     # y = act(x W[:, :K0]^T + extra W[:, K0:]^T + b): the 2 trailing columns ride in the epilogue
+            if first_extra and i - K0 > 4:      # wide trailing input: y = x W[:, :K0]^T + b, then y = act(y + extra W[:, K0:]^T)
+                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, o, b, 0, 0, 1 if tc else 0)
+                capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(y), o, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i, M, o, i - K0,
+                                                            capi.act_arg(self.kind, act), capi.stream_ptr()), "go1_mlp_extra_forward")
+            elif first_extra:   # y = act(x W[:, :K0]^T + extra W[:, K0:]^T + b): the (at most 4) trailing columns ride in the epilogue
                 self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, o, b, act, 0, 1 if tc else 0, extra=extra, w_extra=W.data_ptr() + 4 * K0, ld_w_extra=i)
             else:
                 self._gemm(0, 1, M, o, K, inp, ld_in, Wm, ldw, y, o, b, act, 0, 1 if tc else 0)
@@ -273,12 +278,15 @@ class _Net:
                 else:
                     self._gemm(1, 0, o, K, M, dz, ldz, inp, ld_in, gW, i, None, 0, 1 if tc else 0, 1 if tc else 0)
             if li == 0:
-                if extra is not None and not extra_done:
+                # trailing-input gradients the layer-2 dgrad epilogue did not reduce: d(extra) from dz in either layout, the weight
+                # gradient only from a row-major dz (a transposed one is _first_layer_wgrad's augmented product)
+                if extra is not None and not extra_done and (want_dextra or dz1T is None):
                     E = i - K0
                     if want_dextra:
                         dextra = self._buf((tag, "dextra"), M, E)
-                    capi.check(L.go1_mlp_extra_backward(capi.ptr(dz), ldz, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i, gW.data_ptr() + 4 * K0, i,
-                                                        capi.ptr(dextra) if want_dextra else None, E, M, o, E, 0, st), "extra_backward")
+                    gwx = gW.data_ptr() + 4 * K0 if dz1T is None else None
+                    capi.check(L.go1_mlp_extra_backward(capi.ptr(dz), ldz, 0 if dz1T is None else 1, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i,
+                                                        gwx, i, capi.ptr(dextra) if want_dextra else None, E, M, o, E, 0, st), "extra_backward")
                 return dextra
             # ---- 3. dgrad (+ fused activation derivative): dz_prev[M][i] = (dz[M][o] W[o][i]) * f'(y_prev)
             pwo, pbo, po, pi = self.specs[li - 1]
@@ -289,7 +297,7 @@ class _Net:
             if impl == 1 and self._tma_ok(dz, ldz) and self._tma_ok(W, i) and M >= 64:      # (the 12-wide actor head included: 19 us here, 22 us on the skinny pass)
                 # W read MN-major in place; the bias gradient of layer li-1 (column sums of dprev) rides in the epilogue
                 bx = None
-                if li == 1 and extra is not None and (to_T or 1 <= pi - K0 <= 4):
+                if li == 1 and extra is not None and 1 <= pi - K0 <= 4:
                     # dprev is the first layer's dz: d(extra), and the trailing-input weight gradient unless _first_layer_wgrad makes it,
                     # are reduced in this epilogue too
                     extra_done = True
@@ -317,6 +325,7 @@ class _Net:
 class ActorCritic(nn.Module):
     is_recurrent = False
     HEAD = 16          # floats reserved in front of the flat parameter / gradient buffers (see flatten())
+    MAX_PRIVILEGED_OBS = 64     # widest trailing input the kernels take (go1_mlp_extra_forward / _backward); the eleven priv_observe_* groups give 45
 
     def __init__(self, num_obs, num_privileged_obs, num_obs_history, num_actions, **kwargs):
         if kwargs:
@@ -327,6 +336,8 @@ class ActorCritic(nn.Module):
         if activation not in capi.ACTIVATIONS:
             raise ValueError(f"AC_Args.activation = {activation!r}: expected one of {sorted(capi.ACTIVATIONS)}")
         self.act_kind = capi.ACTIVATIONS[activation]      # fixed per instance: it is baked into the captured CUDA graphs
+        if not 1 <= num_privileged_obs <= self.MAX_PRIVILEGED_OBS:
+            raise ValueError(f"num_privileged_obs = {num_privileged_obs}: the learner kernels take 1..{self.MAX_PRIVILEGED_OBS} privileged observations")
         self.num_obs_history, self.num_privileged_obs, self.num_actions = num_obs_history, num_privileged_obs, num_actions
         self.adaptation_module = _mlp(num_obs_history, AC_Args.adaptation_module_branch_hidden_dims, num_privileged_obs, activation)
         self.actor_body = _mlp(num_privileged_obs + num_obs_history, AC_Args.actor_hidden_dims, num_actions, activation)
@@ -457,9 +468,10 @@ class ActorCritic(nn.Module):
 
     def forward_all(self, observation_history, privileged_observations, tag="act"):
         """update_distribution + evaluate in one pass.  With the tensor-core path the first layers of the three MLPs --
-        which all read obs_history -- run as ONE product [M][256+512+512] = h Wcat^T: bias + activation (+ the critic's two
+        which all read obs_history -- run as ONE product [M][256+512+512] = h Wcat^T: bias + activation (+ the critic's E <= 4
         privileged columns) ride in its epilogue for the adaptation/critic slices; the actor slice is finished
-        (latent columns + activation) by go1_mlp_extra_forward once the adaptation module has produced the latent."""
+        (latent columns + activation) by go1_mlp_extra_forward once the adaptation module has produced the latent.  With E > 4 the
+        epilogue finishes only the adaptation slice and go1_mlp_extra_forward also finishes the critic slice (priv columns)."""
         self.flatten()
         self._check_input(observation_history)
         h, priv = observation_history, privileged_observations.contiguous()
@@ -467,7 +479,7 @@ class ActorCritic(nn.Module):
         nets = self._nets
         na, npol, ncr = nets["adapt"], nets["actor"], nets["critic"]
         E = self.num_privileged_obs
-        fused = impl == 1 and _Net._tma_ok(h, h.stride(0)) and K0 % 4 == 0 and 1 <= E <= 4 and \
+        fused = impl == 1 and _Net._tma_ok(h, h.stride(0)) and K0 % 4 == 0 and 1 <= E <= self.MAX_PRIVILEGED_OBS and \
             npol.specs[0][3] == K0 + E and ncr.specs[0][3] == K0 + E and na.specs[0][3] == K0
         if not fused:
             self.update_distribution(h, tag)
@@ -494,9 +506,14 @@ class ActorCritic(nn.Module):
 
         Wcat, bcat, xcat = na._cached(("l1cat", "all"), build_all)
         y = na._buf((tag, "y1cat"), M, oa + oc + op)
-        na._gemm(0, 1, M, oa + oc + op, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1,
-                 extra=priv, w_extra=xcat.data_ptr(), ld_w_extra=E, lead_cols=oa + oc)
         ya, yc, yp = y[:, :oa], y[:, oa:oa + oc], y[:, oa + oc:]
+        if E <= 4:
+            na._gemm(0, 1, M, oa + oc + op, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1,
+                     extra=priv, w_extra=xcat.data_ptr(), ld_w_extra=E, lead_cols=oa + oc)
+        else:       # wide privileged input: only the adaptation slice is finished in the epilogue; the critic slice gets priv here
+            na._gemm(0, 1, M, oa + oc + op, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1, lead_cols=oa)
+            capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(yc), yc.stride(0), capi.ptr(priv), priv.stride(0), Wc.data_ptr() + 4 * K0, K0 + E,
+                                                        M, oc, E, capi.act_arg(self.act_kind, 1), capi.stream_ptr()), "go1_mlp_extra_forward")
         pair = self.fuse_tail and npol._tail_ok(yp, yp.stride(0), M) and ncr._tail_ok(yc, yc.stride(0), M) and \
             [sp[2:] for sp in npol.specs[1:-1]] == [sp[2:] for sp in ncr.specs[1:-1]] and npol.specs[-1][2] + ncr.specs[-1][2] <= 16
         side = None if pair else self._side_stream(M)
@@ -640,7 +657,7 @@ class ActorCritic(nn.Module):
     def _first_layers_fusable(self, h, priv):
         """The first layers of the three nets can run their backward as one K-major product over hT (history_kmajor)."""
         nets, K0, E = self._nets, self.num_obs_history, self.num_privileged_obs
-        return self._impl() == 1 and h.shape[0] >= 64 and _Net._tma_ok(h, h.stride(0)) and 1 <= E <= 4 and priv.shape[1] == E and \
+        return self._impl() == 1 and h.shape[0] >= 64 and _Net._tma_ok(h, h.stride(0)) and 1 <= E <= self.MAX_PRIVILEGED_OBS and priv.shape[1] == E and \
             nets["actor"].specs[0][3] == K0 + E and nets["critic"].specs[0][3] == K0 + E and nets["adapt"].specs[0][3] == K0
 
     def _first_layer_wgrad(self, names, dz1T, hT, M, tag):

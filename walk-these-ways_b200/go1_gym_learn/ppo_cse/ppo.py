@@ -231,8 +231,12 @@ class PPO:
                 outs = ac.adaptation_forward(hist_b)
                 pred = outs[-1]
                 dpred = ac._nets["adapt"]._buf(("adapt", "dpred"), M, pred.shape[1])
+                # selective_adaptation_module_loss: train and test MSE of privileged column 0 only (ppo.py:177-183)
+                dim = 1 if PPO_Args.selective_adaptation_module_loss else pred.shape[1]
+                if dim < pred.shape[1]:
+                    dpred[:, dim:].zero_()
                 capi.check(L.go1_ppo_mse(capi.ptr(pred), pred.stride(0), capi.ptr(priv_b), priv_b.stride(0), capi.ptr(dpred), dpred.stride(0),
-                                         capi.ptr(self._mse_scalars), M, num_train, pred.shape[1], st()), "mse")
+                                         capi.ptr(self._mse_scalars), M, num_train, dim, st()), "mse")
                 ac.backward_adaptation(hist_b, outs, dpred, hT=getattr(hist_b, "hT", None))
                 if self.process_group is not None:      # adaptation gradients + the MSE pair (buffer head) in one averaging all-reduce
                     import torch.distributed as dist
