@@ -25,6 +25,7 @@ extern "C" {
 #define GO1_MAX_PRIV_OBS 48
 #define GO1_EVENT_STRIDE 6        /* floats per event record */
 #define GO1_RESET_RAND_STRIDE 48  /* injected uniform draws per env (Go1SimBuffers.reset_rand) */
+#define GO1_MAX_LAG_TIMESTEPS 32  /* action FIFO slots reserved per leg in leg_f32 (3 rows each, "lag_buffer") */
 
 /* reward term ids: one per CoRLRewards._reward_<name> (go1_gym/envs/rewards/corl_rewards.py:15-201) */
 enum Go1RewardTerm {
@@ -65,7 +66,9 @@ typedef struct Go1SimConfig {
     float clip_actions, clip_obs;       /* Cfg.normalization */
     int32_t control_type;               /* 0 = actuator_net, 1 = P   (legged_robot.py:928-943) */
     float action_scale, hip_scale_reduction, kp, kd;
-    int32_t use_lag;                    /* Cfg.domain_rand.randomize_lag_timesteps (lag_timesteps must be 6) */
+    int32_t use_lag;                    /* Cfg.domain_rand.randomize_lag_timesteps */
+    int32_t lag_timesteps;              /* Cfg.domain_rand.lag_timesteps: depth L of the action FIFO in physics substeps,
+                                         * 0..GO1_MAX_LAG_TIMESTEPS (legged_robot.py:922-924); ignored when use_lag = 0 */
     float default_dof_pos[GO1_NUM_DOF];
     float soft_limit_lo[GO1_NUM_DOF], soft_limit_hi[GO1_NUM_DOF];   /* legged_robot.py:603-607 */
     float torque_limit;

@@ -129,6 +129,9 @@ static int check_cfg(const Go1SimConfig* c) {
     if (c->num_priv_obs < 0 || c->num_priv_obs > GO1_MAX_PRIV_OBS) return fail("num_priv_obs out of range");
     if (c->num_commands < 3 || c->num_commands > GO1_NUM_COMMANDS) return fail("num_commands out of range");
     if (c->decimation <= 0 || c->sim_dt <= 0.f) return fail("bad sim_dt/decimation");
+    if (c->lag_timesteps < 0 || c->lag_timesteps > GO1_MAX_LAG_TIMESTEPS) {
+        char b[96]; snprintf(b, sizeof b, "lag_timesteps (%d) must be in 0..%d", c->lag_timesteps, GO1_MAX_LAG_TIMESTEPS); return fail(b);
+    }
     if (c->num_active_rewards < 0 || c->num_active_rewards > GO1_NUM_REWARD_TERMS) return fail("bad num_active_rewards");
     for (int i = 0; i < c->num_active_rewards; i++)
         if (c->reward_order[i] < 0 || c->reward_order[i] >= GO1_NUM_REWARD_TERMS) return fail("bad reward_order entry");

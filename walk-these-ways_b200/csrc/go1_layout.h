@@ -17,7 +17,7 @@
 
 #define GO1_LEG_F32_FIELDS(X) \
     X(dof_pos, 3) X(dof_vel, 3) X(last_dof_vel, 3) X(actions, 3) X(last_actions, 3) X(last_last_actions, 3) \
-    X(joint_pos_target, 3) X(last_joint_pos_target, 3) X(last_last_joint_pos_target, 3) X(lag_buffer, 18) \
+    X(joint_pos_target, 3) X(last_joint_pos_target, 3) X(last_last_joint_pos_target, 3) X(lag_buffer, 3 * GO1_MAX_LAG_TIMESTEPS) \
     X(joint_pos_err_last, 3) X(joint_pos_err_last_last, 3) X(joint_vel_last, 3) X(joint_vel_last_last, 3) \
     X(motor_offsets, 3) X(torques, 3) \
     X(clock_inputs, 1) X(doubletime_clock_inputs, 1) X(halftime_clock_inputs, 1) \

@@ -30,6 +30,7 @@ NUM_COMMAND_SUMS = NUM_REWARD_TERMS + 5
 COMMAND_SUM_EXTRAS = ["lin_vel_raw", "ang_vel_raw", "lin_vel_residual", "ang_vel_residual", "ep_timesteps"]
 
 RESET_RAND_STRIDE = 48
+MAX_LAG_TIMESTEPS = 32
 _i, _f = C.c_int32, C.c_float
 
 
@@ -51,7 +52,7 @@ class Go1SimConfig(C.Structure):
     _fields_ = [
         ("num_envs", _i), ("num_train_envs", _i), ("sim_dt", _f), ("decimation", _i),
         ("clip_actions", _f), ("clip_obs", _f), ("control_type", _i),
-        ("action_scale", _f), ("hip_scale_reduction", _f), ("kp", _f), ("kd", _f), ("use_lag", _i),
+        ("action_scale", _f), ("hip_scale_reduction", _f), ("kp", _f), ("kd", _f), ("use_lag", _i), ("lag_timesteps", _i),
         ("default_dof_pos", _f * NUM_DOF), ("soft_limit_lo", _f * NUM_DOF), ("soft_limit_hi", _f * NUM_DOF),
         ("torque_limit", _f),
         ("num_commands", _i), ("observe_gait_commands", _i), ("pacing_offset", _i), ("kappa_gait_probs", _f),

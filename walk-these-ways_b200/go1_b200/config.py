@@ -207,8 +207,13 @@ def build_sim_config(cfg, num_envs=None, num_train_envs=None, seed=0, physics=No
     c.hip_scale_reduction = cfg.control.hip_scale_reduction
     c.kp, c.kd = pd_gains(cfg)
     c.use_lag = int(bool(cfg.domain_rand.randomize_lag_timesteps))
-    if c.use_lag and int(cfg.domain_rand.lag_timesteps) != 6:
-        raise ValueError("the fused step kernel keeps a 6-deep action FIFO: Cfg.domain_rand.lag_timesteps must be 6")
+    # without randomize_lag_timesteps the reference never reads its FIFO (legged_robot.py:921-926), so it needs no rows here
+    if c.use_lag:
+        lag = cfg.domain_rand.lag_timesteps
+        if int(lag) != lag or not 0 <= lag <= capi.MAX_LAG_TIMESTEPS:
+            raise ValueError(f"Cfg.domain_rand.lag_timesteps ({lag!r}) must be an integer in 0..{capi.MAX_LAG_TIMESTEPS}: "
+                             "the fused step kernel reserves that many action FIFO slots")
+        c.lag_timesteps = int(lag)
     c.default_dof_pos[:] = default_dof_pos(cfg).tolist()
     lo, hi = soft_limits(cfg, model)
     c.soft_limit_lo[:] = lo.tolist()
