@@ -19,6 +19,9 @@
 //               (staged epilogue), red.global.add.v4 when split-K partitions the reduction
 //   warp 8      TMA producer: cp.async.bulk.tensor 2D loads of the A and B boxes of a k-block into a ring of 3-8 stages guarded by
 //               full / empty mbarriers; it runs ahead into the next tile while the consumers are in their epilogue
+// The long-K products with K-major operands (the first layers' forward and weight gradient) run as clusters of two CTAs working
+// adjacent tiles: each CTA loads half of the operand box the pair shares and multicasts it to both, so the pair reads 24 KB instead
+// of 32 KB per k-block from L2 (full-chip, these products are bound by the L2-to-SM operand stream, not by the tensor cores).
 // mlp_tail_fwd_kernel chains two such products and a CUDA-core head for the layers behind a first layer.
 #include <cuda_runtime.h>
 #include <cuda.h>
@@ -66,6 +69,29 @@ __device__ __forceinline__ bool elect_one() {
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                  ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
+}
+// the same box delivered to the same shared-memory offset and mbarrier of every CTA of the cluster in cta_mask
+__device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap* map, uint64_t* bar, void* dst, int c0, int c1, uint16_t cta_mask) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
+                 ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask) : "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// every thread of every CTA of the cluster (threads may arrive from different places in the code)
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster.  Default (.release.cta) semantics.  The only
+// ordering this arrive provides is read-before-write: the caller's wgmma.wait_group has retired the tensor core's (async-proxy) reads of
+// the stage before the peer's TMA overwrites it.  It publishes no generic-proxy writes to the peer at cluster scope, and nothing may come
+// to rely on it doing so.  (A .release.cluster arrive would also wait for the thread's outstanding global writes, once per k-block.)
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+    uint32_t remote;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(smem_u32(bar)), "r"(rank));
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 // named barriers of the consumer warps (the producer warp never joins them): 1 = both warpgroups, 2 / 3 = one warpgroup
 __device__ __forceinline__ void cons_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
@@ -123,7 +149,8 @@ struct GemmArgs {
     float* Cg[4]; int nprob, tiles_per_prob;
 };
 constexpr int GEMM_MAXP = 4;
-struct GemmMaps { CUtensorMap a[GEMM_MAXP], b[GEMM_MAXP]; };
+// half: the 64-row box of the operand a CTA pair shares (cluster launches: see gemm_tf32_wgmma)
+struct GemmMaps { CUtensorMap a[GEMM_MAXP], b[GEMM_MAXP], half; };
 
 // Per-warp shared-memory staging of the staged epilogue.  A row-per-lane float4 store touches 32 different 128-byte lines per
 // instruction (8 x the LSU wavefronts of a coalesced store), which bounds every short-K product.  Staged: the warp's
@@ -337,12 +364,20 @@ __device__ __forceinline__ bool epilogue_prefetch(const GemmArgs& g, const int r
 // one wave share A tiles through L2).  Shared memory: [ring: stages x (A | B)][X: 64 KB][derivative operand staging 8 x 4 KB][barriers].
 // X serves the main loop as the double-buffered transposed tiles of MN-major operands (A 2 x 16 KB, B 2 x 16 KB) and the epilogue
 // as the accumulator / output staging (32 KB per warpgroup).
+// CL = 2 (K-major operands, one problem, BN = 128): clusters of two CTAs walk pairs of adjacent tiles, paired along N when tiles_n is
+// even (the pair shares its A box) and along M otherwise (tiles_m even: the pair shares its B box).  Per k-block each CTA loads its
+// own box of the other operand and rank r's 64-row half of the shared box, multicast into both CTAs at byte offset r x 8 KB of the
+// shared operand's slot (the 128B swizzle repeats every 1 KB, so the two halves form the same tile one 128-row box forms).  Both
+// producers write every stage of both rings: empty[s] counts the consumer warps of both CTAs, and each consumer warp releases a
+// stage in its own CTA and in its peer.  Cluster barriers after the mbarrier initialisation and before any thread exits keep a CTA
+// alive while its peer may still multicast into it or arrive on its barriers.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int X_BYTES = 65536;
-template <int BN, bool ANYKIND>
+template <int BN, bool ANYKIND, int CL>
 __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __grid_constant__ GemmMaps gm,
                                                                       const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
                                                                       const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
+    static_assert(CL == 1 || (CL == 2 && BN == BM), "CTA pairs share 128-row operand boxes");
     constexpr int G = EPI_G;
     constexpr int A_BYTES = BM * BK * 4, STAGE_BYTES = (BM + BN) * BK * 4;
     constexpr int MAX_STAGES = 8;
@@ -365,15 +400,30 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
         }
         if (g.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"(&mapC) : "memory");
         if (g.tma_aux) asm volatile("prefetch.tensormap [%0];" ::"l"(&mapY) : "memory");
-        for (int s = 0; s < stages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], NCONS); }
+        if (CL > 1) asm volatile("prefetch.tensormap [%0];" ::"l"(&gm.half) : "memory");
+        for (int s = 0; s < stages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], CL * NCONS); }
         for (int w = 0; w < NCONS; w++) mbar_init(&aux_bar[w], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    __syncthreads();
+    if (CL > 1) cluster_sync();      // the peer's barriers are initialised before any multicast or remote arrive reaches them
+    else __syncthreads();
 
+    // the work of this CTA: (pair-)tiles pt = first(), first() + step(), ... < npt; tile t = cta_tile(pt).  The block / cluster indices
+    // are read where they are used: held in registers across the whole kernel they cost the consumers spill slots.
+    const int npt = total_tiles / CL;
+    auto first = [] { return (int)blockIdx.x / CL; };
+    auto step = [] { return (int)gridDim.x / CL; };
+    auto rank = [] { return CL > 1 ? cluster_ctarank() : 0u; };
+    auto pair_n = [&] { return (tiles_n & 1) == 0; };
+    auto cta_tile = [&](int pt) -> int {
+        if (CL == 1) return pt;
+        if (pair_n()) return 2 * pt + (int)rank();                    // tiles (2 j, 2 j + 1) along N of one row of tiles
+        const int tn = pt % tiles_n, r = pt / tiles_n, hm = tiles_m / 2;
+        return ((r / hm) * tiles_m + 2 * (r % hm) + (int)rank()) * tiles_n + tn;     // tiles (2 j, 2 j + 1) along M of one split
+    };
     // tile -> (m0, n0, k-block range); grouped launches: tile t of problem t / tiles_per_prob
     auto tile_coords = [&](int t, int& m0, int& n0, int& kb0, int& nkb) {
-        if (g.nprob > 1) t %= g.tiles_per_prob;
+        if (CL == 1 && g.nprob > 1) t %= g.tiles_per_prob;
         const int tn = t % tiles_n; t /= tiles_n;
         const int tm = t % tiles_m; const int z = t / tiles_m;
         m0 = tm * BM; n0 = tn * BN; kb0 = z * g.kb_per_split; nkb = min(g.kb_per_split, num_kb_total - kb0);
@@ -383,9 +433,10 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
         // ===== TMA producer =====
         if (elect_one()) {
             int s = 0, ph = 0;      // ring position of this CTA's k-block stream
-            for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+            for (int pt = first(); pt < npt; pt += step()) {
+                const int t = cta_tile(pt);
                 int m0, n0, kb0, nkb; tile_coords(t, m0, n0, kb0, nkb);
-                const int p = g.nprob > 1 ? t / g.tiles_per_prob : 0;
+                const int p = CL == 1 && g.nprob > 1 ? t / g.tiles_per_prob : 0;
                 const CUtensorMap* mapA = &gm.a[p];
                 const CUtensorMap* mapB = &gm.b[p];
                 for (int i = 0; i < nkb; i++) {
@@ -393,40 +444,62 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
                     mbar_expect_tx(&full[s], STAGE_BYTES);
                     uint8_t* a = ring + (size_t)s * STAGE_BYTES;
                     uint8_t* b = a + A_BYTES;
-                    if (g.amn) tma_load_2d(mapA, &full[s], a, m0, (kb0 + i) * BK);        // box [32 k-rows][128 m]
-                    else tma_load_2d(mapA, &full[s], a, (kb0 + i) * BK, m0);              // box [128 m-rows][32 k]
-                    if (g.bmn) tma_load_2d(mapB, &full[s], b, n0, (kb0 + i) * BK);
-                    else tma_load_2d(mapB, &full[s], b, (kb0 + i) * BK, n0);
+                    if (CL > 1) {           // K-major: this CTA's half of the shared box to both CTAs, its own box of the other operand
+                        const int kc = (kb0 + i) * BK;
+                        if (pair_n()) {
+                            tma_load_2d_multicast(&gm.half, &full[s], a + rank() * (A_BYTES / 2), kc, m0 + (int)rank() * (BM / 2), 0x3);
+                            tma_load_2d(mapB, &full[s], b, kc, n0);
+                        } else {
+                            tma_load_2d(mapA, &full[s], a, kc, m0);
+                            tma_load_2d_multicast(&gm.half, &full[s], b + rank() * (A_BYTES / 2), kc, n0 + (int)rank() * (BN / 2), 0x3);
+                        }
+                    } else {
+                        if (g.amn) tma_load_2d(mapA, &full[s], a, m0, (kb0 + i) * BK);        // box [32 k-rows][128 m]
+                        else tma_load_2d(mapA, &full[s], a, (kb0 + i) * BK, m0);              // box [128 m-rows][32 k]
+                        if (g.bmn) tma_load_2d(mapB, &full[s], b, n0, (kb0 + i) * BK);
+                        else tma_load_2d(mapB, &full[s], b, (kb0 + i) * BK, n0);
+                    }
                     if (++s == stages) { s = 0; ph ^= 1; }
                 }
             }
         }
+        if (CL > 1) cluster_sync();
         return;
     }
-    if (warp > NCONS) return;
+    if (warp > NCONS) {
+        if (CL > 1) cluster_sync();
+        return;
+    }
 
     // ===== consumers: warpgroup wgi owns rows [64 wgi, 64 wgi + 64) of the tile =====
     const int wgi = warp >> 2, w = warp & 3, ctid = threadIdx.x;
     const int q = 2 * wgi + (w & 1), grp = w >> 1;      // epilogue: 32-row block q of the tile, column group grp
-    const bool tr = g.amn || g.bmn;
+    const bool tr = CL == 1 && (g.amn || g.bmn);        // pairs read K-major operands only, one problem
     const bool split = g.kb_per_split < num_kb_total;
-    const bool st_out = g.tma_store, st_aux = g.tma_aux;
+    const bool st_out = g.tma_store, st_aux = CL == 1 && g.tma_aux;      // pairs: no derivative operand (act 2)
     uint8_t* xwg = xreg + wgi * (X_BYTES / 2);          // this warpgroup's accumulator staging: [chunk][64 rows][128 B]
     uint8_t* my_aux = stage_aux + warp * 4096;
     uint64_t* my_bar = &aux_bar[warp];
     // derivative operand blocks run one chunk ahead of the epilogue: cursor (pt, pc) = the next chunk of this warp whose block has not been requested yet
-    int pt = blockIdx.x, pc = grp - G;
+    int pt = first(), pc = grp - G;
     auto next_chunk = [&]() -> bool {
         for (;;) {
             pc += G;
-            if (pc >= BN / 32) { pt += gridDim.x; pc = grp; }
-            if (pt >= total_tiles) return false;
-            if (pc < BN / 32 && (pt % tiles_n) * BN + 32 * pc < g.N) return true;
+            if (pc >= BN / 32) { pt += step(); pc = grp; }
+            if (pt >= npt) return false;
+            if (pc < BN / 32 && (cta_tile(pt) % tiles_n) * BN + 32 * pc < g.N) return true;
+        }
+    };
+    // stage s has been read: it returns to the producer of this CTA and, in a pair, to the peer's (whose half of it this CTA received)
+    auto release = [&](int s) {
+        if (lane == 0) {
+            mbar_arrive(&empty[s]);
+            if (CL > 1) mbar_arrive_cluster(&empty[s], rank() ^ 1);
         }
     };
     auto request_aux = [&]() {
         if (next_chunk() && lane == 0) {
-            int m0, n0, kb0, nkb; tile_coords(pt, m0, n0, kb0, nkb);
+            int m0, n0, kb0, nkb; tile_coords(cta_tile(pt), m0, n0, kb0, nkb);
             mbar_expect_tx(my_bar, 4096);
             tma_load_2d(&mapY, my_bar, my_aux, n0 + 32 * pc, m0 + 32 * q);
         }
@@ -435,7 +508,8 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
     uint32_t aux_phase = 0;
     int s = 0, ph = 0;
     float acc[BN / 2];
-    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    for (int tp = first(); tp < npt; tp += step()) {
+        const int t = cta_tile(tp);
         int m0, n0, kb0, nkb; tile_coords(t, m0, n0, kb0, nkb);
         // X is about to be rewritten: the TMA stores of the previous tile have read it
         if (st_out && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
@@ -450,7 +524,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
                 if (g.bmn) { uint8_t* tb = xreg + 2 * A_BYTES + (i & 1) * A_BYTES; transpose_tile<BN>((const float*)b, tb, ctid); b = tb; }
                 if (prev >= 0) {        // k-block i - 1 is done: its stage returns to the producer, and its transposed tiles may be rewritten next round
                     wg::wait<0>();
-                    if (lane == 0) mbar_arrive(&empty[prev]);
+                    release(prev);
                 }
                 fence_async_smem();     // generic-proxy writes -> visible to the tensor core (async proxy)
                 cons_sync();
@@ -460,19 +534,19 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
             wg::commit();
             if (!tr && prev >= 0) {
                 wg::wait<1>();
-                if (lane == 0) mbar_arrive(&empty[prev]);
+                release(prev);
             }
             prev = s;
             if (++s == stages) { s = 0; ph ^= 1; }
         }
         wg::wait<0>();
-        if (lane == 0) mbar_arrive(&empty[prev]);
+        release(prev);
         if (tr) cons_sync();            // both warpgroups are done with the transposed tiles that the staging overlays
 
         const int row = m0 + 32 * q + lane;
-        float* const Cbase = g.nprob > 1 ? g.Cg[t / g.tiles_per_prob] : g.C;
+        float* const Cbase = CL == 1 && g.nprob > 1 ? g.Cg[t / g.tiles_per_prob] : g.C;
         float4 ypre[8];
-        const bool have_pre = !st_aux && (grp < BN / 32) && epilogue_prefetch(g, row, n0 + 32 * grp, split, ypre);
+        const bool have_pre = CL == 1 && !st_aux && (grp < BN / 32) && epilogue_prefetch(g, row, n0 + 32 * grp, split, ypre);
         store_fragment<BN / 8>(acc, xwg, 0, w, lane, [](float2 v, int, int) { return v; });
         wg_sync(wgi);
 #pragma unroll 1
@@ -494,6 +568,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
         }
     }
     if (st_out && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // all stores of this warp have completed
+    if (CL > 1) cluster_sync();
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -581,7 +656,7 @@ __global__ void bias_act_strided(float* C, int ldc, const float* bias, int M, in
     *c = v;
 }
 
-template <int BN, bool ANYKIND>
+template <int BN, bool ANYKIND, int CL>
 int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st) {
     constexpr int STAGE_BYTES = (BM + BN) * BK * 4;
     const size_t staging = X_BYTES + (g.tma_aux ? (size_t)NCONS * 4096 : 0);
@@ -591,18 +666,40 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
     if (stages > 8) stages = 8;
     if (stages < 2) return go1_set_error("go1_gemm impl=1: no room for the operand ring");
     const size_t smem = (size_t)stages * STAGE_BYTES + fixed;
-    static bool configured = false;
-    if (!configured) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_tf32_wgmma<BN, ANYKIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget);
-        if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
-        configured = true;
-    }
+    auto kernel = gemm_tf32_wgmma<BN, ANYKIND, CL>;
     const int tiles_m = (g.M + BM - 1) / BM, tiles_n = (g.N + BN - 1) / BN;
     g.tiles_per_prob = tiles_m * tiles_n * splits;
     const int total = g.tiles_per_prob * (g.nprob > 1 ? g.nprob : 1);
-    const int sms = sm_count();
-    const int grid = total < sms ? total : sms;          // one CTA per SM (the ring and the staging fill its shared memory)
-    gemm_tf32_wgmma<BN, ANYKIND><<<grid, 32 * NCONS + 128, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages);
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = CL; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.blockDim = dim3(32 * NCONS + 128); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    static bool configured = false;
+    static int slots = 0;        // CTAs (clusters of CL) resident at once: one per SM, as far as the GPCs can place the clusters
+    if (!configured) {
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)budget);
+        if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
+        slots = sm_count();
+        if (CL > 1) {
+            cfg.gridDim = dim3(CL * sm_count());
+            int clusters = 0;
+            e = cudaOccupancyMaxActiveClusters(&clusters, kernel, &cfg);
+            if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
+            if (clusters < 1) return go1_set_error("go1_gemm impl=1: no CTA pair of the persistent GEMM fits a GPC");
+            slots = clusters;
+        }
+        configured = true;
+    }
+    // persistent grid: one CTA per SM (the ring and the staging fill its shared memory), CL x (pair-)tile slots for clusters
+    const int units = total / CL;
+    cfg.gridDim = dim3(CL * (units < slots ? units : slots));
+    if (CL == 1) kernel<<<cfg.gridDim, cfg.blockDim, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages);
+    else {
+        cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, gm, mc, my, g, tiles_m, tiles_n, total, stages);
+        if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
+    }
     go1_count_launch(1);
     return 0;
 }
@@ -867,7 +964,7 @@ static bool g_time_on = false;
 static std::vector<cudaEvent_t> g_time_events;
 static size_t g_time_used = 0;
 static double g_time_flop = 0.0;
-struct TimeRec { int M, N, K, amn, bmn, act, nex, splits, kern, colsum; };      // what each timed launch was (GO1_GEMM_TIMING_CSV dump)
+struct TimeRec { int M, N, K, amn, bmn, act, nex, splits, kern, colsum, cluster; };      // what each timed launch was (GO1_GEMM_TIMING_CSV dump)
 static std::vector<TimeRec> g_time_recs;
 static cudaEvent_t timing_event() {
     if (g_time_used == g_time_events.size()) { cudaEvent_t e; cudaEventCreate(&e); g_time_events.push_back(e); }
@@ -887,7 +984,8 @@ extern "C" int go1_gemm_timing(int on, double* total_ms, double* total_flop, lon
         if (csv && i / 2 < g_time_recs.size()) {
             const TimeRec& r = g_time_recs[i / 2];
             fprintf(csv, "%d,%d,%d,%d,%d,%d,%d,%d,%s,%d,%.2f\n", r.M, r.N, r.K, r.amn, r.bmn, r.act, r.nex, r.splits,
-                    r.kern >= 1000 ? (r.kern == 1003 ? "tail3" : "tail2") : (r.kern == 128 ? "p128" : (r.kern == 64 ? "p64" : "p32")), r.colsum, 1e3 * t);
+                    r.kern >= 1000 ? (r.kern == 1003 ? "tail3" : "tail2") : (r.kern == 128 ? (r.cluster == 2 ? "p128c2" : "p128") : (r.kern == 64 ? "p64" : "p32")),
+                    r.colsum, 1e3 * t);
         }
     }
     if (csv) fclose(csv);
@@ -938,6 +1036,15 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     }
     for (int p = nprob; p < GEMM_MAXP; p++) { gm.a[p] = gm.a[0]; gm.b[p] = gm.b[0]; }
     const CUtensorMap& ma = gm.a[0];
+    // CTA pairs (cluster of 2) share one operand box of every k-block by multicast: K-major operands, one problem, 128 x 128 tiles and an
+    // even tile count along N (pairs share A) or else along M (pairs share B).  Same tiles, instructions and order of the sums as one CTA.
+    // No derivative operand (act 2, the dgrads, whose W is MN-major anyway): without its prefetch registers the pair kernels spill less.
+    const int tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN;
+    const int cluster = (!amn && !bmn && nprob == 1 && act != 2 && BN == 128 && (tiles_n % 2 == 0 || tiles_m % 2 == 0)) ? 2 : 1;
+    gm.half = ma;
+    if (cluster == 2) {
+        if (int e = tiles_n % 2 == 0 ? make_map(&gm.half, As[0], M, K, lda, BM / 2) : make_map(&gm.half, Bs[0], N, K, ldb, BN / 2)) return e;
+    }
     if (splits > 1) {
         if (!accumulate)
             for (int p = 0; p < nprob; p++) { const size_t tot = (size_t)M * N; zero_strided<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cs[p], ldc, M, N); go1_count_launch(1); }
@@ -947,7 +1054,7 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     const bool timed = g_time_on && cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone;
     if (timed) {
         cudaEventRecord(timing_event(), st); g_time_flop += 2.0 * (double)M * (double)N * (double)K * nprob;
-        g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, BN, g.colsum ? 1 : 0});
+        g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, BN, g.colsum ? 1 : 0, cluster});
     }
     int e;
     // staged epilogue: C blocks leave the accumulator staging by TMA store, the derivative operand arrives through TMA loads.  The direct
@@ -963,9 +1070,10 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
         }
     }
     const bool any = g.act != 0 && g.kind != GO1_ACT_ELU;
-    if (BN == 128) e = any ? launch_gemm<128, true>(gm, mc, my, g, splits, st) : launch_gemm<128, false>(gm, mc, my, g, splits, st);
-    else if (BN == 64) e = any ? launch_gemm<64, true>(gm, mc, my, g, splits, st) : launch_gemm<64, false>(gm, mc, my, g, splits, st);
-    else e = any ? launch_gemm<32, true>(gm, mc, my, g, splits, st) : launch_gemm<32, false>(gm, mc, my, g, splits, st);
+    if (cluster == 2) e = any ? launch_gemm<128, true, 2>(gm, mc, my, g, splits, st) : launch_gemm<128, false, 2>(gm, mc, my, g, splits, st);
+    else if (BN == 128) e = any ? launch_gemm<128, true, 1>(gm, mc, my, g, splits, st) : launch_gemm<128, false, 1>(gm, mc, my, g, splits, st);
+    else if (BN == 64) e = any ? launch_gemm<64, true, 1>(gm, mc, my, g, splits, st) : launch_gemm<64, false, 1>(gm, mc, my, g, splits, st);
+    else e = any ? launch_gemm<32, true, 1>(gm, mc, my, g, splits, st) : launch_gemm<32, false, 1>(gm, mc, my, g, splits, st);
     if (e) return e;
     if (splits > 1 && (bias || act))
         for (int p = 0; p < nprob; p++) { const size_t tot = (size_t)M * N; bias_act_strided<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cs[p], ldc, bias, M, N, act, ep->act_kind); go1_count_launch(1); }
@@ -1053,7 +1161,7 @@ extern "C" int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int npr
         double fl = 0.0;
         for (int p = 0; p < nprob; p++) fl += 2.0 * (double)M * ((double)K1 * N2 + (double)N2 * N3 + (double)(N3 > 0 ? N3 : N2) * probs[p].nh);
         g_time_flop += fl;
-        g_time_recs.push_back({M * nprob, N2, K1, 0, 0, 1, 0, 1, shape_a ? 1003 : 1002, 0});
+        g_time_recs.push_back({M * nprob, N2, K1, 0, 0, 1, 0, 1, shape_a ? 1003 : 1002, 0, 1});
     }
     int e;
     if (g.kind == GO1_ACT_ELU) e = shape_a ? launch_tail<512, 256, 128, false>(maps, g, st) : launch_tail<256, 128, 0, false>(maps, g, st);
