@@ -274,6 +274,13 @@ int go1_sim_reset_idx_dev(Go1Sim* sim, const int32_t* env_ids, const int32_t* k_
 int go1_history_roll(const float* hist_in, const float* obs, float* hist_out, int n, int num_obs,
                      int history_len, void* stream);
 
+/* The same roll on rows with a pitch: hist_out[n][0:K0] = concat(hist_in[n][num_obs:K0], obs[n]), K0 = num_obs * history_len,
+ * with row strides ld_in / ld_out (floats, >= K0 and multiples of 4) and 16-byte aligned hist_in / hist_out; obs is contiguous
+ * [n][num_obs].  Columns K0..ld_out-1 of hist_out are not written.  HistoryWrapper keeps histories whose K0 is not a multiple of
+ * 4 floats at such a pitch (go1_b200.capi.history_pitch) so that the learner's tensor-core products read them in place. */
+int go1_history_roll_pitched(const float* hist_in, int ld_in, const float* obs, float* hist_out, int ld_out, int n,
+                             int num_obs, int history_len, void* stream);
+
 /* ------------------------------------------------------------------ ppo_cse learner ---------- */
 
 /* Replaces RolloutStorage.compute_returns (go1_gym_learn/ppo_cse/rollout_storage.py:74-88): GAE scan

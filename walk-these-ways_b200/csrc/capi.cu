@@ -14,6 +14,7 @@ extern "C" int go1_launch_reset_dev(const Go1SimBuffers*, const Go1DevTable*, co
 extern "C" int go1_launch_curriculum(const Go1SimBuffers*, const Go1CurriculumConfig*, const Go1CurriculumBuffers*, int, int, cudaStream_t);
 extern "C" int go1_launch_curriculum_pack(const Go1SimBuffers*, const Go1CurriculumConfig*, const Go1CurriculumBuffers*, int, cudaStream_t);
 extern "C" int go1_launch_history_roll(const float*, const float*, float*, int, int, int, cudaStream_t);
+extern "C" int go1_launch_history_roll_pitched(const float*, int, const float*, float*, int, int, int, int, cudaStream_t);
 
 static thread_local std::string g_err;
 static int fail(const std::string& m) { g_err = m; return 1; }
@@ -271,4 +272,21 @@ extern "C" int go1_history_roll(const float* hist_in, const float* obs, float* h
     if (!hist_in || !obs || !hist_out || n <= 0 || num_obs <= 0 || history_len <= 0) return fail("go1_history_roll: bad arguments");
     int e = go1_launch_history_roll(hist_in, obs, hist_out, n, num_obs, history_len, (cudaStream_t)stream);
     return e ? cuda_fail("go1_history_roll launch", e) : 0;
+}
+
+extern "C" int go1_history_roll_pitched(const float* hist_in, int ld_in, const float* obs, float* hist_out, int ld_out, int n, int num_obs,
+                                        int history_len, void* stream) {
+    if (!hist_in || !obs || !hist_out) return fail("go1_history_roll_pitched: null pointer");
+    if (n <= 0 || num_obs <= 0 || history_len <= 0 || (long long)num_obs * history_len > (1 << 30))
+        return fail("go1_history_roll_pitched: n, num_obs and history_len must be positive (num_obs * history_len <= 2^30)");
+    const int nhist = num_obs * history_len;
+    if (ld_in < nhist || ld_out < nhist || (ld_in & 3) || (ld_out & 3)) {
+        char b[160];
+        snprintf(b, sizeof b, "go1_history_roll_pitched: row pitches (ld_in %d, ld_out %d) must be >= num_obs * history_len (%d) and multiples of 4",
+                 ld_in, ld_out, nhist);
+        return fail(b);
+    }
+    if ((((uintptr_t)hist_in) | ((uintptr_t)hist_out)) & 15) return fail("go1_history_roll_pitched: hist_in and hist_out must be 16-byte aligned");
+    int e = go1_launch_history_roll_pitched(hist_in, ld_in, obs, hist_out, ld_out, n, num_obs, history_len, (cudaStream_t)stream);
+    return e ? cuda_fail("go1_history_roll_pitched launch", e) : 0;
 }

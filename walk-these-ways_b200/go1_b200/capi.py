@@ -29,6 +29,15 @@ NUM_EPISODE_SUMS = NUM_REWARD_TERMS + 1
 NUM_COMMAND_SUMS = NUM_REWARD_TERMS + 5
 COMMAND_SUM_EXTRAS = ["lin_vel_raw", "ang_vel_raw", "lin_vel_residual", "ang_vel_residual", "ep_timesteps"]
 
+def history_pitch(width):
+    """Row pitch (floats) of observation-history rows `width` = num_observations x num_observation_history wide, for every buffer that
+    holds them (HistoryWrapper's ping-pong buffers, RolloutStorage's history slab).  TMA, through which the learner's tensor-core
+    products read the histories, needs row strides that are multiples of 16 bytes: widths that are multiples of 4 floats keep their
+    natural pitch, the others are rounded up to a multiple of 32 floats (128-byte aligned rows, as RolloutStorage.hist_pitch)."""
+    width = int(width)
+    return width if width % 4 == 0 else (width + 31) // 32 * 32
+
+
 RESET_RAND_STRIDE = 48
 MAX_LAG_TIMESTEPS = 32
 _i, _f = C.c_int32, C.c_float
@@ -182,6 +191,7 @@ def lib():
         "go1_curriculum_pack": ([vp, C.POINTER(Go1CurriculumConfig), C.POINTER(Go1CurriculumBuffers), vp], ip),
         "go1_sim_reset_idx_dev": ([vp, vp, vp, vp, vp, ip, i64, vp, vp], ip),
         "go1_history_roll": ([vp, vp, vp, ip, ip, ip, vp], ip),
+        "go1_history_roll_pitched": ([vp, ip, vp, vp, ip, ip, ip, ip, vp], ip),
         "go1_ppo_gae": ([vp, vp, vp, vp, vp, vp, vp, ip, ip, _f, _f, vp], ip),
         "go1_ppo_normalize_advantages": ([vp, vp, i64, i64, vp], ip),
         "go1_gemm": ([ip, ip, ip, ip, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, vp], ip),

@@ -1,6 +1,10 @@
 """HistoryWrapper (reference go1_gym/envs/wrappers/history_wrapper.py:6-44): rolling window of the last
 `num_observation_history` observations, produced by the go1_history_roll kernel (ping-pong buffers instead of
-a fresh torch.cat allocation per step).  As in the reference the history is NOT cleared when an env resets."""
+a fresh torch.cat allocation per step).  As in the reference the history is NOT cleared when an env resets.
+
+Each buffer is [num_envs][capi.history_pitch(K0)] and obs_history is its [:, :K0] view (K0 = num_obs_history): contiguous when K0 is a
+multiple of 4 floats, otherwise rows padded to a 16-byte multiple so that the learner's tensor-core products read them in place.  The
+padding columns stay zero."""
 import torch
 
 from go1_b200 import capi
@@ -11,7 +15,9 @@ class HistoryWrapper:
         self.env = env
         self.obs_history_length = self.env.cfg.env.num_observation_history
         self.num_obs_history = self.obs_history_length * self.env.num_obs
-        z = lambda: torch.zeros(self.env.num_envs, self.num_obs_history, dtype=torch.float, device=self.env.device, requires_grad=False)
+        K0 = self.num_obs_history
+        self._pitch = capi.history_pitch(K0)
+        z = lambda: torch.zeros(self.env.num_envs, self._pitch, dtype=torch.float, device=self.env.device, requires_grad=False)[:, :K0]
         self._bufs = [z(), z()]
         self._cur = 0
         self.obs_history = self._bufs[0]
@@ -31,8 +37,12 @@ class HistoryWrapper:
 
     def _roll(self, obs):
         src, dst = self._bufs[self._cur], self._bufs[self._cur ^ 1]
-        capi.check(capi.lib().go1_history_roll(capi.ptr(src), capi.ptr(obs), capi.ptr(dst), self.env.num_envs, self.env.num_obs,
-                                               self.obs_history_length, capi.stream_ptr()), "go1_history_roll")
+        if self._pitch == self.num_obs_history:
+            capi.check(capi.lib().go1_history_roll(capi.ptr(src), capi.ptr(obs), capi.ptr(dst), self.env.num_envs, self.env.num_obs,
+                                                   self.obs_history_length, capi.stream_ptr()), "go1_history_roll")
+        else:
+            capi.check(capi.lib().go1_history_roll_pitched(capi.ptr(src), self._pitch, capi.ptr(obs), capi.ptr(dst), self._pitch, self.env.num_envs,
+                                                           self.env.num_obs, self.obs_history_length, capi.stream_ptr()), "go1_history_roll_pitched")
         self._cur ^= 1
         self.obs_history = dst
 

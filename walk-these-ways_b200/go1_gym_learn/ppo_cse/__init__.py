@@ -183,14 +183,15 @@ class Runner:
         ins = [None, None, hist, actions, core.rew, values, ac._logp, ac._mean, ac.std.data, dc.env_bins_f32]
         outs = [stg.observations, stg.privileged_observations, stg.observation_histories, stg.actions, stg.rewards, stg.values, stg.actions_log_prob,
                 stg.mu, stg.sigma, stg.env_bins]
-        for x in ins[2:]:
+        for x in ins[3:]:
             assert x.is_contiguous() and x.dtype == torch.float32
+        assert stg.history_rows_fit(hist) and hist.dtype == torch.float32      # the store copies whole rows at the slab's pitch
         from .ppo import PPO_Args
 
         def store_and_advance():
             capi.check(L.go1_rollout_store_transition((C.c_void_p * 10)(*[x.data_ptr() if x is not None else None for x in ins]), capi.ptr(core.reset_u8),
                                                       capi.ptr(dc.time_outs_u8) if send_to else None, (C.c_void_p * 10)(*[x.data_ptr() for x in outs]),
-                                                      capi.ptr(stg.dones), capi.ptr(sg["slot"]), N, core.num_obs, core.num_priv, hist.shape[1],
+                                                      capi.ptr(stg.dones), capi.ptr(sg["slot"]), N, core.num_obs, core.num_priv, stg.hist_row_pitch,
                                                       actions.shape[1], float(PPO_Args.gamma), sp()), "go1_rollout_store_transition")
             capi.check(L.go1_rollout_advance(capi.ptr(sg["acc"]), capi.ptr(sg["acc_hist"]), sg["W"], sg["T"], capi.ptr(sg["slot"]), capi.ptr(core.step_dev), sp()),
                        "go1_rollout_advance")

@@ -169,14 +169,12 @@ class _Net:
             Wm, ldw = W, i
             tc = impl == 1 and self._tma_ok(inp, ld_in)
             if tc and (not self._tma_ok(W, i) or (li == 0 and K >= 1024 and i % 32 != 0)):
-                # pack W[:, :K] into a TMA-readable copy whose row pitch is a multiple of 128 bytes (K % 4 == 0); for the long first-layer
-                # rows the aligned pitch alone is worth 30 % (misaligned 128-byte box rows cost an extra L2 sector each)
-                if K % 4 == 0:
-                    KPk = (K + 31) // 32 * 32
-                    Wm = self._cached(("pack", li), lambda old, W=W, o=o, i=i, K=K, KPk=KPk: (old if old is not None else _empty(o, KPk, device=W.device)[:, :K]).copy_(W.view(o, i)[:, :K]))
-                    ldw = KPk
-                else:
-                    tc = False
+                # pack W[:, :K] into a TMA-readable copy whose row pitch is a multiple of 128 bytes (any K: the kernel reads the K tail as
+                # zeros); for the long first-layer rows the aligned pitch alone is worth 30 % (misaligned 128-byte box rows cost an extra L2
+                # sector each)
+                KPk = (K + 31) // 32 * 32
+                Wm = self._cached(("pack", li), lambda old, W=W, o=o, i=i, K=K, KPk=KPk: (old if old is not None else _empty(o, KPk, device=W.device)[:, :K]).copy_(W.view(o, i)[:, :K]))
+                ldw = KPk
             if first_extra and i - K0 > 4:      # wide trailing input: y = x W[:, :K0]^T + b, then y = act(y + extra W[:, K0:]^T)
                 self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, o, b, 0, 0, 1 if tc else 0)
                 capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(y), o, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i, M, o, i - K0,
@@ -479,7 +477,7 @@ class ActorCritic(nn.Module):
         nets = self._nets
         na, npol, ncr = nets["adapt"], nets["actor"], nets["critic"]
         E = self.num_privileged_obs
-        fused = impl == 1 and _Net._tma_ok(h, h.stride(0)) and K0 % 4 == 0 and 1 <= E <= self.MAX_PRIVILEGED_OBS and \
+        fused = impl == 1 and _Net._tma_ok(h, h.stride(0)) and 1 <= E <= self.MAX_PRIVILEGED_OBS and \
             npol.specs[0][3] == K0 + E and ncr.specs[0][3] == K0 + E and na.specs[0][3] == K0
         if not fused:
             self.update_distribution(h, tag)

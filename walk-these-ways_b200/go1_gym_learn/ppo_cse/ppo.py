@@ -7,6 +7,7 @@ from go1_b200 import capi
 from go1_gym_learn.ppo_cse import ActorCritic
 from go1_gym_learn.ppo_cse import RolloutStorage
 from go1_gym_learn.ppo_cse import caches
+from go1_gym_learn.ppo_cse.actor_critic import _Net
 from params_proto import PrefixProto
 
 
@@ -109,8 +110,10 @@ class PPO:
             del st[stale]
         g = st.get(key)
         if g is None:
-            inplace = obs_history.is_contiguous() and privileged_obs.is_contiguous() and \
-                sum(1 for k2 in st if k2[2] is not None) < self._MAX_INPLACE_GRAPHS
+            # in place: contiguous histories, and rows at a TMA-readable pitch (HistoryWrapper's padded rows, capi.history_pitch)
+            h_rows = obs_history.is_contiguous() or (obs_history.dim() == 2 and obs_history.stride(1) == 1 and
+                                                     _Net._tma_ok(obs_history, obs_history.stride(0)))
+            inplace = h_rows and privileged_obs.is_contiguous() and sum(1 for k2 in st if k2[2] is not None) < self._MAX_INPLACE_GRAPHS
             if not inplace:
                 key = (obs_history.shape[0], ac._impl(), None, None, ac.flat_params.data_ptr())
                 g = st.get(key)
@@ -171,7 +174,9 @@ class PPO:
         tr.dones = dones
         tr.env_bins = infos["env_bins"]
         f32 = lambda x: x.is_cuda and x.is_contiguous() and x.dtype == torch.float32
-        fused = f32(rewards) and f32(tr.observation_histories) and f32(tr.env_bins) and f32(tr.values) and tr.env_bins.numel() == rewards.numel()
+        h = tr.observation_histories
+        fused = f32(rewards) and h.is_cuda and h.dtype == torch.float32 and self.storage.history_rows_fit(h) and f32(tr.env_bins) and f32(tr.values) and \
+            tr.env_bins.numel() == rewards.numel()
         if fused:   # rewards += gamma * values * time_outs (ppo.py:84-86) happens inside the store kernel
             tr.rewards = rewards
             tr.action_sigma_vec = self.actor_critic.std.data

@@ -33,11 +33,15 @@ class RolloutStorage:
         z = lambda *s, **k: torch.zeros(T, N, *s, device=self.device, **k)
         self.observations = z(*obs_shape)
         self.privileged_observations = z(*privileged_obs_shape)
-        self.observation_histories = z(*obs_history_shape)
+        # the history slab [T][N][hist_row_pitch] (the pitch of HistoryWrapper's rows, capi.history_pitch) and its [T][N][K0] view
+        K0 = int(obs_history_shape[-1])
+        self.hist_row_pitch = capi.history_pitch(K0)
+        self._hist_slab = z(self.hist_row_pitch)
+        self.observation_histories = self._hist_slab[..., :K0]
         # Row pitch of the GATHERED minibatch histories: a multiple of 32 floats, so that every 128-byte row of a TMA box of the first-layer
         # products starts on a 128-byte line.  Measured (tools/epi_bench.py): the 24576 x 1280 x 2100 product runs in 180 us with a
         # 2112-float pitch against 259 us with the natural 2100 (each misaligned box row costs a fifth L2 sector).
-        self.hist_pitch = (int(obs_history_shape[-1]) + 31) // 32 * 32
+        self.hist_pitch = (K0 + 31) // 32 * 32
         self.rewards = z(1)
         self.actions = z(*actions_shape)
         self.dones = z(1).byte()
@@ -86,6 +90,14 @@ class RolloutStorage:
             so.copy_(obs); sp.copy_(privileged_obs)
         return so, sp
 
+    def history_rows_fit(self, h):
+        """The fused transition store copies whole hist_row_pitch-wide rows: h [N][K0] qualifies if it is contiguous (pitch K0) or, for a
+        padded pitch, has exactly that row stride over storage that holds every full row (HistoryWrapper's buffers)."""
+        P = self.hist_row_pitch
+        if P == h.shape[-1]:
+            return h.is_contiguous()
+        return h.dim() == 2 and h.stride(1) == 1 and h.stride(0) == P and h.untyped_storage().nbytes() >= 4 * (h.storage_offset() + h.shape[0] * P)
+
     def add_transitions_fused(self, tr, time_outs, gamma):
         """add_transitions + the time-out bootstrap in ONE kernel (go1_store_transition)."""
         import ctypes as C
@@ -99,13 +111,14 @@ class RolloutStorage:
                tr.observation_histories, tr.actions, tr.rewards, tr.values, tr.actions_log_prob, tr.action_mean, tr.action_sigma_vec, tr.env_bins]
         outs = [self.observations[t], self.privileged_observations[t], self.observation_histories[t], self.actions[t], self.rewards[t], self.values[t],
                 self.actions_log_prob[t], self.mu[t], self.sigma[t], self.env_bins[t]]
-        for x in ins:
-            assert x is None or (x.is_contiguous() and x.dtype == torch.float32 and x.is_cuda), "transition tensors must be contiguous float32 CUDA tensors"
+        for k, x in enumerate(ins):
+            assert x is None or ((self.history_rows_fit(x) if k == 2 else x.is_contiguous()) and x.dtype == torch.float32 and x.is_cuda), \
+                "transition tensors must be contiguous float32 CUDA tensors (histories: rows at hist_row_pitch)"
         assert tr.env_bins.numel() == self.num_envs and dones.numel() == self.num_envs
         arr_in = (C.c_void_p * 10)(*[x.data_ptr() if x is not None else None for x in ins])
         arr_out = (C.c_void_p * 10)(*[x.data_ptr() for x in outs])
         capi.check(capi.lib().go1_store_transition(arr_in, capi.ptr(dones), capi.ptr(touts), arr_out, capi.ptr(self.dones[t]), self.num_envs,
-                                                   self.observations.shape[-1], self.privileged_observations.shape[-1], self.observation_histories.shape[-1],
+                                                   self.observations.shape[-1], self.privileged_observations.shape[-1], self.hist_row_pitch,
                                                    self.actions.shape[-1], float(gamma), capi.stream_ptr()), "go1_store_transition")
         self.step += 1
 
@@ -160,7 +173,8 @@ class RolloutStorage:
                 idx = indices[i * mini_batch_size:(i + 1) * mini_batch_size].contiguous()
                 obs = self.gather(self.observations, idx)
                 priv_b = self.gather(self.privileged_observations, idx)
-                hist_b = self.gather(self.observation_histories, idx, key=("hist", i), ldd=self.hist_pitch)
+                # whole slab rows: go1_gather_rows reads its source at a row pitch equal to the width it copies
+                hist_b = self.gather(self._hist_slab, idx, key=("hist", i), ldd=self.hist_pitch)[:, :self.observation_histories.shape[-1]]
                 # its K-major transpose [history | 1 | priv | latent rows] for the first layers' weight-gradient products, built once per
                 # update and read by every epoch (ActorCritic.backward_ppo / backward_adaptation); 830 MB for 4 minibatches at 4096 envs
                 M, w, P = hist_b.shape[0], hist_b.shape[1], priv_b.shape[1]
