@@ -351,8 +351,11 @@ int go1_gemm_grouped(int transA, int transB, int M, int N, int K, int nprob, con
 /* The layers BEHIND a first layer of one of ActorCritic's MLPs in one launch (impl 1, wgmma; actor_critic.py:38-77, 113-144):
  *   y2 = ELU(x W2^T + b2) [M][N2];   y3 = ELU(y2 W3^T + b3) [M][N3]  (N3 = 0: skipped);   out = y_last Wh^T + bh [M][nh], nh <= 16.
  * x is the first layer's activated output (K1 columns, row stride ldx); W* are torch nn.Linear weights [out][in], contiguous; y2 / y3 are
- * kept for the backward pass.  Supported tails: K1-N2-N3 = 512-256-128 (actor / critic bodies of scripts/train.py) and 256-128-0
- * (adaptation module); the activations between the layers never leave the SM (wgmma accumulators in registers -> shared memory -> tensor core). */
+ * kept for the backward pass.  Any K1 >= 1, N2 = 1..256, N3 = 0..128: 512-256-128 (actor / critic bodies of scripts/train.py) and 256-128-0
+ * (adaptation module) run on exact-width kernels, every other shape on kernels whose tiles cover N2 / N3 (64, 128 or 256 columns), with the
+ * rows and columns beyond the widths read as zeros (the y2 stores write whole 16-byte chunks: when N2 % 4 != 0, row padding columns
+ * N2 .. (N2 rounded up to 4) - 1 may be overwritten); the activations between the layers never leave the SM (wgmma accumulators in
+ * registers -> shared memory -> tensor core). */
 int go1_mlp_tail_forward(const float* x, int ldx, int M, int K1, const float* W2, const float* b2, int N2, float* y2, int ldy2,
                          const float* W3, const float* b3, int N3, float* y3, int ldy3, const float* Wh, const float* bh, int nh,
                          float* out, int ldout, void* stream);
@@ -362,6 +365,7 @@ typedef struct Go1TailProblem {
     const float* x; int32_t ldx; const float* W2; const float* b2; float* y2; int32_t ldy2;
     const float* W3; const float* b3; float* y3; int32_t ldy3; const float* Wh; const float* bh; int32_t nh; float* out; int32_t ldout;
     int32_t act_kind;    /* Go1Activation in place of ELU (0 = ELU); the problems of one launch share it */
+    int32_t ldw2, ldw3;  /* row strides of W2 / W3 in floats, multiples of 4 (0: contiguous, K1 / N2) */
 } Go1TailProblem;
 int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int nprob, int M, int K1, int N2, int N3, void* stream);
 

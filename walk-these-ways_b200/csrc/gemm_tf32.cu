@@ -758,11 +758,18 @@ __device__ __forceinline__ void head_partial(const float (&v)[4 * NJ], const flo
     }
 }
 
-template <int K1, int N2, int N3, bool ANYKIND>
-__global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_kernel(const __grid_constant__ TailMaps maps, const TailArgs g) {
+// The true widths of a ragged tail (mlp_tail_fwd_ragged_kernel): k1 any, n2 <= N2, n3 <= N3 (0 with N3), where N2 / N3 are the
+// instantiated tile widths.  TMA reads the W rows and columns beyond them as zeros and clips the y2 stores; the biases and head weights of
+// the padded columns are zero in shared memory, so those columns add nothing whatever f(0) is.
+struct TailDims { int k1, n2, n3; };
+
+template <int K1, int N2, int N3, bool ANYKIND, bool RAGGED>
+__device__ __forceinline__ void mlp_tail_fwd_body(const TailMaps& maps, const TailArgs& g, const TailDims d) {
     const int kind = ANYKIND ? g.kind : (int)GO1_ACT_ELU;
     using L = TailSmem<K1, N2, N3>;
-    constexpr int S1 = L::S1, S2 = (L::S2 > 0 ? L::S2 : 1), KB1 = L::KB1, KB2 = L::KB2, STAGE1 = L::STAGE1, STAGE2 = L::STAGE2, NL = L::NL;
+    constexpr int S1 = L::S1, S2 = (L::S2 > 0 ? L::S2 : 1), KB2 = L::KB2, STAGE1 = L::STAGE1, STAGE2 = L::STAGE2, NL = L::NL;
+    const int KB1 = RAGGED ? (d.k1 + BK - 1) / BK : L::KB1;
+    const int n2 = RAGGED ? d.n2 : N2, n3 = RAGGED ? d.n3 : N3, nl = RAGGED ? (N3 > 0 ? d.n3 : d.n2) : NL;
     constexpr int NH2 = N2 / 2, NH3 = (N3 > 0 ? N3 : 64) / 2;      // columns per warpgroup
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* base = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -792,12 +799,13 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_kernel(const
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     // biases and head weights: read by every consumer thread for every row -> shared memory
-    for (int i = threadIdx.x; i < TAIL_MAXP * N2; i += blockDim.x) { const int p = i / N2; s_b2[i] = (p < g.nprob && g.p[p].b2) ? __ldg(g.p[p].b2 + (i - p * N2)) : 0.f; }
-    if (N3 > 0) for (int i = threadIdx.x; i < TAIL_MAXP * N3; i += blockDim.x) { const int p = i / (N3 > 0 ? N3 : 1); s_b3[i] = (p < g.nprob && g.p[p].b3) ? __ldg(g.p[p].b3 + (i - p * N3)) : 0.f; }
+    for (int i = threadIdx.x; i < TAIL_MAXP * N2; i += blockDim.x) { const int p = i / N2; s_b2[i] = (p < g.nprob && g.p[p].b2 && i - p * N2 < n2) ? __ldg(g.p[p].b2 + (i - p * N2)) : 0.f; }
+    if (N3 > 0) for (int i = threadIdx.x; i < TAIL_MAXP * N3; i += blockDim.x) { const int p = i / (N3 > 0 ? N3 : 1); s_b3[i] = (p < g.nprob && g.p[p].b3 && i - p * N3 < n3) ? __ldg(g.p[p].b3 + (i - p * N3)) : 0.f; }
     for (int i = threadIdx.x; i < 16 * NL; i += blockDim.x) {
         const int n = i / NL, k = i - n * NL;
         float v = 0.f;
-        for (int p = 0; p < g.nprob; p++) { const int r = n - g.p[p].wh_row0; if (r >= 0 && r < g.p[p].nh) v = __ldg(g.p[p].Wh + (size_t)r * NL + k); }
+        if (k < nl)
+            for (int p = 0; p < g.nprob; p++) { const int r = n - g.p[p].wh_row0; if (r >= 0 && r < g.p[p].nh) v = __ldg(g.p[p].Wh + (size_t)r * nl + k); }
         s_wh[i] = v;
     }
     if (threadIdx.x < TAIL_MAXP * 16) { const int p = threadIdx.x >> 4, n = threadIdx.x & 15; s_bh[threadIdx.x] = (p < g.nprob && n < g.p[p].nh && g.p[p].bh) ? __ldg(g.p[p].bh + n) : 0.f; }
@@ -874,7 +882,8 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_kernel(const
         fence_async_smem();                                  // generic-proxy stores -> visible to the async proxy (tensor core, TMA store)
         cons_sync();
         if (lane == 0) {
-            for (int b = warp; b < 2 * KB2; b += NCONS) tma_store_2d(&maps.y2[p], y2t + (size_t)b * 4096, 32 * (b >> 1), m0 + 32 * (b & 1));      // rows beyond M are clipped
+            for (int b = warp; b < 2 * KB2; b += NCONS)      // rows beyond M (and columns beyond n2) are clipped
+                if (!RAGGED || 32 * (b >> 1) < n2) tma_store_2d(&maps.y2[p], y2t + (size_t)b * 4096, 32 * (b >> 1), m0 + 32 * (b & 1));
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         }
         if (N3 > 0) {
@@ -900,8 +909,13 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_kernel(const
                     const float2 bb = *reinterpret_cast<const float2*>(b3 + col);
                     acc[4 * j] = act_fast<KD>(acc[4 * j] + bb.x); acc[4 * j + 1] = act_fast<KD>(acc[4 * j + 1] + bb.y);
                     acc[4 * j + 2] = act_fast<KD>(acc[4 * j + 2] + bb.x); acc[4 * j + 3] = act_fast<KD>(acc[4 * j + 3] + bb.y);
-                    if (ok0) *reinterpret_cast<float2*>(pr.y3 + (size_t)(m0 + rA) * pr.ldy3 + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
-                    if (ok1) *reinterpret_cast<float2*>(pr.y3 + (size_t)(m0 + rA + 8) * pr.ldy3 + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+                    if (!RAGGED || col + 1 < n3) {
+                        if (ok0) *reinterpret_cast<float2*>(pr.y3 + (size_t)(m0 + rA) * pr.ldy3 + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+                        if (ok1) *reinterpret_cast<float2*>(pr.y3 + (size_t)(m0 + rA + 8) * pr.ldy3 + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+                    } else if (col < n3) {
+                        if (ok0) pr.y3[(size_t)(m0 + rA) * pr.ldy3 + col] = acc[4 * j];
+                        if (ok1) pr.y3[(size_t)(m0 + rA + 8) * pr.ldy3 + col] = acc[4 * j + 2];
+                    }
                 })
             head_partial<NH3 / 8>(acc, wh, NL, pr.nh, wgi * NH3, lane, hp);
         }
@@ -937,6 +951,18 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_kernel(const
     if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
+// the tails of scripts/train.py's shapes (512-256-128 and 256-128), every width a compile-time constant
+template <int K1, int N2, int N3, bool ANYKIND>
+__global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_kernel(const __grid_constant__ TailMaps maps, const TailArgs g) {
+    mlp_tail_fwd_body<K1, N2, N3, ANYKIND, false>(maps, g, TailDims{K1, N2, N3});
+}
+// any other tail: K1 streamed at run time, N2 / N3 the tile widths that cover n2 / n3 (N2 64, 128 or 256; N3 0 (two-layer tail), 64 or
+// 128: a 256-wide N3 would need 237 KB of shared memory with two W3 stages, and spills 1.2 KB with one)
+template <int N2, int N3, bool ANYKIND>
+__global__ void __launch_bounds__(32 * NCONS + 128, 1) mlp_tail_fwd_ragged_kernel(const __grid_constant__ TailMaps maps, const TailArgs g, const TailDims d) {
+    mlp_tail_fwd_body<BK, N2, N3, ANYKIND, true>(maps, g, d);
+}
+
 template <int K1, int N2, int N3, bool ANYKIND>
 int launch_tail(const TailMaps& maps, const TailArgs& g, cudaStream_t st) {
     using L = TailSmem<K1, N2, N3>;
@@ -955,6 +981,36 @@ int launch_tail(const TailMaps& maps, const TailArgs& g, cudaStream_t st) {
     return 0;
 }
 
+template <int N2, int N3, bool ANYKIND>
+int launch_tail_ragged(const TailMaps& maps, const TailArgs& g, const TailDims d, cudaStream_t st) {
+    using L = TailSmem<BK, N2, N3>;      // (K1 only sets the k-block count, which the ragged kernel takes at run time)
+    static_assert(L::TOTAL <= 227 * 1024, "fused tail: shared memory budget");
+    const size_t smem = L::TOTAL;
+    static bool configured = false;
+    if (!configured) {
+        cudaError_t e = cudaFuncSetAttribute(mlp_tail_fwd_ragged_kernel<N2, N3, ANYKIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
+        configured = true;
+    }
+    const int sms = sm_count();
+    const int grid = g.tiles < sms ? g.tiles : sms;
+    mlp_tail_fwd_ragged_kernel<N2, N3, ANYKIND><<<grid, 32 * NCONS + 128, smem, st>>>(maps, g, d);
+    go1_count_launch(1);
+    return 0;
+}
+
+// the ragged instantiation whose tiles cover (n2, n3)
+template <bool ANYKIND>
+int launch_tail_ragged_any(const TailMaps& maps, const TailArgs& g, const TailDims d, cudaStream_t st) {
+    const int w2 = d.n2 <= 64 ? 64 : d.n2 <= 128 ? 128 : 256, w3 = d.n3 == 0 ? 0 : d.n3 <= 64 ? 64 : d.n3 <= 128 ? 128 : -1;
+#define GO1_TAIL_CASE(A, B) if (w2 == A && w3 == B) return launch_tail_ragged<A, B, ANYKIND>(maps, g, d, st);
+    GO1_TAIL_CASE(64, 0) GO1_TAIL_CASE(64, 64) GO1_TAIL_CASE(64, 128)
+    GO1_TAIL_CASE(128, 0) GO1_TAIL_CASE(128, 64) GO1_TAIL_CASE(128, 128)
+    GO1_TAIL_CASE(256, 0) GO1_TAIL_CASE(256, 64) GO1_TAIL_CASE(256, 128)
+#undef GO1_TAIL_CASE
+    return go1_set_error("go1_mlp_tail_forward: tail widths N2 1..256, N3 0..128");
+}
+
 }  // namespace
 
 // ---- optional per-launch timing of the tensor-core GEMM (bench.py's roofline): CUDA events on the launch stream around every
@@ -964,7 +1020,9 @@ static bool g_time_on = false;
 static std::vector<cudaEvent_t> g_time_events;
 static size_t g_time_used = 0;
 static double g_time_flop = 0.0;
-struct TimeRec { int M, N, K, amn, bmn, act, nex, splits, kern, colsum, cluster; };      // what each timed launch was (GO1_GEMM_TIMING_CSV dump)
+// what each timed launch was (GO1_GEMM_TIMING_CSV dump).  Fused tails: N = N2, K = K1, n3 = N3 (0: two-layer tail), heads = the head
+// columns of all problems, problems = the problems in the grid (M counts the rows of all of them)
+struct TimeRec { int M, N, K, amn, bmn, act, nex, splits, kern, colsum, cluster, n3, heads, problems; };
 static std::vector<TimeRec> g_time_recs;
 static cudaEvent_t timing_event() {
     if (g_time_used == g_time_events.size()) { cudaEvent_t e; cudaEventCreate(&e); g_time_events.push_back(e); }
@@ -975,7 +1033,7 @@ extern "C" int go1_gemm_timing(int on, double* total_ms, double* total_flop, lon
     g_time_on = false;
     double ms = 0.0;
     FILE* csv = getenv("GO1_GEMM_TIMING_CSV") ? fopen(getenv("GO1_GEMM_TIMING_CSV"), "w") : nullptr;
-    if (csv) fprintf(csv, "M,N,K,a_mn_major,b_mn_major,act,num_extra,splits,kernel,colsum,us\n");
+    if (csv) fprintf(csv, "M,N,K,a_mn_major,b_mn_major,act,num_extra,splits,kernel,colsum,us,n3,heads,problems\n");
     for (size_t i = 0; i + 1 < g_time_used; i += 2) {
         if (cudaEventSynchronize(g_time_events[i + 1]) != cudaSuccess) return go1_set_error("go1_gemm_timing: event sync failed");
         float t = 0.f;
@@ -983,9 +1041,9 @@ extern "C" int go1_gemm_timing(int on, double* total_ms, double* total_flop, lon
         ms += t;
         if (csv && i / 2 < g_time_recs.size()) {
             const TimeRec& r = g_time_recs[i / 2];
-            fprintf(csv, "%d,%d,%d,%d,%d,%d,%d,%d,%s,%d,%.2f\n", r.M, r.N, r.K, r.amn, r.bmn, r.act, r.nex, r.splits,
+            fprintf(csv, "%d,%d,%d,%d,%d,%d,%d,%d,%s,%d,%.2f,%d,%d,%d\n", r.M, r.N, r.K, r.amn, r.bmn, r.act, r.nex, r.splits,
                     r.kern >= 1000 ? (r.kern == 1003 ? "tail3" : "tail2") : (r.kern == 128 ? (r.cluster == 2 ? "p128c2" : "p128") : (r.kern == 64 ? "p64" : "p32")),
-                    r.colsum, 1e3 * t);
+                    r.colsum, 1e3 * t, r.n3, r.heads, r.problems);
         }
     }
     if (csv) fclose(csv);
@@ -1054,7 +1112,7 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     const bool timed = g_time_on && cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone;
     if (timed) {
         cudaEventRecord(timing_event(), st); g_time_flop += 2.0 * (double)M * (double)N * (double)K * nprob;
-        g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, BN, g.colsum ? 1 : 0, cluster});
+        g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, BN, g.colsum ? 1 : 0, cluster, 0, 0, nprob});
     }
     int e;
     // staged epilogue: C blocks leave the accumulator staging by TMA store, the derivative operand arrives through TMA loads.  The direct
@@ -1127,8 +1185,11 @@ extern "C" int go1_transpose(const float* src, int lds, float* dst, int ldd, int
 extern "C" int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int nprob, int M, int K1, int N2, int N3, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     if (!probs || nprob < 1 || nprob > TAIL_MAXP || M <= 0) return go1_set_error("go1_mlp_tail_forward: 1 or 2 problems of the same shape");
-    const bool shape_a = (K1 == 512 && N2 == 256 && N3 == 128), shape_b = (K1 == 256 && N2 == 128 && N3 == 0);
-    if (!shape_a && !shape_b) return go1_set_error("go1_mlp_tail_forward: supported tails are 512-256-128-head and 256-128-head");
+    if (K1 < 1 || N2 < 1 || N2 > 256 || N3 < 0 || N3 > 128) return go1_set_error("go1_mlp_tail_forward: tail widths N2 1..256, N3 0..128 (K1 >= 1)");
+    // scripts/train.py's two tails on their exact-width kernels, every other shape on the ragged ones
+    bool shape_a = (K1 == 512 && N2 == 256 && N3 == 128), shape_b = (K1 == 256 && N2 == 128 && N3 == 0);
+    for (int p = 0; p < nprob; p++)
+        if ((probs[p].ldw2 != 0 && probs[p].ldw2 != K1) || (N3 > 0 && probs[p].ldw3 != 0 && probs[p].ldw3 != N2)) shape_a = shape_b = false;
     TailMaps maps;
     TailArgs g;
     g.nprob = nprob; g.M = M; g.tiles_per_prob = (M + TAIL_BM - 1) / TAIL_BM; g.tiles = g.tiles_per_prob * nprob;
@@ -1140,13 +1201,16 @@ extern "C" int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int npr
         if (q.act_kind != g.kind) return go1_set_error("go1_mlp_tail_forward: the problems of one launch share their activation kind");
         if (!q.x || !q.W2 || !q.y2 || !q.Wh || !q.out || q.nh < 1 || q.nh > TAIL_HPW || q.ldout < q.nh) return go1_set_error("go1_mlp_tail_forward: bad arguments (head width 1..12)");
         if (N3 > 0 && (!q.W3 || !q.y3)) return go1_set_error("go1_mlp_tail_forward: the three-layer tail needs W3 / y3");
-        if ((q.ldx & 3) || (q.ldy2 & 3) || (N3 > 0 && (q.ldy3 & 3)) ||
+        const int ldw2 = q.ldw2 ? q.ldw2 : K1, ldw3 = q.ldw3 ? q.ldw3 : N2;
+        if ((q.ldx & 3) || (q.ldy2 & 3) || (N3 > 0 && (q.ldy3 & 3)) || (ldw2 & 3) || ldw2 < K1 || (N3 > 0 && ((ldw3 & 3) || ldw3 < N2)) ||
             ((((uintptr_t)q.x | (uintptr_t)q.W2 | (uintptr_t)q.y2 | (uintptr_t)(N3 > 0 ? (const void*)q.W3 : (const void*)q.W2) |
                (uintptr_t)(N3 > 0 ? (const void*)q.y3 : (const void*)q.y2)) & 15) != 0))
             return go1_set_error("go1_mlp_tail_forward: operands must be 16-byte aligned with row strides that are multiples of 4 floats");
         if (int e = make_map(&maps.x[p], q.x, M, K1, q.ldx, TAIL_BM)) return e;
-        if (int e = make_map(&maps.w2[p], q.W2, N2, K1, K1, N2)) return e;
-        if (N3 > 0) { if (int e = make_map(&maps.w3[p], q.W3, N3, N2, N2, N3)) return e; } else maps.w3[p] = maps.w2[p];
+        // boxes of the tile widths: the rows beyond N2 / N3 of a ragged tail read as zeros
+        const int t2 = N2 <= 64 ? 64 : N2 <= 128 ? 128 : 256, t3 = N3 <= 64 ? 64 : 128;
+        if (int e = make_map(&maps.w2[p], q.W2, N2, K1, ldw2, t2)) return e;
+        if (N3 > 0) { if (int e = make_map(&maps.w3[p], q.W3, N3, N2, ldw3, t3)) return e; } else maps.w3[p] = maps.w2[p];
         if (int e = make_map(&maps.y2[p], q.y2, M, N2, q.ldy2, 32)) return e;
         TailProb& d = g.p[p];
         d.b2 = q.b2; d.b3 = q.b3; d.Wh = q.Wh; d.bh = q.bh; d.y3 = q.y3; d.out = q.out; d.ldy3 = q.ldy3; d.ldout = q.ldout; d.nh = q.nh; d.wh_row0 = rows;
@@ -1161,11 +1225,13 @@ extern "C" int go1_mlp_tail_forward_grouped(const Go1TailProblem* probs, int npr
         double fl = 0.0;
         for (int p = 0; p < nprob; p++) fl += 2.0 * (double)M * ((double)K1 * N2 + (double)N2 * N3 + (double)(N3 > 0 ? N3 : N2) * probs[p].nh);
         g_time_flop += fl;
-        g_time_recs.push_back({M * nprob, N2, K1, 0, 0, 1, 0, 1, shape_a ? 1003 : 1002, 0, 1});
+        g_time_recs.push_back({M * nprob, N2, K1, 0, 0, 1, 0, 1, N3 > 0 ? 1003 : 1002, 0, 1, N3, rows, nprob});
     }
     int e;
-    if (g.kind == GO1_ACT_ELU) e = shape_a ? launch_tail<512, 256, 128, false>(maps, g, st) : launch_tail<256, 128, 0, false>(maps, g, st);
-    else e = shape_a ? launch_tail<512, 256, 128, true>(maps, g, st) : launch_tail<256, 128, 0, true>(maps, g, st);
+    const bool any = g.kind != GO1_ACT_ELU;
+    if (shape_a) e = any ? launch_tail<512, 256, 128, true>(maps, g, st) : launch_tail<512, 256, 128, false>(maps, g, st);
+    else if (shape_b) e = any ? launch_tail<256, 128, 0, true>(maps, g, st) : launch_tail<256, 128, 0, false>(maps, g, st);
+    else e = any ? launch_tail_ragged_any<true>(maps, g, TailDims{K1, N2, N3}, st) : launch_tail_ragged_any<false>(maps, g, TailDims{K1, N2, N3}, st);
     if (e) return e;
     if (timed) cudaEventRecord(timing_event(), st);
     cudaError_t ce = cudaGetLastError();

@@ -29,13 +29,20 @@ NUM_EPISODE_SUMS = NUM_REWARD_TERMS + 1
 NUM_COMMAND_SUMS = NUM_REWARD_TERMS + 5
 COMMAND_SUM_EXTRAS = ["lin_vel_raw", "ang_vel_raw", "lin_vel_residual", "ang_vel_residual", "ep_timesteps"]
 
+def row_pitch(width):
+    """Row pitch (floats) of a buffer whose rows are `width` floats wide and that a tensor-core product reads or writes through TMA, which
+    needs row strides that are multiples of 16 bytes: widths that are multiples of 4 floats keep their natural pitch, the others are
+    rounded up to a multiple of 32 floats (128-byte aligned rows).  Holders expose the width as a [:, :width] view."""
+    width = int(width)
+    return width if width % 4 == 0 else (width + 31) // 32 * 32
+
+
 def history_pitch(width):
     """Row pitch (floats) of observation-history rows `width` = num_observations x num_observation_history wide, for every buffer that
     holds them (HistoryWrapper's ping-pong buffers, RolloutStorage's history slab).  TMA, through which the learner's tensor-core
     products read the histories, needs row strides that are multiples of 16 bytes: widths that are multiples of 4 floats keep their
     natural pitch, the others are rounded up to a multiple of 32 floats (128-byte aligned rows, as RolloutStorage.hist_pitch)."""
-    width = int(width)
-    return width if width % 4 == 0 else (width + 31) // 32 * 32
+    return row_pitch(width)
 
 
 RESET_RAND_STRIDE = 48
@@ -139,7 +146,7 @@ class Go1GemmEpilogue(C.Structure):
 class Go1TailProblem(C.Structure):
     _fields_ = [("x", C.c_void_p), ("ldx", _i), ("W2", C.c_void_p), ("b2", C.c_void_p), ("y2", C.c_void_p), ("ldy2", _i),
                 ("W3", C.c_void_p), ("b3", C.c_void_p), ("y3", C.c_void_p), ("ldy3", _i), ("Wh", C.c_void_p), ("bh", C.c_void_p), ("nh", _i),
-                ("out", C.c_void_p), ("ldout", _i), ("act_kind", _i)]
+                ("out", C.c_void_p), ("ldout", _i), ("act_kind", _i), ("ldw2", _i), ("ldw3", _i)]
 
 
 class Go1CopySeg(C.Structure):

@@ -12,6 +12,8 @@ the reference's names, .act / .evaluate / .act_student / .act_teacher / .get_act
     the product for 4 < E <= 64);
   * no autograd graph: the backward pass is written out (see `backward_ppo`, `backward_adaptation`).
 """
+import numbers
+
 import torch
 import torch.nn as nn
 from params_proto import PrefixProto
@@ -65,8 +67,13 @@ class _Net:
     impl 0: every product is one fp32 CUDA-core go1_gemm.  impl 1: the large products run on the wgmma TF32 kernel,
     which reads its operands through TMA (16-byte aligned rows) in either major: forward K-major, dgrad with W as an
     MN-major B operand, wgrad with dz and the layer input as MN-major A and B operands -- except the first layers' wgrad, which
-    ActorCritic runs K-major on transposed copies (history_kmajor, dz1T).  Only the first-layer weight block W[:, :K0] (row
-    stride 2102 floats) is packed to a TMA-readable copy, cached per weight version."""
+    ActorCritic runs K-major on transposed copies (history_kmajor, dz1T).  Hidden activations and their gradients live in buffers whose
+    row pitch is capi.row_pitch(width) (_hbuf); a weight whose rows are not a multiple of 4 floats long (the first-layer block W[:, :K0],
+    any hidden width that is not) is read through a packed TMA-readable copy, cached per weight version (_packed).
+
+    The layers behind the first one run as a fused tail (go1_mlp_tail_forward_grouped) from layer `tail_start` on: the last two hidden
+    layers and the head when their widths are at most 256 and 128, else the last hidden layer (up to 256 wide) and the head; earlier
+    layers run one by one."""
 
     def __init__(self, seq, flat, grad, offsets, owner):
         self.linears = [m for m in seq if isinstance(m, nn.Linear)]
@@ -81,13 +88,40 @@ class _Net:
         self._cache = {}
         self._ep = capi.Go1GemmEpilogue()
         self.kind = self._ep.act_kind = owner.act_kind      # Go1Activation of the hidden layers, passed to every kernel that applies f or f'
+        hidden = [sp[2] for sp in self.specs[:-1]]
+        if len(hidden) >= 3 and hidden[-2] <= 256 and hidden[-1] <= 128:
+            self.tail_start = len(hidden) - 2
+        elif len(hidden) >= 2 and hidden[-1] <= 256:
+            self.tail_start = len(hidden) - 1
+        else:
+            self.tail_start = None
 
-    def _buf(self, key, M, width):
+    def _buf(self, key, M, width, pitch=None):
+        """[M][width] view of a cached buffer with row pitch `pitch` (default: width)."""
+        pitch = width if pitch is None else pitch
         t = self.acts.get(key)
-        if t is None or t.shape[0] < M or t.shape[1] != width:
-            t = _empty(M, width, device=self.flat.device)
+        if t is None or t.shape[0] < M or t.shape[1] != pitch:
+            t = _empty(M, pitch, device=self.flat.device)
             self.acts[key] = t
-        return t[:M]
+        return t[:M, :width]
+
+    def _hbuf(self, key, M, width):
+        """A hidden activation or gradient buffer: TMA-readable rows whatever the width."""
+        return self._buf(key, M, width, capi.row_pitch(width))
+
+    def _packed(self, li, K):
+        """(copy, pitch): W[:, :K] of layer li in a TMA-readable copy whose row pitch is a multiple of 128 bytes (any K: the kernels read the
+        K tail as zeros), rebuilt once per weight version."""
+        wo, bo, o, i = self.specs[li]
+        W = self.flat[wo:wo + o * i]
+        KPk = (K + 31) // 32 * 32
+        return self._cached(("pack", li), lambda old: (old if old is not None else _empty(o, KPk, device=W.device)[:, :K]).copy_(W.view(o, i)[:, :K])), KPk
+
+    def _weight_tma(self, li):
+        """(W, row stride) of layer li for a TMA operand: in place when its rows allow it, else the packed copy."""
+        wo, bo, o, i = self.specs[li]
+        W = self.flat[wo:wo + o * i]
+        return (W, i) if self._tma_ok(W, i) else self._packed(li, i)
 
     def _cached(self, key, build):
         """A packed copy of weights, rebuilt when the weights changed (weights_version).  The entry keeps its builder so that
@@ -143,9 +177,10 @@ class _Net:
         p = x.data_ptr() if torch.is_tensor(x) else x
         return (p & 15) == 0 and (ld & 3) == 0
 
-    def forward(self, x, ldx, K0, extra, M, impl, tag="a", first_out=None):
+    def forward(self, x, ldx, K0, extra, M, impl, tag="a", first_out=None, defer_tail=False):
         """x: [M][K0] rows with stride ldx; extra: [M][E] contiguous or None. Returns list of layer outputs.
-        first_out: the first layer's activated output if the caller already produced it (ActorCritic.forward_all)."""
+        first_out: the first layer's activated output if the caller already produced it (ActorCritic.forward_all).
+        defer_tail: stop before the fused tail (the caller launches it, grouped with another net's) and return the outputs so far."""
         outs, inp, ld_in = [], x, ldx
         n = len(self.specs)
         for li, (wo, bo, o, i) in enumerate(self.specs):
@@ -153,80 +188,72 @@ class _Net:
                 outs.append(first_out)
                 inp, ld_in = first_out, first_out.stride(0)
                 continue
-            if li == 1 and impl == 1 and self._tail_ok(inp, ld_in, M):
-                return outs + self._forward_tail(inp, ld_in, M, tag)
-            y = self._buf((tag, li), M, o)
+            if li == self.tail_start and impl == 1 and self._tail_ok() and self._tma_ok(inp, ld_in):
+                return outs if defer_tail else outs + self._forward_tail(inp, ld_in, M, tag)
+            y = self._hbuf((tag, li), M, o) if li < n - 1 else self._buf((tag, li), M, o)
             W = self.flat[wo:wo + o * i]
             b = self.flat[bo:bo + o]
             act = 1 if li < n - 1 else 0
             first_extra = li == 0 and extra is not None
             if impl == 1 and li == n - 1 and li > 0 and o <= 16 and i % 4 == 0 and i <= 512 and self._tma_ok(inp, ld_in):
                 # the narrow head: one bandwidth-bound pass instead of a padded tensor-core tile
-                capi.check(capi.lib().go1_skinny_forward(self._p(inp), ld_in, W.data_ptr(), i, b.data_ptr(), capi.ptr(y), o, M, o, i, capi.stream_ptr()), "skinny_forward")
+                capi.check(capi.lib().go1_skinny_forward(self._p(inp), ld_in, W.data_ptr(), i, b.data_ptr(), capi.ptr(y), y.stride(0), M, o, i, capi.stream_ptr()), "skinny_forward")
                 outs.append(y)
                 continue
             K = K0 if first_extra else i
             Wm, ldw = W, i
             tc = impl == 1 and self._tma_ok(inp, ld_in)
             if tc and (not self._tma_ok(W, i) or (li == 0 and K >= 1024 and i % 32 != 0)):
-                # pack W[:, :K] into a TMA-readable copy whose row pitch is a multiple of 128 bytes (any K: the kernel reads the K tail as
-                # zeros); for the long first-layer rows the aligned pitch alone is worth 30 % (misaligned 128-byte box rows cost an extra L2
-                # sector each)
-                KPk = (K + 31) // 32 * 32
-                Wm = self._cached(("pack", li), lambda old, W=W, o=o, i=i, K=K, KPk=KPk: (old if old is not None else _empty(o, KPk, device=W.device)[:, :K]).copy_(W.view(o, i)[:, :K]))
-                ldw = KPk
+                # for the long first-layer rows the packed copy's aligned pitch alone is worth 30 % (misaligned 128-byte box rows cost an
+                # extra L2 sector each)
+                Wm, ldw = self._packed(li, K)
+            ldy = y.stride(0)
             if first_extra and i - K0 > 4:      # wide trailing input: y = x W[:, :K0]^T + b, then y = act(y + extra W[:, K0:]^T)
-                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, o, b, 0, 0, 1 if tc else 0)
-                capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(y), o, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i, M, o, i - K0,
+                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, ldy, b, 0, 0, 1 if tc else 0)
+                capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(y), ldy, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i, M, o, i - K0,
                                                             capi.act_arg(self.kind, act), capi.stream_ptr()), "go1_mlp_extra_forward")
             elif first_extra:   # y = act(x W[:, :K0]^T + extra W[:, K0:]^T + b): the (at most 4) trailing columns ride in the epilogue
-                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, o, b, act, 0, 1 if tc else 0, extra=extra, w_extra=W.data_ptr() + 4 * K0, ld_w_extra=i)
+                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, ldy, b, act, 0, 1 if tc else 0, extra=extra, w_extra=W.data_ptr() + 4 * K0, ld_w_extra=i)
             else:
-                self._gemm(0, 1, M, o, K, inp, ld_in, Wm, ldw, y, o, b, act, 0, 1 if tc else 0)
+                self._gemm(0, 1, M, o, K, inp, ld_in, Wm, ldw, y, ldy, b, act, 0, 1 if tc else 0)
             outs.append(y)
             inp, ld_in = y, y.stride(0)
         return outs
 
-    _TAILS = {(512, 256, 128): 3, (256, 128): 2}       # hidden widths behind the first layer that go1_mlp_tail_forward fuses
-
-    def _tail_ok(self, x1, ldx1, M):
-        """The layers behind the first one form a tail the fused kernel supports (and its TMA operands are aligned)."""
-        if not self.owner.fuse_tail:
-            return False
-        widths = tuple(sp[2] for sp in self.specs[:-1])
-        if self._TAILS.get(widths) != len(self.specs) - 1 or self.specs[-1][2] > 12:
-            return False
-        ok = self._tma_ok(x1, ldx1)
-        for wo, bo, o, i in self.specs[1:-1]:
-            ok = ok and ((self.flat.data_ptr() + 4 * wo) & 15) == 0 and i % 4 == 0
-        return ok
+    def _tail_ok(self):
+        """This net has a tail the fused kernel supports (hidden widths up to 256 behind the tail's input, a head of at most 12 columns)."""
+        return self.owner.fuse_tail and self.tail_start is not None and self.specs[-1][2] <= 12
 
     def _tail_problem(self, x1, ldx1, M, tag):
-        """(Go1TailProblem, [outputs of layers 1..]) of this net's tail for go1_mlp_tail_forward_grouped."""
-        sp, flat = self.specs, self.flat
+        """(Go1TailProblem, [outputs of layers tail_start..]) of this net's tail for go1_mlp_tail_forward_grouped; x1 is the output of
+        layer tail_start - 1."""
+        ts, flat = self.tail_start, self.flat
+        sp = self.specs[ts:]
         ptr = lambda off: flat.data_ptr() + 4 * off
         q = capi.Go1TailProblem()
         q.act_kind = self.kind
-        (w2, b2, n2, k1) = sp[1]
-        y2 = self._buf((tag, 1), M, n2)
-        q.x, q.ldx, q.W2, q.b2, q.y2, q.ldy2 = self._p(x1), ldx1, ptr(w2), ptr(b2), y2.data_ptr(), y2.stride(0)
-        if len(sp) == 4:
-            (w3, b3, n3, _), (wh, bh, nh, _) = sp[2], sp[3]
-            y3 = self._buf((tag, 2), M, n3)
-            out = self._buf((tag, 3), M, nh)
-            q.W3, q.b3, q.y3, q.ldy3 = ptr(w3), ptr(b3), y3.data_ptr(), y3.stride(0)
+        (w2, b2, n2, k1) = sp[0]
+        y2 = self._hbuf((tag, ts), M, n2)
+        W2, q.ldw2 = self._weight_tma(ts)
+        q.x, q.ldx, q.W2, q.b2, q.y2, q.ldy2 = self._p(x1), ldx1, self._p(W2), ptr(b2), y2.data_ptr(), y2.stride(0)
+        if len(sp) == 3:
+            (w3, b3, n3, _), (wh, bh, nh, _) = sp[1], sp[2]
+            y3 = self._hbuf((tag, ts + 1), M, n3)
+            out = self._buf((tag, ts + 2), M, nh)
+            W3, q.ldw3 = self._weight_tma(ts + 1)
+            q.W3, q.b3, q.y3, q.ldy3 = self._p(W3), ptr(b3), y3.data_ptr(), y3.stride(0)
             outs = [y2, y3, out]
         else:
-            (wh, bh, nh, _) = sp[2]
+            (wh, bh, nh, _) = sp[1]
             n3 = 0
-            out = self._buf((tag, 2), M, nh)
+            out = self._buf((tag, ts + 1), M, nh)
             q.W3, q.b3, q.y3, q.ldy3 = None, None, None, 0
             outs = [y2, out]
         q.Wh, q.bh, q.nh, q.out, q.ldout = ptr(wh), ptr(bh), nh, out.data_ptr(), out.stride(0)
         return q, outs, (k1, n2, n3)
 
     def _forward_tail(self, x1, ldx1, M, tag):
-        """Layers 1.. (and the head) in ONE launch; returns their outputs in layer order."""
+        """Layers tail_start.. (and the head) in ONE launch; returns their outputs in layer order."""
         q, outs, (k1, n2, n3) = self._tail_problem(x1, ldx1, M, tag)
         arr = (capi.Go1TailProblem * 1)(q)
         capi.check(capi.lib().go1_mlp_tail_forward_grouped(arr, 1, M, k1, n2, n3, capi.stream_ptr()), "go1_mlp_tail_forward")
@@ -255,7 +282,14 @@ class _Net:
             else:
                 inp, ld_in, K = outs[li - 1], outs[li - 1].stride(0), i
             wgrad_done = li == 0 and dz1T is not None       # made by the caller
-            skinny = not wgrad_done and o <= 16 and K >= 32  # the narrow heads: one bandwidth-bound pass instead of a padded GEMM tile
+            if impl == 1 and M >= 64 and not self._tma_ok(dz, ldz) and (o > 16 or (li == 1 and dz1T is not None)):
+                # a head gradient whose rows TMA cannot read ([M][1] values, [M][E] latents) where a tensor-core product must read it: the
+                # wgrad and dgrad of a head wider than the skinny kernels take, or a one-hidden-layer net's dgrad that stores the first-layer
+                # dz transposed
+                dzp = self._buf((tag, "dhead"), M, o, capi.row_pitch(o))
+                dzp.copy_(dz)
+                dz, ldz = dzp, dzp.stride(0)
+            skinny = not wgrad_done and o <= 16              # the narrow layers (heads): one bandwidth-bound pass instead of a padded GEMM tile
             # ---- 1. bias gradient: reduced by the dgrad that made dz, by the skinny wgrad, or by go1_colsum
             if not bias_done:
                 if skinny and K % 4 == 0 and self._tma_ok(inp, ld_in):
@@ -270,7 +304,7 @@ class _Net:
             elif skinny:
                 capi.check(L.go1_skinny_wgrad(capi.ptr(dz), ldz, capi.ptr(inp), ld_in, gW.data_ptr(), i, M, o, K, 1, st), "skinny_wgrad")
             else:       # impl 1: both operands MN-major, read in place by the wgmma kernel; split-K partial tiles add into the zeroed gradient
-                tc = impl == 1 and M >= 64 and K >= 8 and self._tma_ok(dz, ldz) and self._tma_ok(inp, ld_in)
+                tc = impl == 1 and M >= 64 and self._tma_ok(dz, ldz) and self._tma_ok(inp, ld_in)
                 if tc and wgrads is not None:
                     wgrads.append((o, K, M, ldz, ld_in, i, dz, inp, gW))
                 else:
@@ -290,10 +324,12 @@ class _Net:
             pwo, pbo, po, pi = self.specs[li - 1]
             gb_prev, yprev = self.grad[pbo:pbo + po], outs[li - 1]
             to_T = li == 1 and dz1T is not None
-            dprev = dz1T if to_T else self._buf((tag, "d", li - 1), M, i)
+            dprev = dz1T if to_T else self._hbuf((tag, "d", li - 1), M, i)
             ldp = dprev.stride(0)
-            if impl == 1 and self._tma_ok(dz, ldz) and self._tma_ok(W, i) and M >= 64:      # (the 12-wide actor head included: 19 us here, 22 us on the skinny pass)
-                # W read MN-major in place; the bias gradient of layer li-1 (column sums of dprev) rides in the epilogue
+            if impl == 1 and self._tma_ok(dz, ldz) and M >= 64:      # (the 12-wide actor head included: 19 us here, 22 us on the skinny pass)
+                # W read MN-major (in place, or its packed copy when its rows are not 16-byte multiples); the bias gradient of layer li-1
+                # (column sums of dprev) rides in the epilogue
+                Wd, ldwd = self._weight_tma(li)
                 bx = None
                 if li == 1 and extra is not None and 1 <= pi - K0 <= 4:
                     # dprev is the first layer's dz: d(extra), and the trailing-input weight gradient unless _first_layer_wgrad makes it,
@@ -304,7 +340,7 @@ class _Net:
                     gwx = None if to_T else self.grad.data_ptr() + 4 * (pwo + K0)
                     if dextra is not None or gwx is not None:
                         bx = (extra, self.flat.data_ptr() + 4 * (pwo + K0), pi, gwx, pi, dextra)
-                self._gemm(0, 0, M, i, o, dz, ldz, W, i, dprev, ldp, None, 2, 0, 1, dact_y=yprev, colsum=None if to_T else gb_prev, bwd_extra=bx,
+                self._gemm(0, 0, M, i, o, dz, ldz, Wd, ldwd, dprev, ldp, None, 2, 0, 1, dact_y=yprev, colsum=None if to_T else gb_prev, bwd_extra=bx,
                            store_transposed=1 if to_T else 0)
                 bias_done = True
             elif to_T:
@@ -337,6 +373,10 @@ class ActorCritic(nn.Module):
         if not 1 <= num_privileged_obs <= self.MAX_PRIVILEGED_OBS:
             raise ValueError(f"num_privileged_obs = {num_privileged_obs}: the learner kernels take 1..{self.MAX_PRIVILEGED_OBS} privileged observations")
         self.num_obs_history, self.num_privileged_obs, self.num_actions = num_obs_history, num_privileged_obs, num_actions
+        for field in ("adaptation_module_branch_hidden_dims", "actor_hidden_dims", "critic_hidden_dims"):
+            dims = getattr(AC_Args, field)
+            if len(dims) == 0 or not all(isinstance(d, numbers.Integral) and not isinstance(d, bool) and d > 0 for d in dims):
+                raise ValueError(f"AC_Args.{field} = {dims!r}: expected a non-empty list of positive layer widths")
         self.adaptation_module = _mlp(num_obs_history, AC_Args.adaptation_module_branch_hidden_dims, num_privileged_obs, activation)
         self.actor_body = _mlp(num_privileged_obs + num_obs_history, AC_Args.actor_hidden_dims, num_actions, activation)
         self.critic_body = _mlp(num_privileged_obs + num_obs_history, AC_Args.critic_hidden_dims, 1, activation)
@@ -483,6 +523,8 @@ class ActorCritic(nn.Module):
             self.update_distribution(h, tag)
             return self._mean, self.evaluate(h, priv, tag)
         oa, op, oc = na.specs[0][2], npol.specs[0][2], ncr.specs[0][2]
+        Pa, Pc = (oa + 3) // 4 * 4, (oc + 3) // 4 * 4     # the slices start on 16-byte boundaries (zero weight rows in between)
+        NC = Pa + Pc + (op + 3) // 4 * 4
         flat = self._flat
 
         def w1(net):
@@ -495,25 +537,29 @@ class ActorCritic(nn.Module):
 
         def build_all(old):     # the packed block [adapt | critic | actor] x K0 (128-byte row pitch), its bias row and the trailing-input
             if old is None:     # weights of the leading (adaptation | critic) columns (zeros | Wc[:, K0:]): ONE launch for all seven pieces
-                old = (_empty(oa + oc + op, KP, device=flat.device)[:, :K0], _empty(1, oa + oc + op, device=flat.device),
-                       _empty(oa + oc, E, device=flat.device).zero_())
+                old = (_empty(NC, KP, device=flat.device)[:, :K0], _empty(1, NC, device=flat.device), _empty(Pa + Pc, E, device=flat.device).zero_())
+                if NC != oa + oc + op:      # the padding rows between the slices stay zero
+                    old[0].zero_()
+                    old[1].zero_()
             W, b, x = old
-            capi.copy_segments([(W[:oa], Wa), (W[oa:oa + oc], Wc[:, :K0]), (W[oa + oc:], Wp[:, :K0]),
-                                (b[:, :oa], ba.view(1, -1)), (b[:, oa:oa + oc], bc.view(1, -1)), (b[:, oa + oc:], bp.view(1, -1)), (x[oa:], Wc[:, K0:])])
+            capi.copy_segments([(W[:oa], Wa), (W[Pa:Pa + oc], Wc[:, :K0]), (W[Pa + Pc:Pa + Pc + op], Wp[:, :K0]),
+                                (b[:, :oa], ba.view(1, -1)), (b[:, Pa:Pa + oc], bc.view(1, -1)), (b[:, Pa + Pc:Pa + Pc + op], bp.view(1, -1)),
+                                (x[Pa:Pa + oc], Wc[:, K0:])])
             return old
 
         Wcat, bcat, xcat = na._cached(("l1cat", "all"), build_all)
-        y = na._buf((tag, "y1cat"), M, oa + oc + op)
-        ya, yc, yp = y[:, :oa], y[:, oa:oa + oc], y[:, oa + oc:]
+        y = na._buf((tag, "y1cat"), M, NC)
+        ya, yc, yp = y[:, :oa], y[:, Pa:Pa + oc], y[:, Pa + Pc:Pa + Pc + op]
         if E <= 4:
-            na._gemm(0, 1, M, oa + oc + op, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1,
-                     extra=priv, w_extra=xcat.data_ptr(), ld_w_extra=E, lead_cols=oa + oc)
+            na._gemm(0, 1, M, NC, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1,
+                     extra=priv, w_extra=xcat.data_ptr(), ld_w_extra=E, lead_cols=Pa + Pc)
         else:       # wide privileged input: only the adaptation slice is finished in the epilogue; the critic slice gets priv here
-            na._gemm(0, 1, M, oa + oc + op, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1, lead_cols=oa)
+            na._gemm(0, 1, M, NC, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1, lead_cols=Pa)
             capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(yc), yc.stride(0), capi.ptr(priv), priv.stride(0), Wc.data_ptr() + 4 * K0, K0 + E,
                                                         M, oc, E, capi.act_arg(self.act_kind, 1), capi.stream_ptr()), "go1_mlp_extra_forward")
-        pair = self.fuse_tail and npol._tail_ok(yp, yp.stride(0), M) and ncr._tail_ok(yc, yc.stride(0), M) and \
-            [sp[2:] for sp in npol.specs[1:-1]] == [sp[2:] for sp in ncr.specs[1:-1]] and npol.specs[-1][2] + ncr.specs[-1][2] <= 16
+        ts = npol.tail_start
+        pair = npol._tail_ok() and ncr._tail_ok() and ts == ncr.tail_start and _Net._tma_ok(yp, yp.stride(0)) and _Net._tma_ok(yc, yc.stride(0)) and \
+            [sp[2:] for sp in npol.specs[ts:-1]] == [sp[2:] for sp in ncr.specs[ts:-1]] and npol.specs[-1][2] + ncr.specs[-1][2] <= 16
         side = None if pair else self._side_stream(M)
         if side is not None:        # the critic's tail does not depend on the adaptation module: it runs beside adapt -> actor
             self._fork(side)
@@ -523,12 +569,14 @@ class ActorCritic(nn.Module):
         latent = self._latent = self._a_out[-1]
         capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(yp), yp.stride(0), capi.ptr(latent), latent.stride(0), Wp.data_ptr() + 4 * K0, K0 + E,
                                                     M, op, E, capi.act_arg(self.act_kind, 1), capi.stream_ptr()), "go1_mlp_extra_forward")
-        if pair:                    # the equal-shape tails of the actor and critic bodies in ONE grid
-            qp, outs_p, shape = npol._tail_problem(yp, yp.stride(0), M, tag)
-            qc, outs_c, _ = ncr._tail_problem(yc, yc.stride(0), M, tag)
+        if pair:                    # the equal-shape tails of the actor and critic bodies in ONE grid (behind their layers before the tail)
+            lead_p = npol.forward(h, h.stride(0), K0, latent, M, impl, tag, first_out=yp, defer_tail=True)
+            lead_c = ncr.forward(h, h.stride(0), K0, priv, M, impl, tag, first_out=yc, defer_tail=True)
+            qp, outs_p, shape = npol._tail_problem(lead_p[-1], lead_p[-1].stride(0), M, tag)
+            qc, outs_c, _ = ncr._tail_problem(lead_c[-1], lead_c[-1].stride(0), M, tag)
             arr = (capi.Go1TailProblem * 2)(qp, qc)
             capi.check(capi.lib().go1_mlp_tail_forward_grouped(arr, 2, M, shape[0], shape[1], shape[2], capi.stream_ptr()), "go1_mlp_tail_forward")
-            self._p_out, self._c_out = [yp] + outs_p, [yc] + outs_c
+            self._p_out, self._c_out = lead_p + outs_p, lead_c + outs_c
             self._mean, self._value = self._p_out[-1], self._c_out[-1]
             return self._mean, self._value
         self._p_out = npol.forward(h, h.stride(0), K0, latent, M, impl, tag, first_out=yp)
