@@ -313,7 +313,7 @@ typedef enum Go1Activation { GO1_ACT_ELU = 0, GO1_ACT_SELU, GO1_ACT_RELU, GO1_AC
  * Row strides let a layer read/write column slices of wider buffers, so cat(obs_history, latent)
  * (actor_critic.py:115) is never materialised.  accumulate: add into C instead of overwriting
  * (bias/act are applied after the accumulation).  act: 0 none, 1 ELU(alpha=1), GO1_ACT(kind, 1) another activation.
- * impl: 0 = fp32 CUDA cores (exact-fp32 path), 1 = wgmma TF32 tensor cores with fp32 accumulation. */
+ * impl: 0 = fp32 CUDA cores (exact-fp32 path), 1 = wgmma TF32 tensor cores with fp32 accumulation (BF16 operands: go1_gemm_bf16_ex). */
 int go1_gemm(int transA, int transB, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
              float* C, int ldc, const float* bias, int act, int accumulate, int impl, void* stream);
 /* Same product with the full fused epilogue, applied in this order to each output element v = sum_k a*b:
@@ -341,9 +341,35 @@ typedef struct Go1GemmEpilogue {
                                  * C[m][n]); gives the next product a K-major operand: the first-layer dz of the weight-gradient product.
                                  * Needs M >= 32, accumulate 0, a 16-byte aligned C and ldc % 4 == 0.  The TMA store writes whole 16-byte
                                  * chunks: when M % 4 != 0, row padding columns M .. (M rounded up to 4) - 1 may be overwritten. */
+    uint16_t* out_bf16;  /* optional, with store_transposed: the transposed result goes here as BF16 (round to nearest even of the fp32 value
+                          * the fp32 store would write) instead of to C, which is then not written and may be NULL.  [N][M] with row stride
+                          * ld_out_bf16 elements (>= M, a multiple of 8), 16-byte aligned.  The column sums and trailing-input terms above still
+                          * see the fp32 values.  The A operand of a go1_gemm_bf16_ex weight gradient.  As above, whole 16-byte chunks are
+                          * written: when M % 8 != 0, row padding columns M .. (M rounded up to 8) - 1 may be overwritten. */
+    int32_t ld_out_bf16;
 } Go1GemmEpilogue;
 int go1_gemm_ex(int transA, int transB, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
                 float* C, int ldc, const Go1GemmEpilogue* ep, int impl, void* stream);
+/* The same product with BF16 operands (bit patterns of torch.bfloat16, leading dimensions in elements) on the wgmma BF16 tensor-core path,
+ * fp32 accumulation, fp32 output and the full fused epilogue above: the first-layer products of AC_Args.gemm_impl = 2, which reduce over the
+ * observation history.  Both operands K-major: transA = 0 (A [M][K]) and transB = 1 (B [N][K]); 16-byte aligned, lda / ldb multiples of 8.
+ * Any other layout returns non-zero before any launch. */
+int go1_gemm_bf16_ex(int transA, int transB, int M, int N, int K, const uint16_t* A, int lda, const uint16_t* B, int ldb,
+                     float* C, int ldc, const Go1GemmEpilogue* ep, void* stream);
+/* Conversions to BF16 for those products, each rounding once to nearest even (torch's .to(torch.bfloat16)); columns of dst beyond the
+ * copied width (row pitch padding) are not written.
+ *   go1_convert_bf16:       dst[r][c] = bf16(src[r][c])                  rows x cols, row strides lds / ldd (elements)
+ *   go1_gather_rows_bf16:   dst[i][c] = src[idx[i]][c], c < width        BF16 source (the rollout's BF16 history slab: no rounding)
+ *   go1_rollout_store_rows_bf16: slab[slot][r][c] = src[r][c]           BF16 rows into slot *slot_dev (slot 0 if NULL) of a [T][rows][ldd]
+ *                           slab: the history the policy evaluated, stored by the captured env step (go1_rollout_store_transition then
+ *                           takes in_f32[2] = NULL)
+ *   go1_transpose_to_bf16:  dst[c][r] = bf16(src[r][c])                  fp32 source
+ *   go1_transpose_bf16:     dst[c][r] = src[r][c]                        BF16 source (no rounding) */
+int go1_convert_bf16(const float* src, int lds, uint16_t* dst, int ldd, int rows, int cols, void* stream);
+int go1_gather_rows_bf16(const uint16_t* src, int lds, const int64_t* idx, uint16_t* dst, int ldd, int64_t rows, int width, void* stream);
+int go1_rollout_store_rows_bf16(const uint16_t* src, int lds, uint16_t* dst_base, int ldd, const int32_t* slot_dev, int rows, int cols, void* stream);
+int go1_transpose_to_bf16(const float* src, int lds, uint16_t* dst, int ldd, int rows, int cols, void* stream);
+int go1_transpose_bf16(const uint16_t* src, int lds, uint16_t* dst, int ldd, int rows, int cols, void* stream);
 /* nprob (<= 4) wgmma products of the SAME shape and operand strides in one grid: C[p] (+)= op(A[p]) op(B[p]) (impl 1 only, no fused
  * epilogue operands).  Used for the equal-shape split-K wgrads of the three MLPs (nn.Linear weight gradients, actor_critic.py:38-77). */
 int go1_gemm_grouped(int transA, int transB, int M, int N, int K, int nprob, const float* const* A, int lda, const float* const* B, int ldb,
@@ -461,7 +487,8 @@ int go1_ppo_adaptive_lr(const float* scalars, float* lr_dev, float desired_kl, f
  * PPO.process_env_step (ppo.py:84-86: rewards += gamma * values * time_outs) in one launch.
  * in_f32[10]  = {obs[n][nobs] or NULL, priv[n][npriv] or NULL, obs_history[n][nhist], actions[n][nact], rewards[n], values[n], log_prob[n],
  *                action_mean[n][nact], std[nact], env_bins[n] or NULL};  dones/time_outs: uint8 [n] (time_outs may be NULL)
- * out_f32[10] = the slot `step` of the storage slabs in the same order (sigma[n][nact] for std);  s_dones: uint8 [n]. */
+ * out_f32[10] = the slot `step` of the storage slabs in the same order (sigma[n][nact] for std);  s_dones: uint8 [n].
+ * obs_history may be NULL: the history is then not stored (a BF16 slab, filled by go1_rollout_store_rows_bf16). */
 int go1_store_transition(const float* const* in_f32, const uint8_t* dones, const uint8_t* time_outs, float* const* out_f32, uint8_t* s_dones,
                          int n, int nobs, int npriv, int nhist, int nact, float gamma, void* stream);
 

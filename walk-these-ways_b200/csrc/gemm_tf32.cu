@@ -25,6 +25,7 @@
 // mlp_tail_fwd_kernel chains two such products and a CUDA-core head for the layers behind a first layer.
 #include <cuda_runtime.h>
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <mutex>
@@ -140,6 +141,7 @@ struct GemmArgs {
     int lead;                // > 0: extra columns + activation only for output columns < lead
     int amn, bmn;            // operand is MN-major in HBM (A given as [K][M], B given as [K][N]); persistent kernel only
     int ct;                  // C is stored transposed, element (m, n) at C[n * ldc + m]: staged epilogue only (tma_store)
+    int c16;                 // with ct: the transposed blocks leave as BF16 (round to nearest even) through a BF16 map of the output
     float* colsum;           // optional [N]: += column sums of the values written (bias gradient fused into the dgrad epilogue)
     const float* bx; const float* bwx; float* gwx; float* dx;     // fused trailing-input backward (see Go1GemmEpilogue)
     int ldbx, ldbwx, ldgwx, lddx, nbx;
@@ -319,7 +321,11 @@ __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const C
         }
     }
     if (es.out) {           // warp-uniform: all 32 lanes stage their row (rows / columns beyond M / N are clipped by the TMA store)
-        if (g.ct) {         // the block of C^T: this lane's row becomes column `lane`; store j writes row j of the block, 32 lanes x 4 bytes of
+        if (g.ct && g.c16) {    // BF16 block of C^T, unswizzled 64-byte rows: store j writes row j, 32 lanes x 2 consecutive bytes (conflict-free)
+            __syncwarp();
+#pragma unroll
+            for (int j = 0; j < 32; j++) *reinterpret_cast<__nv_bfloat16*>(es.out + j * 64 + lane * 2) = __float2bfloat16_rn(v[j]);
+        } else if (g.ct) {  // the block of C^T: this lane's row becomes column `lane`; store j writes row j of the block, 32 lanes x 4 bytes of
             __syncwarp();   // one 128-byte row (swizzled chunk (lane / 4) ^ (j % 8): conflict-free).  Every lane has read its row of the block.
 #pragma unroll
             for (int j = 0; j < 32; j++)
@@ -372,8 +378,10 @@ __device__ __forceinline__ bool epilogue_prefetch(const GemmArgs& g, const int r
 // stage in its own CTA and in its peer.  Cluster barriers after the mbarrier initialisation and before any thread exits keep a CTA
 // alive while its peer may still multicast into it or arrive on its barriers.
 // ---------------------------------------------------------------------------------------------------------------
+// BF16 = true: the operands are BF16 (K-major only), a k-block is 64 of them (the same 128-byte rows, boxes, ring and multicast as 32
+// floats) and the tensor core runs m64nBNk16 BF16 instructions; the epilogue is the same fp32 code.
 constexpr int X_BYTES = 65536;
-template <int BN, bool ANYKIND, int CL>
+template <int BN, bool ANYKIND, int CL, bool BF16>
 __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __grid_constant__ GemmMaps gm,
                                                                       const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
                                                                       const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
@@ -381,6 +389,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
     constexpr int G = EPI_G;
     constexpr int A_BYTES = BM * BK * 4, STAGE_BYTES = (BM + BN) * BK * 4;
     constexpr int MAX_STAGES = 8;
+    constexpr int KE = BF16 ? 2 * BK : BK;       // operand elements per k-block
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t* base = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
     uint8_t* ring = base;
@@ -391,7 +400,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
     uint64_t* aux_bar = empty + MAX_STAGES;      // [NCONS]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int num_kb_total = (g.K + BK - 1) / BK;
+    const int num_kb_total = (g.K + KE - 1) / KE;
 
     if (threadIdx.x == 0) {
         for (int p = 0; p < g.nprob; p++) {
@@ -445,7 +454,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
                     uint8_t* a = ring + (size_t)s * STAGE_BYTES;
                     uint8_t* b = a + A_BYTES;
                     if (CL > 1) {           // K-major: this CTA's half of the shared box to both CTAs, its own box of the other operand
-                        const int kc = (kb0 + i) * BK;
+                        const int kc = (kb0 + i) * KE;
                         if (pair_n()) {
                             tma_load_2d_multicast(&gm.half, &full[s], a + rank() * (A_BYTES / 2), kc, m0 + (int)rank() * (BM / 2), 0x3);
                             tma_load_2d(mapB, &full[s], b, kc, n0);
@@ -454,10 +463,10 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
                             tma_load_2d_multicast(&gm.half, &full[s], b + rank() * (A_BYTES / 2), kc, n0 + (int)rank() * (BN / 2), 0x3);
                         }
                     } else {
-                        if (g.amn) tma_load_2d(mapA, &full[s], a, m0, (kb0 + i) * BK);        // box [32 k-rows][128 m]
-                        else tma_load_2d(mapA, &full[s], a, (kb0 + i) * BK, m0);              // box [128 m-rows][32 k]
-                        if (g.bmn) tma_load_2d(mapB, &full[s], b, n0, (kb0 + i) * BK);
-                        else tma_load_2d(mapB, &full[s], b, (kb0 + i) * BK, n0);
+                        if (g.amn) tma_load_2d(mapA, &full[s], a, m0, (kb0 + i) * KE);        // box [32 k-rows][128 m]
+                        else tma_load_2d(mapA, &full[s], a, (kb0 + i) * KE, m0);              // box [128 m-rows][32 k]
+                        if (g.bmn) tma_load_2d(mapB, &full[s], b, n0, (kb0 + i) * KE);
+                        else tma_load_2d(mapB, &full[s], b, (kb0 + i) * KE, n0);
                     }
                     if (++s == stages) { s = 0; ph ^= 1; }
                 }
@@ -474,7 +483,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
     // ===== consumers: warpgroup wgi owns rows [64 wgi, 64 wgi + 64) of the tile =====
     const int wgi = warp >> 2, w = warp & 3, ctid = threadIdx.x;
     const int q = 2 * wgi + (w & 1), grp = w >> 1;      // epilogue: 32-row block q of the tile, column group grp
-    const bool tr = CL == 1 && (g.amn || g.bmn);        // pairs read K-major operands only, one problem
+    const bool tr = !BF16 && CL == 1 && (g.amn || g.bmn);        // pairs read K-major operands only, one problem; BF16: K-major only
     const bool split = g.kb_per_split < num_kb_total;
     const bool st_out = g.tma_store, st_aux = CL == 1 && g.tma_aux;      // pairs: no derivative operand (act 2)
     uint8_t* xwg = xreg + wgi * (X_BYTES / 2);          // this warpgroup's accumulator staging: [chunk][64 rows][128 B]
@@ -530,7 +539,7 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
                 cons_sync();
             }
             wg::fence();
-            wg::mma_kblock<BN>(acc, a + (size_t)wgi * 64 * 128, b, i > 0);
+            wg::mma_kblock<BN, BF16>(acc, a + (size_t)wgi * 64 * 128, b, i > 0);
             wg::commit();
             if (!tr && prev >= 0) {
                 wg::wait<1>();
@@ -582,23 +591,25 @@ int sm_count() {
     return sms;
 }
 
-int make_map_uncached(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int box_rows, int box_cols, CUtensorMapSwizzle swz);
+int make_map_uncached(CUtensorMap* map, const void* ptr, int rows, int cols, int ld, int box_rows, int box_cols, CUtensorMapSwizzle swz, int esize);
 // Encoding a tensor map costs about a microsecond of host time and the learner issues the same few hundred (pointer, shape) combinations
 // every update: keep them.
-struct MapKey { const float* ptr; int rows, cols, ld, box_rows, box_cols, swz; bool operator==(const MapKey& o) const { return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && box_cols == o.box_cols && swz == o.swz; } };
-struct MapKeyHash { size_t operator()(const MapKey& k) const { size_t h = (size_t)k.ptr; h = h * 1000003u ^ (size_t)k.rows; h = h * 1000003u ^ (size_t)k.cols; h = h * 1000003u ^ (size_t)k.ld; h = h * 1000003u ^ (size_t)(k.box_rows * 8 + k.swz); h = h * 1000003u ^ (size_t)k.box_cols; return h; } };
+struct MapKey { const void* ptr; int rows, cols, ld, box_rows, box_cols, swz, esize; bool operator==(const MapKey& o) const { return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box_rows == o.box_rows && box_cols == o.box_cols && swz == o.swz && esize == o.esize; } };
+struct MapKeyHash { size_t operator()(const MapKey& k) const { size_t h = (size_t)k.ptr; h = h * 1000003u ^ (size_t)k.rows; h = h * 1000003u ^ (size_t)k.cols; h = h * 1000003u ^ (size_t)k.ld; h = h * 1000003u ^ (size_t)((k.box_rows * 8 + k.swz) * 8 + k.esize); h = h * 1000003u ^ (size_t)k.box_cols; return h; } };
 std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_map_cache;
 std::mutex g_map_mutex;
 // rows x cols fp32 matrix with row stride ld; box = box_rows x box_cols.  K-major operand tiles and 32 x 32 output blocks: 32-float (128-byte)
-// box rows, 128B-swizzled.  MN-major operand boxes ([32 k-rows][tile width]): unswizzled, transposed on the SM.
-int make_map(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int box_rows, int box_cols = BK, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
-    const MapKey key{ptr, rows, cols, ld, box_rows, box_cols, (int)swz};
+// box rows, 128B-swizzled.  MN-major operand boxes ([32 k-rows][tile width]): unswizzled, transposed on the SM.  esize 2: a BF16 matrix
+// (ld and box_cols in elements; K-major operand boxes are 64 wide, the same 128-byte rows).
+int make_map(CUtensorMap* map, const void* ptr, int rows, int cols, int ld, int box_rows, int box_cols = BK, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B,
+             int esize = 4) {
+    const MapKey key{ptr, rows, cols, ld, box_rows, box_cols, (int)swz, esize};
     {
         std::lock_guard<std::mutex> lk(g_map_mutex);
         auto it = g_map_cache.find(key);
         if (it != g_map_cache.end()) { *map = it->second; return 0; }
     }
-    if (int e = make_map_uncached(map, ptr, rows, cols, ld, box_rows, box_cols, swz)) return e;
+    if (int e = make_map_uncached(map, ptr, rows, cols, ld, box_rows, box_cols, swz, esize)) return e;
     std::lock_guard<std::mutex> lk(g_map_mutex);
     if (g_map_cache.size() > 8192) g_map_cache.clear();
     g_map_cache.emplace(key, *map);
@@ -607,7 +618,7 @@ int make_map(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int
 int make_map_mn(CUtensorMap* map, const float* ptr, int k_rows, int mn_cols, int ld, int width) {
     return make_map(map, ptr, k_rows, mn_cols, ld, BK, width, CU_TENSOR_MAP_SWIZZLE_NONE);
 }
-int make_map_uncached(CUtensorMap* map, const float* ptr, int rows, int cols, int ld, int box_rows, int box_cols, CUtensorMapSwizzle swz) {
+int make_map_uncached(CUtensorMap* map, const void* ptr, int rows, int cols, int ld, int box_rows, int box_cols, CUtensorMapSwizzle swz, int esize) {
     std::call_once(g_once, [] {
         void* fn = nullptr;
         cudaDriverEntryPointQueryResult q;
@@ -615,10 +626,10 @@ int make_map_uncached(CUtensorMap* map, const float* ptr, int rows, int cols, in
     });
     if (!g_encode) return go1_set_error("cuTensorMapEncodeTiled unavailable");
     cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
+    cuuint64_t strides[1] = {(cuuint64_t)ld * esize};
     cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
-    CUresult r = g_encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    CUresult r = g_encode(map, esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                           swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { char b[96]; snprintf(b, sizeof b, "cuTensorMapEncodeTiled failed (%d)", (int)r); return go1_set_error(b); }
     return 0;
@@ -656,7 +667,7 @@ __global__ void bias_act_strided(float* C, int ldc, const float* bias, int M, in
     *c = v;
 }
 
-template <int BN, bool ANYKIND, int CL>
+template <int BN, bool ANYKIND, int CL, bool BF16>
 int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st) {
     constexpr int STAGE_BYTES = (BM + BN) * BK * 4;
     const size_t staging = X_BYTES + (g.tma_aux ? (size_t)NCONS * 4096 : 0);
@@ -666,7 +677,7 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
     if (stages > 8) stages = 8;
     if (stages < 2) return go1_set_error("go1_gemm impl=1: no room for the operand ring");
     const size_t smem = (size_t)stages * STAGE_BYTES + fixed;
-    auto kernel = gemm_tf32_wgmma<BN, ANYKIND, CL>;
+    auto kernel = gemm_tf32_wgmma<BN, ANYKIND, CL, BF16>;
     const int tiles_m = (g.M + BM - 1) / BM, tiles_n = (g.N + BN - 1) / BN;
     g.tiles_per_prob = tiles_m * tiles_n * splits;
     const int total = g.tiles_per_prob * (g.nprob > 1 ? g.nprob : 1);
@@ -1022,7 +1033,7 @@ static size_t g_time_used = 0;
 static double g_time_flop = 0.0;
 // what each timed launch was (GO1_GEMM_TIMING_CSV dump).  Fused tails: N = N2, K = K1, n3 = N3 (0: two-layer tail), heads = the head
 // columns of all problems, problems = the problems in the grid (M counts the rows of all of them)
-struct TimeRec { int M, N, K, amn, bmn, act, nex, splits, kern, colsum, cluster, n3, heads, problems; };
+struct TimeRec { int M, N, K, amn, bmn, act, nex, splits, kern, colsum, cluster, n3, heads, problems, bf16; };
 static std::vector<TimeRec> g_time_recs;
 static cudaEvent_t timing_event() {
     if (g_time_used == g_time_events.size()) { cudaEvent_t e; cudaEventCreate(&e); g_time_events.push_back(e); }
@@ -1033,7 +1044,7 @@ extern "C" int go1_gemm_timing(int on, double* total_ms, double* total_flop, lon
     g_time_on = false;
     double ms = 0.0;
     FILE* csv = getenv("GO1_GEMM_TIMING_CSV") ? fopen(getenv("GO1_GEMM_TIMING_CSV"), "w") : nullptr;
-    if (csv) fprintf(csv, "M,N,K,a_mn_major,b_mn_major,act,num_extra,splits,kernel,colsum,us,n3,heads,problems\n");
+    if (csv) fprintf(csv, "M,N,K,a_mn_major,b_mn_major,act,num_extra,splits,kernel,colsum,us,n3,heads,problems,bf16\n");
     for (size_t i = 0; i + 1 < g_time_used; i += 2) {
         if (cudaEventSynchronize(g_time_events[i + 1]) != cudaSuccess) return go1_set_error("go1_gemm_timing: event sync failed");
         float t = 0.f;
@@ -1041,9 +1052,9 @@ extern "C" int go1_gemm_timing(int on, double* total_ms, double* total_flop, lon
         ms += t;
         if (csv && i / 2 < g_time_recs.size()) {
             const TimeRec& r = g_time_recs[i / 2];
-            fprintf(csv, "%d,%d,%d,%d,%d,%d,%d,%d,%s,%d,%.2f,%d,%d,%d\n", r.M, r.N, r.K, r.amn, r.bmn, r.act, r.nex, r.splits,
+            fprintf(csv, "%d,%d,%d,%d,%d,%d,%d,%d,%s,%d,%.2f,%d,%d,%d,%d\n", r.M, r.N, r.K, r.amn, r.bmn, r.act, r.nex, r.splits,
                     r.kern >= 1000 ? (r.kern == 1003 ? "tail3" : "tail2") : (r.kern == 128 ? (r.cluster == 2 ? "p128c2" : "p128") : (r.kern == 64 ? "p64" : "p32")),
-                    r.colsum, 1e3 * t, r.n3, r.heads, r.problems);
+                    r.colsum, 1e3 * t, r.n3, r.heads, r.problems, r.bf16);
         }
     }
     if (csv) fclose(csv);
@@ -1053,31 +1064,41 @@ extern "C" int go1_gemm_timing(int on, double* total_ms, double* total_flop, lon
     return 0;
 }
 
-static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob, const float* const* As, int lda, const float* const* Bs, int ldb,
-                          float* const* Cs, int ldc, const Go1GemmEpilogue* ep, cudaStream_t st) {
+// T = float: TF32 products (operands in either major); T = uint16_t: BF16 products (K-major operands only, go1_gemm_bf16_ex).  One code path
+// for both: only the operand maps, the k-block width and the tensor-core instruction differ.
+template <typename T>
+static int gemm_wgmma_impl(int transA, int transB, int M, int N, int K, int nprob, const T* const* As, int lda, const T* const* Bs, int ldb,
+                           float* const* Cs, int ldc, const Go1GemmEpilogue* ep, cudaStream_t st) {
+    constexpr bool BF16 = sizeof(T) == 2;
+    constexpr int ES = sizeof(T), KE = 128 / ES;      // operand element size, operand elements per k-block (one 128-byte row)
     float* Cm = Cs[0];
     const float* bias = ep->bias; const int act = ep->act, accumulate = ep->accumulate;
     if (act < 0 || act > 2) return go1_set_error("go1_gemm_ex: act must be 0, 1 or 2");
     if (!go1_act_kind_ok(ep->act_kind)) return go1_set_error("go1_gemm_ex: unknown activation kind (Go1Activation)");
     const int amn = transA ? 1 : 0, bmn = transB ? 0 : 1;     // A given as [K][M] / B given as [K][N]: MN-major operands
+    if (BF16 && (amn || bmn)) return go1_set_error("go1_gemm_bf16_ex: both operands must be K-major (transA = 0, transB = 1)");
+    const bool c16 = ep->out_bf16 != nullptr;
+    if (c16 && (!ep->store_transposed || (ep->ld_out_bf16 & 7) || ep->ld_out_bf16 < M || (((uintptr_t)ep->out_bf16) & 15)))
+        return go1_set_error("go1_gemm_ex: out_bf16 needs store_transposed, a 16-byte aligned output and ld_out_bf16 >= M, a multiple of 8");
     for (int p = 0; p < nprob; p++)
-        if ((lda & 3) || (ldb & 3) || (((uintptr_t)As[p] | (uintptr_t)Bs[p]) & 15) || !Cs[p])
-            return go1_set_error("go1_gemm impl=1: A/B must be 16-byte aligned with row strides that are multiples of 4 floats (TMA)");
+        if (((lda * ES) & 15) || ((ldb * ES) & 15) || (((uintptr_t)As[p] | (uintptr_t)Bs[p]) & 15) || (!Cs[p] && !c16))
+            return go1_set_error(BF16 ? "go1_gemm_bf16_ex: A/B must be 16-byte aligned with row strides that are multiples of 8 elements (TMA)"
+                                      : "go1_gemm impl=1: A/B must be 16-byte aligned with row strides that are multiples of 4 floats (TMA)");
     GemmArgs g;
     g.nprob = nprob; g.tiles_per_prob = 0;
     for (int p = 0; p < GEMM_MAXP; p++) g.Cg[p] = Cs[p < nprob ? p : 0];
     g.C = Cm; g.bias = bias; g.M = M; g.N = N; g.K = K; g.ldc = ldc; g.act = act; g.kind = ep->act_kind; g.accumulate = accumulate;
     g.ex = ep->extra; g.ldex = ep->ld_extra; g.wex = ep->w_extra; g.ldwex = ep->ld_w_extra; g.nex = ep->extra ? ep->num_extra : 0;
     g.aux = ep->dact_y; g.ldaux = ep->ld_dact_y;
-    g.amn = amn; g.bmn = bmn; g.lead = ep->lead_cols; g.colsum = ep->colsum; g.ct = ep->store_transposed ? 1 : 0;
+    g.amn = amn; g.bmn = bmn; g.lead = ep->lead_cols; g.colsum = ep->colsum; g.ct = ep->store_transposed ? 1 : 0; g.c16 = c16 ? 1 : 0;
     g.nbx = ep->num_bwd_extra; g.bx = ep->bwd_extra; g.bwx = ep->bwd_w_extra; g.gwx = ep->g_w_extra; g.dx = ep->d_extra;
     g.ldbx = ep->ld_bwd_extra; g.ldbwx = ep->ld_bwd_w_extra; g.ldgwx = ep->ld_g_w_extra; g.lddx = ep->ld_d_extra;
     if (g.nbx < 0 || g.nbx > 4 || (g.nbx > 0 && ((g.gwx && !g.bx) || (!g.gwx && !g.dx) || (g.dx && !g.bwx)))) return go1_set_error("go1_gemm_ex: bad fused trailing-input backward arguments");
     if (g.nex < 0 || g.nex > 4) return go1_set_error("go1_gemm_ex: num_extra must be 0..4");
     if (act == 2 && !g.aux) return go1_set_error("go1_gemm_ex: act 2 needs dact_y");
-    if (g.ct && (nprob != 1 || accumulate || M < 32 || (ldc & 3) || (((uintptr_t)Cm) & 15)))      // the transposed blocks leave by TMA store only
+    if (g.ct && (nprob != 1 || accumulate || M < 32 || (!c16 && ((ldc & 3) || (((uintptr_t)Cm) & 15)))))      // the transposed blocks leave by TMA store only
         return go1_set_error("go1_gemm_ex: store_transposed needs M >= 32, no accumulate and a 16-byte aligned C with ldc a multiple of 4");
-    const int num_kb = (K + BK - 1) / BK;
+    const int num_kb = (K + KE - 1) / KE;
     // Tile selection: 128 x BN tiles, BN = the smallest of 32 / 64 / 128 that covers N (128 beyond).  Plain products (no fused epilogue) with a
     // long reduction are split along K (partial tiles meet in C by vector reductions).
     constexpr int SPLIT_MIN_KB = 16;          // least k-blocks per split
@@ -1089,8 +1110,8 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     GemmMaps gm;
     // K-major: rows = M (or N), cols = K, box BK x tile rows.  MN-major: rows = K, cols = M (or N), box tile width x BK k-rows.
     for (int p = 0; p < nprob; p++) {
-        if (int e = amn ? make_map_mn(&gm.a[p], As[p], K, M, lda, BM) : make_map(&gm.a[p], As[p], M, K, lda, BM)) return e;
-        if (int e = bmn ? make_map_mn(&gm.b[p], Bs[p], K, N, ldb, BN) : make_map(&gm.b[p], Bs[p], N, K, ldb, BN)) return e;
+        if (int e = amn ? make_map_mn(&gm.a[p], (const float*)As[p], K, M, lda, BM) : make_map(&gm.a[p], As[p], M, K, lda, BM, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES)) return e;
+        if (int e = bmn ? make_map_mn(&gm.b[p], (const float*)Bs[p], K, N, ldb, BN) : make_map(&gm.b[p], Bs[p], N, K, ldb, BN, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES)) return e;
     }
     for (int p = nprob; p < GEMM_MAXP; p++) { gm.a[p] = gm.a[0]; gm.b[p] = gm.b[0]; }
     const CUtensorMap& ma = gm.a[0];
@@ -1101,7 +1122,8 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     const int cluster = (!amn && !bmn && nprob == 1 && act != 2 && BN == 128 && (tiles_n % 2 == 0 || tiles_m % 2 == 0)) ? 2 : 1;
     gm.half = ma;
     if (cluster == 2) {
-        if (int e = tiles_n % 2 == 0 ? make_map(&gm.half, As[0], M, K, lda, BM / 2) : make_map(&gm.half, Bs[0], N, K, ldb, BN / 2)) return e;
+        if (int e = tiles_n % 2 == 0 ? make_map(&gm.half, As[0], M, K, lda, BM / 2, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES)
+                                     : make_map(&gm.half, Bs[0], N, K, ldb, BN / 2, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES)) return e;
     }
     if (splits > 1) {
         if (!accumulate)
@@ -1112,26 +1134,31 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
     const bool timed = g_time_on && cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone;
     if (timed) {
         cudaEventRecord(timing_event(), st); g_time_flop += 2.0 * (double)M * (double)N * (double)K * nprob;
-        g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, BN, g.colsum ? 1 : 0, cluster, 0, 0, nprob});
+        g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, BN, g.colsum ? 1 : 0, cluster, 0, 0, nprob, BF16 ? 1 : 0});
     }
     int e;
     // staged epilogue: C blocks leave the accumulator staging by TMA store, the derivative operand arrives through TMA loads.  The direct
     // row-per-lane stores serve the rest: split-K partial tiles, accumulate, grouped launches, N < 32 and a misaligned C.
     CUtensorMap mc = ma, my = ma;
     g.tma_store = g.tma_aux = 0;
-    if (nprob == 1 && splits == 1 && !accumulate && (g.ct ? M : N) >= 32 && (ldc & 3) == 0 && (((uintptr_t)Cm) & 15) == 0) {
+    if (c16) {          // (a BF16 transposed store: checked above) 32 x 32 blocks of 64-byte rows, unswizzled
+        if (int e2 = make_map(&mc, ep->out_bf16, N, M, ep->ld_out_bf16, 32, 32, CU_TENSOR_MAP_SWIZZLE_NONE, 2)) return e2;
+        g.tma_store = 1;
+    } else if (nprob == 1 && splits == 1 && !accumulate && (g.ct ? M : N) >= 32 && (ldc & 3) == 0 && (((uintptr_t)Cm) & 15) == 0) {
         if (int e2 = g.ct ? make_map(&mc, Cm, N, M, ldc, 32) : make_map(&mc, Cm, M, N, ldc, 32)) return e2;
         g.tma_store = 1;
+    }
+    if (g.tma_store) {
         if (g.act == 2 && (g.ldaux & 3) == 0 && (((uintptr_t)g.aux) & 15) == 0) {
             if (int e2 = make_map(&my, g.aux, M, N, g.ldaux, 32)) return e2;
             g.tma_aux = 1;
         }
     }
     const bool any = g.act != 0 && g.kind != GO1_ACT_ELU;
-    if (cluster == 2) e = any ? launch_gemm<128, true, 2>(gm, mc, my, g, splits, st) : launch_gemm<128, false, 2>(gm, mc, my, g, splits, st);
-    else if (BN == 128) e = any ? launch_gemm<128, true, 1>(gm, mc, my, g, splits, st) : launch_gemm<128, false, 1>(gm, mc, my, g, splits, st);
-    else if (BN == 64) e = any ? launch_gemm<64, true, 1>(gm, mc, my, g, splits, st) : launch_gemm<64, false, 1>(gm, mc, my, g, splits, st);
-    else e = any ? launch_gemm<32, true, 1>(gm, mc, my, g, splits, st) : launch_gemm<32, false, 1>(gm, mc, my, g, splits, st);
+    if (cluster == 2) e = any ? launch_gemm<128, true, 2, BF16>(gm, mc, my, g, splits, st) : launch_gemm<128, false, 2, BF16>(gm, mc, my, g, splits, st);
+    else if (BN == 128) e = any ? launch_gemm<128, true, 1, BF16>(gm, mc, my, g, splits, st) : launch_gemm<128, false, 1, BF16>(gm, mc, my, g, splits, st);
+    else if (BN == 64) e = any ? launch_gemm<64, true, 1, BF16>(gm, mc, my, g, splits, st) : launch_gemm<64, false, 1, BF16>(gm, mc, my, g, splits, st);
+    else e = any ? launch_gemm<32, true, 1, BF16>(gm, mc, my, g, splits, st) : launch_gemm<32, false, 1, BF16>(gm, mc, my, g, splits, st);
     if (e) return e;
     if (splits > 1 && (bias || act))
         for (int p = 0; p < nprob; p++) { const size_t tot = (size_t)M * N; bias_act_strided<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cs[p], ldc, bias, M, N, act, ep->act_kind); go1_count_launch(1); }
@@ -1143,7 +1170,14 @@ static int gemm_tf32_impl(int transA, int transB, int M, int N, int K, int nprob
 
 extern "C" int go1_gemm_tf32(int transA, int transB, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
                              float* Cm, int ldc, const Go1GemmEpilogue* ep, cudaStream_t st) {
-    return gemm_tf32_impl(transA, transB, M, N, K, 1, &A, lda, &B, ldb, &Cm, ldc, ep, st);
+    return gemm_wgmma_impl<float>(transA, transB, M, N, K, 1, &A, lda, &B, ldb, &Cm, ldc, ep, st);
+}
+// BF16 operands, fp32 accumulation and output, the full fused epilogue of go1_gemm_ex impl 1 (include/go1_b200.h)
+extern "C" int go1_gemm_bf16_ex(int transA, int transB, int M, int N, int K, const uint16_t* A, int lda, const uint16_t* B, int ldb,
+                                float* Cm, int ldc, const Go1GemmEpilogue* ep, void* stream) {
+    if (!A || !B || !ep || M <= 0 || N <= 0 || K <= 0) return go1_set_error("go1_gemm_bf16_ex: bad arguments");
+    if (!ep->out_bf16 && (!Cm || ldc < N)) return go1_set_error("go1_gemm_bf16_ex: bad output");
+    return gemm_wgmma_impl<uint16_t>(transA, transB, M, N, K, 1, &A, lda, &B, ldb, &Cm, ldc, ep, (cudaStream_t)stream);
 }
 // nprob (<= 4) products of the same shape and operand strides in ONE grid: C[p] (+)= op(A[p]) op(B[p]).  Meant for the equal-shape
 // split-K wgrads of the three MLPs (128 x 256 x 24576 three times, 256 x 512 x 24576 twice per optimizer step): one launch fills the
@@ -1153,7 +1187,7 @@ extern "C" int go1_gemm_grouped(int transA, int transB, int M, int N, int K, int
     if (!A || !B || !C || nprob < 1 || nprob > GEMM_MAXP || M <= 0 || N <= 0 || K <= 0) return go1_set_error("go1_gemm_grouped: 1..4 problems");
     Go1GemmEpilogue ep = {};
     ep.accumulate = accumulate;
-    return gemm_tf32_impl(transA, transB, M, N, K, nprob, A, lda, B, ldb, C, ldc, &ep, (cudaStream_t)stream);
+    return gemm_wgmma_impl<float>(transA, transB, M, N, K, nprob, A, lda, B, ldb, C, ldc, &ep, (cudaStream_t)stream);
 }
 
 // dst[c][r] = src[r][c]  (32x32 smem tiles)

@@ -257,7 +257,7 @@ extern "C" int go1_gemm_tf32(int transA, int transB, int M, int N, int K, const 
 
 extern "C" int go1_gemm_ex(int transA, int transB, int M, int N, int K, const float* A, int lda, const float* B, int ldb,
                            float* Cm, int ldc, const Go1GemmEpilogue* epi, int impl, void* stream) {
-    if (!A || !B || !Cm || !epi || M <= 0 || N <= 0 || K <= 0) return go1_set_error("go1_gemm: bad arguments");
+    if (!A || !B || !epi || (!Cm && !epi->out_bf16) || M <= 0 || N <= 0 || K <= 0) return go1_set_error("go1_gemm: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
     if (epi->act < 0 || epi->act > 2) return go1_set_error("go1_gemm_ex: act must be 0, 1 or 2");
     if (!go1_act_kind_ok(epi->act_kind)) return go1_set_error("go1_gemm_ex: unknown activation kind (Go1Activation)");
@@ -265,7 +265,7 @@ extern "C" int go1_gemm_ex(int transA, int transB, int M, int N, int K, const fl
     if (impl != 0) return go1_set_error("go1_gemm: unknown impl");
     if (epi->lead_cols > 0) return go1_set_error("go1_gemm_ex: lead_cols is implemented by impl 1 only");
     if (epi->colsum || epi->num_bwd_extra > 0) return go1_set_error("go1_gemm_ex: the fused column sum / trailing-input backward are implemented by impl 1 only");
-    if (epi->store_transposed) return go1_set_error("go1_gemm_ex: store_transposed is implemented by impl 1 only");
+    if (epi->store_transposed || epi->out_bf16) return go1_set_error("go1_gemm_ex: store_transposed / out_bf16 are implemented by impl 1 only");
     const float* bias = epi->bias; const int act = epi->act, kind = epi->act_kind, accumulate = epi->accumulate;
     SgemmEp ep; ep.ex = epi->extra; ep.wex = epi->w_extra; ep.aux = epi->dact_y; ep.ldex = epi->ld_extra; ep.ldwex = epi->ld_w_extra;
     ep.nex = epi->extra ? epi->num_extra : 0; ep.ldaux = epi->ld_dact_y;
@@ -1261,10 +1261,12 @@ __global__ void __launch_bounds__(256) store_transition_kernel(StoreArgs a) {
     const int t = threadIdx.x;
     if (a.slot_dev) {
         const size_t off = (size_t)(*a.slot_dev) * a.n;
-        a.s_obs += off * a.nobs; a.s_priv += off * a.npriv; a.s_hist += off * a.nhist; a.s_actions += off * a.nact; a.s_rewards += off;
+        a.s_obs += off * a.nobs; a.s_priv += off * a.npriv; if (a.hist) a.s_hist += off * a.nhist; a.s_actions += off * a.nact; a.s_rewards += off;
         a.s_values += off; a.s_logp += off; a.s_mu += off * a.nact; a.s_sigma += off * a.nact; a.s_env_bins += off; a.s_dones += off;
     }
-    if ((a.nhist & 3) == 0) {
+    if (!a.hist) {
+        // (the history is stored by go1_rollout_store_rows_bf16: AC_Args.gemm_impl = 2 keeps a BF16 slab)
+    } else if ((a.nhist & 3) == 0) {
         const float4* src = reinterpret_cast<const float4*>(a.hist + (size_t)e * a.nhist);
         float4* dst = reinterpret_cast<float4*>(a.s_hist + (size_t)e * a.nhist);
         for (int c = t; c < a.nhist / 4; c += blockDim.x) dst[c] = src[c];
@@ -1343,7 +1345,8 @@ extern "C" int go1_store_transition(const float* const* in_f32, const uint8_t* d
     a.s_obs = out_f32[0]; a.s_priv = out_f32[1]; a.s_hist = out_f32[2]; a.s_actions = out_f32[3]; a.s_rewards = out_f32[4]; a.s_values = out_f32[5];
     a.s_logp = out_f32[6]; a.s_mu = out_f32[7]; a.s_sigma = out_f32[8]; a.s_env_bins = out_f32[9]; a.s_dones = s_dones;
     a.n = n; a.nobs = nobs; a.npriv = npriv; a.nhist = nhist; a.nact = nact; a.gamma = gamma; a.slot_dev = nullptr;
-    for (int i = 2; i < 9; i++) if (!in_f32[i] || !out_f32[i]) return go1_set_error("go1_store_transition: null tensor");
+    for (int i = 3; i < 9; i++) if (!in_f32[i] || !out_f32[i]) return go1_set_error("go1_store_transition: null tensor");
+    if (in_f32[2] && !out_f32[2]) return go1_set_error("go1_store_transition: null tensor");
     if ((in_f32[0] && !out_f32[0]) || (in_f32[1] && !out_f32[1])) return go1_set_error("go1_store_transition: null tensor");
     if (!out_f32[9]) return go1_set_error("go1_store_transition: null tensor");
     store_transition_kernel<<<n, 256, 0, (cudaStream_t)stream>>>(a); go1_count_launch(1);
@@ -1362,7 +1365,8 @@ extern "C" int go1_rollout_store_transition(const float* const* in_f32, const ui
     a.s_values = out_base_f32[5]; a.s_logp = out_base_f32[6]; a.s_mu = out_base_f32[7]; a.s_sigma = out_base_f32[8]; a.s_env_bins = out_base_f32[9];
     a.s_dones = s_dones_base; a.slot_dev = slot_dev;
     a.n = n; a.nobs = nobs; a.npriv = npriv; a.nhist = nhist; a.nact = nact; a.gamma = gamma;
-    for (int i = 2; i < 9; i++) if (!in_f32[i] || !out_base_f32[i]) return go1_set_error("go1_rollout_store_transition: null tensor");
+    for (int i = 3; i < 9; i++) if (!in_f32[i] || !out_base_f32[i]) return go1_set_error("go1_rollout_store_transition: null tensor");
+    if (in_f32[2] && !out_base_f32[2]) return go1_set_error("go1_rollout_store_transition: null tensor");
     if (!out_base_f32[9] || (in_f32[0] && !out_base_f32[0]) || (in_f32[1] && !out_base_f32[1])) return go1_set_error("go1_rollout_store_transition: null tensor");
     store_transition_kernel<<<n, 256, 0, (cudaStream_t)stream>>>(a); go1_count_launch(1);
     return cuda_rc("go1_rollout_store_transition");

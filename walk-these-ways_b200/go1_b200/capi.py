@@ -45,6 +45,14 @@ def history_pitch(width):
     return row_pitch(width)
 
 
+def bf16_pitch(width):
+    """Row pitch (elements) of a BF16 buffer that a tensor-core product reads or writes through TMA (AC_Args.gemm_impl = 2): row strides must
+    be multiples of 16 bytes, 8 elements.  Widths that are multiples of 8 keep their natural pitch, the others are rounded up to a multiple
+    of 64 elements (128-byte aligned rows, the width of one TMA box row).  Holders expose the width as a [:, :width] view."""
+    width = int(width)
+    return width if width % 8 == 0 else (width + 63) // 64 * 64
+
+
 RESET_RAND_STRIDE = 48
 MAX_LAG_TIMESTEPS = 32
 _i, _f = C.c_int32, C.c_float
@@ -140,7 +148,7 @@ class Go1GemmEpilogue(C.Structure):
                 ("ld_w_extra", _i), ("num_extra", _i), ("dact_y", C.c_void_p), ("ld_dact_y", _i), ("lead_cols", _i), ("colsum", C.c_void_p),
                 ("bwd_extra", C.c_void_p), ("bwd_w_extra", C.c_void_p), ("g_w_extra", C.c_void_p), ("d_extra", C.c_void_p),
                 ("ld_bwd_extra", _i), ("ld_bwd_w_extra", _i), ("ld_g_w_extra", _i), ("ld_d_extra", _i), ("num_bwd_extra", _i), ("act_kind", _i),
-                ("store_transposed", _i)]
+                ("store_transposed", _i), ("out_bf16", C.c_void_p), ("ld_out_bf16", _i)]
 
 
 class Go1TailProblem(C.Structure):
@@ -214,6 +222,12 @@ def lib():
         "go1_skinny_dgrad_ex": ([vp, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, vp], ip),
         "go1_skinny_dgrad_act": ([vp, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, ip, vp], ip),
         "go1_skinny_wgrad_ex": ([vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, ip, vp], ip),
+        "go1_gemm_bf16_ex": ([ip, ip, ip, ip, ip, vp, ip, vp, ip, vp, ip, C.POINTER(Go1GemmEpilogue), vp], ip),
+        "go1_convert_bf16": ([vp, ip, vp, ip, ip, ip, vp], ip),
+        "go1_gather_rows_bf16": ([vp, ip, vp, vp, ip, i64, ip, vp], ip),
+        "go1_rollout_store_rows_bf16": ([vp, ip, vp, ip, vp, ip, ip, vp], ip),
+        "go1_transpose_to_bf16": ([vp, ip, vp, ip, ip, ip, vp], ip),
+        "go1_transpose_bf16": ([vp, ip, vp, ip, ip, ip, vp], ip),
         "go1_gemm_grouped": ([ip, ip, ip, ip, ip, ip, C.POINTER(vp), ip, C.POINTER(vp), ip, C.POINTER(vp), ip, ip, vp], ip),
         "go1_copy_segments": ([C.POINTER(Go1CopySeg), ip, vp], ip),
         "go1_skinny_forward": ([vp, ip, vp, ip, vp, vp, ip, ip, ip, ip, vp], ip),

@@ -180,12 +180,14 @@ class Runner:
         else:
             env._roll(core.obs)
         send_to = bool(base.cfg.env.send_timeouts)
-        ins = [None, None, hist, actions, core.rew, values, ac._logp, ac._mean, ac.std.data, dc.env_bins_f32]
+        h16 = ac.model_inputs.get("act") if stg.hist_bf16 else None       # a BF16 slab stores the BF16 history the policy just evaluated
+        assert h16 is not None or not stg.hist_bf16
+        ins = [None, None, None if stg.hist_bf16 else hist, actions, core.rew, values, ac._logp, ac._mean, ac.std.data, dc.env_bins_f32]
         outs = [stg.observations, stg.privileged_observations, stg.observation_histories, stg.actions, stg.rewards, stg.values, stg.actions_log_prob,
                 stg.mu, stg.sigma, stg.env_bins]
         for x in ins[3:]:
             assert x.is_contiguous() and x.dtype == torch.float32
-        assert stg.history_rows_fit(hist) and hist.dtype == torch.float32      # the store copies whole rows at the slab's pitch
+        assert stg.hist_bf16 or (stg.history_rows_fit(hist) and hist.dtype == torch.float32)      # the store copies whole rows at the slab's pitch
         from .ppo import PPO_Args
 
         def store_and_advance():
@@ -193,6 +195,9 @@ class Runner:
                                                       capi.ptr(dc.time_outs_u8) if send_to else None, (C.c_void_p * 10)(*[x.data_ptr() for x in outs]),
                                                       capi.ptr(stg.dones), capi.ptr(sg["slot"]), N, core.num_obs, core.num_priv, stg.hist_row_pitch,
                                                       actions.shape[1], float(PPO_Args.gamma), sp()), "go1_rollout_store_transition")
+            if h16 is not None:
+                capi.check(L.go1_rollout_store_rows_bf16(capi.ptr(h16), h16.stride(0), capi.ptr(stg._hist_slab), stg.hist_row_pitch, capi.ptr(sg["slot"]),
+                                                         N, h16.shape[1], sp()), "go1_rollout_store_rows_bf16")
             capi.check(L.go1_rollout_advance(capi.ptr(sg["acc"]), capi.ptr(sg["acc_hist"]), sg["W"], sg["T"], capi.ptr(sg["slot"]), capi.ptr(core.step_dev), sp()),
                        "go1_rollout_advance")
 

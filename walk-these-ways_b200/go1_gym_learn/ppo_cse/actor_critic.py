@@ -29,7 +29,8 @@ class AC_Args(PrefixProto, cli=False):
     activation = 'elu'  # can be elu, relu, selu, crelu, lrelu, tanh, sigmoid (all run on the fused kernels; crelu is nn.ReLU, as in the reference)
     adaptation_module_branch_hidden_dims = [256, 128]
     use_decoder = False
-    gemm_impl = 1       # 1 = wgmma TF32 tensor cores (default; torch 1.10, the reference's pin, also ran these matmuls in TF32), 0 = fp32 CUDA cores (exact)
+    gemm_impl = 1       # 1 = wgmma TF32 tensor cores (default; torch 1.10, the reference's pin, also ran these matmuls in TF32), 0 = fp32 CUDA cores (exact),
+                        # 2 = as 1, but the products that reduce over the observation history (the first layers) take BF16 operands (fp32 accumulation)
 
 
 def _mlp(in_dim, hidden, out_dim, activation):
@@ -41,11 +42,11 @@ def _mlp(in_dim, hidden, out_dim, activation):
     return nn.Sequential(*layers)
 
 
-def _empty(*shape, device):
+def _empty(*shape, device, dtype=torch.float32):
     """Scratch buffers outlive the Runner's torch.inference_mode() rollout block and are written again by the update,
     so they must be ordinary (non-inference) tensors whichever mode they are first needed in."""
     with torch.inference_mode(False):
-        return torch.empty(*shape, device=device)
+        return torch.empty(*shape, device=device, dtype=dtype)
 
 
 def history_kmajor(h, priv, out):
@@ -58,6 +59,18 @@ def history_kmajor(h, priv, out):
     out[K0, :M].fill_(1.0)
     if priv is not None:
         capi.check(L.go1_transpose(capi.ptr(priv), priv.stride(0), capi.ptr(out[K0 + 1:]), out.stride(0), M, priv.shape[1], st), "transpose")
+    return out
+
+
+def history_kmajor_bf16(h16, priv, out):
+    """history_kmajor for AC_Args.gemm_impl = 2: h16 is the BF16 history [M][K0], out a BF16 [K0 + 1 + 2E][>= M] buffer (row pitch a
+    multiple of 8 elements); the history rows are copied, the ones row is exact and priv is rounded to BF16 (nearest even)."""
+    M, K0 = h16.shape[0], h16.shape[1]
+    L, st = capi.lib(), capi.stream_ptr()
+    capi.check(L.go1_transpose_bf16(capi.ptr(h16), h16.stride(0), capi.ptr(out), out.stride(0), M, K0, st), "transpose_bf16")
+    out[K0, :M].fill_(1.0)
+    if priv is not None:
+        capi.check(L.go1_transpose_to_bf16(capi.ptr(priv), priv.stride(0), capi.ptr(out[K0 + 1:]), out.stride(0), M, priv.shape[1], st), "transpose_to_bf16")
     return out
 
 
@@ -96,14 +109,18 @@ class _Net:
         else:
             self.tail_start = None
 
-    def _buf(self, key, M, width, pitch=None):
+    def _buf(self, key, M, width, pitch=None, dtype=torch.float32):
         """[M][width] view of a cached buffer with row pitch `pitch` (default: width)."""
         pitch = width if pitch is None else pitch
         t = self.acts.get(key)
-        if t is None or t.shape[0] < M or t.shape[1] != pitch:
-            t = _empty(M, pitch, device=self.flat.device)
+        if t is None or t.shape[0] < M or t.shape[1] != pitch or t.dtype != dtype:
+            t = _empty(M, pitch, device=self.flat.device, dtype=dtype)
             self.acts[key] = t
         return t[:M, :width]
+
+    def _buf16(self, key, M, width):
+        """A BF16 operand buffer of AC_Args.gemm_impl = 2 (TMA-readable rows: capi.bf16_pitch)."""
+        return self._buf(key, M, width, capi.bf16_pitch(width), torch.bfloat16)
 
     def _hbuf(self, key, M, width):
         """A hidden activation or gradient buffer: TMA-readable rows whatever the width."""
@@ -116,6 +133,19 @@ class _Net:
         W = self.flat[wo:wo + o * i]
         KPk = (K + 31) // 32 * 32
         return self._cached(("pack", li), lambda old: (old if old is not None else _empty(o, KPk, device=W.device)[:, :K]).copy_(W.view(o, i)[:, :K])), KPk
+
+    def _packed16(self, li, K):
+        """(copy, pitch): W[:, :K] of layer li in BF16 (rounded to nearest even), row pitch capi.bf16_pitch(K), rebuilt once per weight version
+        (AC_Args.gemm_impl = 2: the first layers' operand)."""
+        wo, bo, o, i = self.specs[li]
+        W = self.flat[wo:wo + o * i]
+        KPk = capi.bf16_pitch(K)
+
+        def build(old):
+            dst = old if old is not None else _empty(o, KPk, device=W.device, dtype=torch.bfloat16)[:, :K]
+            capi.check(capi.lib().go1_convert_bf16(W.data_ptr(), i, capi.ptr(dst), KPk, o, K, capi.stream_ptr()), "convert_bf16")
+            return dst
+        return self._cached(("pack16", li), build), KPk
 
     def _weight_tma(self, li):
         """(W, row stride) of layer li for a TMA operand: in place when its rows allow it, else the packed copy."""
@@ -147,8 +177,11 @@ class _Net:
         return x.data_ptr() if torch.is_tensor(x) else x
 
     def _gemm(self, ta, tb, M, N, K, A, lda, B, ldb, Cm, ldc, bias=None, act=0, acc=0, impl=0, extra=None, w_extra=0, ld_w_extra=0, dact_y=None, lead_cols=0,
-              colsum=None, bwd_extra=None, store_transposed=0):
+              colsum=None, bwd_extra=None, store_transposed=0, bf16=False, out16=None):
+        """go1_gemm_ex (impl 0 / 1), or go1_gemm_bf16_ex with bf16: A and B BF16.  out16: a BF16 tensor that receives the transposed result
+        (store_transposed) in place of Cm."""
         ep = self._ep
+        ep.out_bf16, ep.ld_out_bf16 = (out16.data_ptr(), out16.stride(0)) if out16 is not None else (None, 0)
         ep.lead_cols = lead_cols
         ep.store_transposed = store_transposed
         ep.colsum = self._p(colsum) if colsum is not None else None
@@ -169,7 +202,10 @@ class _Net:
             ep.dact_y, ep.ld_dact_y = dact_y.data_ptr(), dact_y.stride(0)
         else:
             ep.dact_y = None
-        capi.check(capi.lib().go1_gemm_ex(ta, tb, M, N, K, self._p(A), lda, self._p(B), ldb, self._p(Cm), ldc, ep, impl, capi.stream_ptr()), "go1_gemm")
+        if bf16:
+            capi.check(capi.lib().go1_gemm_bf16_ex(ta, tb, M, N, K, self._p(A), lda, self._p(B), ldb, self._p(Cm), ldc, ep, capi.stream_ptr()), "go1_gemm_bf16")
+        else:
+            capi.check(capi.lib().go1_gemm_ex(ta, tb, M, N, K, self._p(A), lda, self._p(B), ldb, self._p(Cm), ldc, ep, impl, capi.stream_ptr()), "go1_gemm")
 
     @staticmethod
     def _tma_ok(x, ld):
@@ -188,34 +224,40 @@ class _Net:
                 outs.append(first_out)
                 inp, ld_in = first_out, first_out.stride(0)
                 continue
-            if li == self.tail_start and impl == 1 and self._tail_ok() and self._tma_ok(inp, ld_in):
+            if li == self.tail_start and impl >= 1 and self._tail_ok() and self._tma_ok(inp, ld_in):
                 return outs if defer_tail else outs + self._forward_tail(inp, ld_in, M, tag)
             y = self._hbuf((tag, li), M, o) if li < n - 1 else self._buf((tag, li), M, o)
             W = self.flat[wo:wo + o * i]
             b = self.flat[bo:bo + o]
             act = 1 if li < n - 1 else 0
             first_extra = li == 0 and extra is not None
-            if impl == 1 and li == n - 1 and li > 0 and o <= 16 and i % 4 == 0 and i <= 512 and self._tma_ok(inp, ld_in):
+            if impl >= 1 and li == n - 1 and li > 0 and o <= 16 and i % 4 == 0 and i <= 512 and self._tma_ok(inp, ld_in):
                 # the narrow head: one bandwidth-bound pass instead of a padded tensor-core tile
                 capi.check(capi.lib().go1_skinny_forward(self._p(inp), ld_in, W.data_ptr(), i, b.data_ptr(), capi.ptr(y), y.stride(0), M, o, i, capi.stream_ptr()), "skinny_forward")
                 outs.append(y)
                 continue
             K = K0 if first_extra else i
             Wm, ldw = W, i
-            tc = impl == 1 and self._tma_ok(inp, ld_in)
-            if tc and (not self._tma_ok(W, i) or (li == 0 and K >= 1024 and i % 32 != 0)):
+            bf16 = li == 0 and impl == 2        # the history product: BF16 input (ActorCritic._model_input) and weights
+            if li == 0 and (inp.dtype == torch.bfloat16) != bf16:
+                raise capi.Go1Error("BF16 observation histories are the input of AC_Args.gemm_impl = 2 only")
+            tc = impl >= 1 and self._tma_ok(inp, ld_in)
+            if bf16:
+                Wm, ldw = self._packed16(li, K)
+            elif tc and (not self._tma_ok(W, i) or (li == 0 and K >= 1024 and i % 32 != 0)):
                 # for the long first-layer rows the packed copy's aligned pitch alone is worth 30 % (misaligned 128-byte box rows cost an
                 # extra L2 sector each)
                 Wm, ldw = self._packed(li, K)
             ldy = y.stride(0)
             if first_extra and i - K0 > 4:      # wide trailing input: y = x W[:, :K0]^T + b, then y = act(y + extra W[:, K0:]^T)
-                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, ldy, b, 0, 0, 1 if tc else 0)
+                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, ldy, b, 0, 0, 1 if tc else 0, bf16=bf16)
                 capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(y), ldy, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i, M, o, i - K0,
                                                             capi.act_arg(self.kind, act), capi.stream_ptr()), "go1_mlp_extra_forward")
             elif first_extra:   # y = act(x W[:, :K0]^T + extra W[:, K0:]^T + b): the (at most 4) trailing columns ride in the epilogue
-                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, ldy, b, act, 0, 1 if tc else 0, extra=extra, w_extra=W.data_ptr() + 4 * K0, ld_w_extra=i)
+                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, ldy, b, act, 0, 1 if tc else 0, extra=extra, w_extra=W.data_ptr() + 4 * K0, ld_w_extra=i,
+                           bf16=bf16)
             else:
-                self._gemm(0, 1, M, o, K, inp, ld_in, Wm, ldw, y, ldy, b, act, 0, 1 if tc else 0)
+                self._gemm(0, 1, M, o, K, inp, ld_in, Wm, ldw, y, ldy, b, act, 0, 1 if tc else 0, bf16=bf16)
             outs.append(y)
             inp, ld_in = y, y.stride(0)
         return outs
@@ -266,12 +308,14 @@ class _Net:
         the activation's derivative, computed from the saved layer output (fused epilogue).  dz1T: optional [o1][M] strided view; when
         given the first layer's dz is stored there transposed (K-major for the weight-gradient product) and that layer's wgrad, bias
         gradient and trailing-input weight gradients are left to the caller (ActorCritic._first_layer_wgrad: augmented rows of the
-        transposed input).  wgrads: optional list that collects the tensor-core wgrads instead of launching them (ActorCritic._flush_wgrads
+        transposed input).  A BF16 dz1T (AC_Args.gemm_impl = 2) receives the rounded dz; the bias, d(extra) and trailing-input reductions
+        see the fp32 values.  wgrads: optional list that collects the tensor-core wgrads instead of launching them (ActorCritic._flush_wgrads
         launches equal shapes as grouped products).  Returns d(extra) [M][E] if requested."""
         L, st = capi.lib(), capi.stream_ptr()
         dz, dextra = dout, None
         bias_done = False      # this layer's bias gradient was reduced by the dgrad that made its dz, or is left to the caller
         extra_done = False     # likewise the first layer's trailing-input gradients
+        dz1T16 = None          # a BF16 dz1T filled from the fp32 dz once go1_mlp_extra_backward has read that
         for li in range(len(self.specs) - 1, -1, -1):
             wo, bo, o, i = self.specs[li]
             W = self.flat[wo:wo + o * i]
@@ -282,7 +326,7 @@ class _Net:
             else:
                 inp, ld_in, K = outs[li - 1], outs[li - 1].stride(0), i
             wgrad_done = li == 0 and dz1T is not None       # made by the caller
-            if impl == 1 and M >= 64 and not self._tma_ok(dz, ldz) and (o > 16 or (li == 1 and dz1T is not None)):
+            if impl >= 1 and M >= 64 and not self._tma_ok(dz, ldz) and (o > 16 or (li == 1 and dz1T is not None)):
                 # a head gradient whose rows TMA cannot read ([M][1] values, [M][E] latents) where a tensor-core product must read it: the
                 # wgrad and dgrad of a head wider than the skinny kernels take, or a one-hidden-layer net's dgrad that stores the first-layer
                 # dz transposed
@@ -304,7 +348,7 @@ class _Net:
             elif skinny:
                 capi.check(L.go1_skinny_wgrad(capi.ptr(dz), ldz, capi.ptr(inp), ld_in, gW.data_ptr(), i, M, o, K, 1, st), "skinny_wgrad")
             else:       # impl 1: both operands MN-major, read in place by the wgmma kernel; split-K partial tiles add into the zeroed gradient
-                tc = impl == 1 and M >= 64 and self._tma_ok(dz, ldz) and self._tma_ok(inp, ld_in)
+                tc = impl >= 1 and M >= 64 and self._tma_ok(dz, ldz) and self._tma_ok(inp, ld_in)
                 if tc and wgrads is not None:
                     wgrads.append((o, K, M, ldz, ld_in, i, dz, inp, gW))
                 else:
@@ -319,14 +363,23 @@ class _Net:
                     gwx = gW.data_ptr() + 4 * K0 if dz1T is None else None
                     capi.check(L.go1_mlp_extra_backward(capi.ptr(dz), ldz, 0 if dz1T is None else 1, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i,
                                                         gwx, i, capi.ptr(dextra) if want_dextra else None, E, M, o, E, 0, st), "extra_backward")
+                if dz1T16 is not None:
+                    capi.check(L.go1_convert_bf16(capi.ptr(dz), ldz, capi.ptr(dz1T16), dz1T16.stride(0), o, M, st), "convert_bf16")
                 return dextra
             # ---- 3. dgrad (+ fused activation derivative): dz_prev[M][i] = (dz[M][o] W[o][i]) * f'(y_prev)
             pwo, pbo, po, pi = self.specs[li - 1]
             gb_prev, yprev = self.grad[pbo:pbo + po], outs[li - 1]
             to_T = li == 1 and dz1T is not None
             dprev = dz1T if to_T else self._hbuf((tag, "d", li - 1), M, i)
-            ldp = dprev.stride(0)
-            if impl == 1 and self._tma_ok(dz, ldz) and M >= 64:      # (the 12-wide actor head included: 19 us here, 22 us on the skinny pass)
+            out16 = None
+            if to_T and dz1T.dtype == torch.bfloat16:
+                if extra is not None and pi - K0 > 4 and want_dextra:
+                    # a wide trailing input's d(extra) is a pass over the stored dz (go1_mlp_extra_backward): fp32 first, the BF16 copy after it
+                    dz1T16, dprev = dz1T, self._buf((tag, "dz1T32"), i, M, capi.row_pitch(M))
+                else:
+                    out16, dprev = dz1T, None
+            ldp = dprev.stride(0) if dprev is not None else 0
+            if impl >= 1 and self._tma_ok(dz, ldz) and M >= 64:      # (the 12-wide actor head included: 19 us here, 22 us on the skinny pass)
                 # W read MN-major (in place, or its packed copy when its rows are not 16-byte multiples); the bias gradient of layer li-1
                 # (column sums of dprev) rides in the epilogue
                 Wd, ldwd = self._weight_tma(li)
@@ -341,19 +394,19 @@ class _Net:
                     if dextra is not None or gwx is not None:
                         bx = (extra, self.flat.data_ptr() + 4 * (pwo + K0), pi, gwx, pi, dextra)
                 self._gemm(0, 0, M, i, o, dz, ldz, Wd, ldwd, dprev, ldp, None, 2, 0, 1, dact_y=yprev, colsum=None if to_T else gb_prev, bwd_extra=bx,
-                           store_transposed=1 if to_T else 0)
+                           store_transposed=1 if to_T else 0, out16=out16)
                 bias_done = True
             elif to_T:
                 raise capi.Go1Error("transposed first-layer dz: the dgrad that produces it must be a tensor-core product")
             elif o <= 16:
                 # the bias gradient of layer li-1 (column sums of dprev) is reduced in the same pass where the operands allow it
-                bias_done = impl == 1 and i % 4 == 0 and self._tma_ok(W, i) and self._tma_ok(dprev, ldp) and self._tma_ok(yprev, yprev.stride(0))
+                bias_done = impl >= 1 and i % 4 == 0 and self._tma_ok(W, i) and self._tma_ok(dprev, ldp) and self._tma_ok(yprev, yprev.stride(0))
                 capi.check(L.go1_skinny_dgrad_act(capi.ptr(dz), ldz, capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(dprev), ldp,
                                                   gb_prev.data_ptr() if bias_done else None, M, o, i, self.kind, st), "skinny_dgrad")
             else:
                 self._gemm(0, 0, M, i, o, dz, ldz, W, i, dprev, ldp, None, 2, 0, 0, dact_y=yprev)
                 bias_done = False
-            dz = dprev
+            dz = dprev if dprev is not None else out16
 
 
 class ActorCritic(nn.Module):
@@ -393,6 +446,7 @@ class ActorCritic(nn.Module):
         import os
         self.update_streams = os.environ.get("GO1_UPDATE_STREAMS", "1") != "0"     # critic chain on a second stream during the update (measured -1.3 ms / iteration)
         self._side = None
+        self.model_inputs = {}        # AC_Args.gemm_impl = 2: tag -> the BF16 history the last call with that tag read (see _model_input)
         self.fuse_tail = os.environ.get("GO1_FUSE_TAIL", "1") != "0"     # layers behind a first layer in one wgmma launch (go1_mlp_tail_forward_grouped: actor + critic bodies in one grid)
 
     # ------------------------------------------------------------------ flat storage
@@ -486,17 +540,32 @@ class ActorCritic(nn.Module):
         return (0.5 + 0.5 * torch.log(torch.tensor(2 * torch.pi)) + torch.log(self.std.detach())).sum().expand(self._mean.shape[0])
 
     def _impl(self):
-        return int(AC_Args.gemm_impl)
+        impl = int(AC_Args.gemm_impl)
+        if impl not in (0, 1, 2):
+            raise ValueError(f"AC_Args.gemm_impl = {AC_Args.gemm_impl!r}: expected 0 (fp32 CUDA cores), 1 (TF32 tensor cores) or 2 (BF16 history products)")
+        return impl
 
     def _check_input(self, h):
         if not h.is_cuda:
             raise capi.Go1Error("ActorCritic runs on CUDA kernels only (no CPU fallback)")
-        assert h.dtype == torch.float32 and h.stride(1) == 1
+        assert (h.dtype == torch.float32 or (h.dtype == torch.bfloat16 and self._impl() == 2)) and h.stride(1) == 1
+
+    def _model_input(self, h, tag):
+        """The observation history as the first layers read it: at AC_Args.gemm_impl = 2 in BF16 (rounded to nearest even, once per call, into a
+        buffer kept per tag; a BF16 history -- RolloutStorage's minibatches -- is used as it is), else h itself.  The rollout's policy
+        evaluation reads the copy that RolloutStorage then stores in its BF16 slab, so the update reads the identical operands."""
+        self._check_input(h)
+        if self._impl() != 2 or h.dtype == torch.bfloat16:
+            return h
+        M, K0 = h.shape[0], self.num_obs_history
+        h16 = self._nets["adapt"]._buf16((tag, "h16"), M, K0)
+        capi.check(capi.lib().go1_convert_bf16(capi.ptr(h), h.stride(0), capi.ptr(h16), h16.stride(0), M, K0, capi.stream_ptr()), "convert_bf16")
+        self.model_inputs[tag] = h16
+        return h16
 
     def update_distribution(self, observation_history, tag="act"):
         self.flatten()
-        self._check_input(observation_history)
-        h = observation_history
+        h = self._model_input(observation_history, tag)
         M, K0 = h.shape[0], self.num_obs_history
         self._a_out = self._nets["adapt"].forward(h, h.stride(0), K0, None, M, self._impl(), tag)
         latent = self._a_out[-1]
@@ -511,13 +580,12 @@ class ActorCritic(nn.Module):
         (latent columns + activation) by go1_mlp_extra_forward once the adaptation module has produced the latent.  With E > 4 the
         epilogue finishes only the adaptation slice and go1_mlp_extra_forward also finishes the critic slice (priv columns)."""
         self.flatten()
-        self._check_input(observation_history)
-        h, priv = observation_history, privileged_observations.contiguous()
+        h, priv = self._model_input(observation_history, tag), privileged_observations.contiguous()
         M, K0, impl = h.shape[0], self.num_obs_history, self._impl()
         nets = self._nets
         na, npol, ncr = nets["adapt"], nets["actor"], nets["critic"]
         E = self.num_privileged_obs
-        fused = impl == 1 and _Net._tma_ok(h, h.stride(0)) and 1 <= E <= self.MAX_PRIVILEGED_OBS and \
+        fused = impl >= 1 and _Net._tma_ok(h, h.stride(0)) and 1 <= E <= self.MAX_PRIVILEGED_OBS and \
             npol.specs[0][3] == K0 + E and ncr.specs[0][3] == K0 + E and na.specs[0][3] == K0
         if not fused:
             self.update_distribution(h, tag)
@@ -548,13 +616,21 @@ class ActorCritic(nn.Module):
             return old
 
         Wcat, bcat, xcat = na._cached(("l1cat", "all"), build_all)
+        bf16 = impl == 2
+        if bf16:                # the block in BF16 (rounded to nearest even; the padding rows stay zero), refreshed with the fp32 one
+            def build_all16(old):
+                W32 = na._cached(("l1cat", "all"), build_all)[0]
+                W16 = old if old is not None else _empty(NC, capi.bf16_pitch(K0), device=flat.device, dtype=torch.bfloat16)[:, :K0]
+                capi.check(capi.lib().go1_convert_bf16(capi.ptr(W32), W32.stride(0), capi.ptr(W16), W16.stride(0), NC, K0, capi.stream_ptr()), "convert_bf16")
+                return W16
+            Wcat = na._cached(("l1cat16", "all"), build_all16)
         y = na._buf((tag, "y1cat"), M, NC)
         ya, yc, yp = y[:, :oa], y[:, Pa:Pa + oc], y[:, Pa + Pc:Pa + Pc + op]
         if E <= 4:
             na._gemm(0, 1, M, NC, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1,
-                     extra=priv, w_extra=xcat.data_ptr(), ld_w_extra=E, lead_cols=Pa + Pc)
+                     extra=priv, w_extra=xcat.data_ptr(), ld_w_extra=E, lead_cols=Pa + Pc, bf16=bf16)
         else:       # wide privileged input: only the adaptation slice is finished in the epilogue; the critic slice gets priv here
-            na._gemm(0, 1, M, NC, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1, lead_cols=Pa)
+            na._gemm(0, 1, M, NC, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1, lead_cols=Pa, bf16=bf16)
             capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(yc), yc.stride(0), capi.ptr(priv), priv.stride(0), Wc.data_ptr() + 4 * K0, K0 + E,
                                                         M, oc, E, capi.act_arg(self.act_kind, 1), capi.stream_ptr()), "go1_mlp_extra_forward")
         ts = npol.tail_start
@@ -664,22 +740,21 @@ class ActorCritic(nn.Module):
         if observation_history.shape[0] == 0:
             return observation_history.new_zeros(0, self.num_actions)
         self.flatten()
-        h = observation_history
+        h = self._model_input(observation_history, "teacher")
         out = self._nets["actor"].forward(h, h.stride(0), self.num_obs_history, privileged_info.contiguous(), h.shape[0], self._impl(), "teacher")
         policy_info["latents"] = privileged_info
         return out[-1]
 
     def evaluate(self, observation_history, privileged_observations, tag="act", **kwargs):
         self.flatten()
-        self._check_input(observation_history)
-        h = observation_history
+        h = self._model_input(observation_history, tag)
         self._c_out = self._nets["critic"].forward(h, h.stride(0), self.num_obs_history, privileged_observations.contiguous(), h.shape[0], self._impl(), tag)
         self._value = self._c_out[-1]
         return self._value
 
     def get_student_latent(self, observation_history):
         self.flatten()
-        h = observation_history
+        h = self._model_input(observation_history, "latent")
         return self._nets["adapt"].forward(h, h.stride(0), self.num_obs_history, None, h.shape[0], self._impl(), "latent")[-1]
 
     # ------------------------------------------------------------------ explicit backward passes (ppo.py:154-189)
@@ -703,20 +778,21 @@ class ActorCritic(nn.Module):
     def _first_layers_fusable(self, h, priv):
         """The first layers of the three nets can run their backward as one K-major product over hT (history_kmajor)."""
         nets, K0, E = self._nets, self.num_obs_history, self.num_privileged_obs
-        return self._impl() == 1 and h.shape[0] >= 64 and _Net._tma_ok(h, h.stride(0)) and 1 <= E <= self.MAX_PRIVILEGED_OBS and priv.shape[1] == E and \
+        return self._impl() >= 1 and h.shape[0] >= 64 and _Net._tma_ok(h, h.stride(0)) and 1 <= E <= self.MAX_PRIVILEGED_OBS and priv.shape[1] == E and \
             nets["actor"].specs[0][3] == K0 + E and nets["critic"].specs[0][3] == K0 + E and nets["adapt"].specs[0][3] == K0
 
     def _first_layer_wgrad(self, names, dz1T, hT, M, tag):
         """Weight gradients of the listed nets' first layers as ONE tensor-core product with both operands K-major,
         gcat[sum o][KA] = dz1T[sum o][M] hT[KA][M]^T (dz1T: the first-layer dz of the nets, stacked in `names` order, transposed by the
         dgrad epilogues that made it).  The augmented rows of hT make column K0 the bias gradient and columns K0 + 1.. the trailing-input
-        weight gradients of the critic (priv) and the actor (latent); they are copied into the flat gradient buffer (overwriting)."""
+        weight gradients of the critic (priv) and the actor (latent); they are copied into the flat gradient buffer (overwriting).
+        BF16 dz1T and hT (AC_Args.gemm_impl = 2): a BF16 product."""
         nets, K0, E = self._nets, self.num_obs_history, self.num_privileged_obs
         KA = hT.shape[0]
         KP = (KA + 31) // 32 * 32
         n0 = nets["adapt"]
         gcat = n0._buf((tag, "gWcat"), dz1T.shape[0], KP)
-        n0._gemm(0, 1, dz1T.shape[0], KA, M, dz1T, dz1T.stride(0), hT, hT.stride(0), gcat, KP, None, 0, 0, 1)
+        n0._gemm(0, 1, dz1T.shape[0], KA, M, dz1T, dz1T.stride(0), hT, hT.stride(0), gcat, KP, None, 0, 0, 1, bf16=dz1T.dtype == torch.bfloat16)
         row, pairs = 0, []
         for name in names:
             xcol = {"adapt": None, "actor": K0 + 1 + E, "critic": K0 + 1}[name]
@@ -732,12 +808,24 @@ class ActorCritic(nn.Module):
     def backward_ppo(self, h, priv, dmean, dvalue, dstd, hT=None):
         """Gradients of the PPO loss into flat_grads[HEAD:] (overwrites; the loss scalars in the head are left alone). h/priv are the
         minibatch inputs of the forward pass just run with tag='train'; dmean [M,A], dvalue [M,1], dstd [A].
-        hT: history_kmajor(h, priv) if the caller keeps one (RolloutStorage builds it once per update); built here otherwise.  Its latent
-        rows are written here."""
+        hT: history_kmajor(h, priv) if the caller keeps one (RolloutStorage builds it once per update; at AC_Args.gemm_impl = 2
+        history_kmajor_bf16 of the BF16 history); built here otherwise.  Its latent rows are written here."""
         M, K0 = h.shape[0], self.num_obs_history
         nets = self._nets
+        bf16 = self._impl() == 2
         self._grad[self.HEAD:].zero_()      # one fill; every kernel below adds into it (atomics in the epilogues and split-K products)
-        if self._first_layers_fusable(h, priv):
+        if self._first_layers_fusable(h, priv) and bf16:
+            # the BF16 history products: dz1 stored in BF16 by the layer-2 dgrads, the wgrad over the BF16 hT
+            oa, op, oc = nets["adapt"].specs[0][2], nets["actor"].specs[0][2], nets["critic"].specs[0][2]
+            E = self.num_privileged_obs
+            if hT is None:
+                hT = history_kmajor_bf16(self._model_input(h, "train"), priv, nets["adapt"]._buf16(("train", "hT16"), K0 + 1 + 2 * E, M))
+            capi.check(capi.lib().go1_transpose_to_bf16(capi.ptr(self._latent), self._latent.stride(0), capi.ptr(hT[K0 + 1 + E:]), hT.stride(0), M, E,
+                                                        capi.stream_ptr()), "transpose_to_bf16")
+            dz1 = nets["adapt"]._buf(("train", "dz1catT16"), oa + op + oc, M, hT.stride(0), torch.bfloat16)
+            self._backward_bodies(h, priv, dmean, dvalue, dz1, oa, op, M, K0)
+            self._first_layer_wgrad(("adapt", "actor", "critic"), dz1, hT, M, "train")
+        elif self._first_layers_fusable(h, priv):
             # the three first layers share their input: ONE transposed dz [o_a+o_p+o_c][M] (each net's layer-2 dgrad stores its
             # first-layer dz into its row slice) and ONE tensor-core wgrad with K-major operands (_first_layer_wgrad)
             oa, op, oc = nets["adapt"].specs[0][2], nets["actor"].specs[0][2], nets["critic"].specs[0][2]
@@ -747,28 +835,35 @@ class ActorCritic(nn.Module):
             L, st = capi.lib(), capi.stream_ptr()
             capi.check(L.go1_transpose(capi.ptr(self._latent), self._latent.stride(0), capi.ptr(hT[K0 + 1 + E:]), hT.stride(0), M, E, st), "transpose")
             dz1 = nets["adapt"]._buf(("train", "dz1catT"), oa + op + oc, hT.stride(0))
-            impl = 1
-            wgrads = []             # the tensor-core wgrads behind the first layers, launched as grouped products once all dz exist
-            side = self._side_stream(M)
-            if side is not None:    # critic chain beside actor -> adaptation chain
-                self._fork(side)
-                with torch.cuda.stream(side):
-                    nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, tag="train", dz1T=dz1[oa + op:], wgrads=wgrads)
-            dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, impl, want_dextra=True, tag="train", dz1T=dz1[oa:oa + op],
-                                          wgrads=wgrads)
-            if side is None:
-                nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, tag="train", dz1T=dz1[oa + op:], wgrads=wgrads)
-            nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, tag="train", dz1T=dz1[:oa], wgrads=wgrads)
-            if side is not None:
-                self._join(side)
-            self._flush_wgrads(wgrads)
+            self._backward_bodies(h, priv, dmean, dvalue, dz1, oa, op, M, K0)
             self._first_layer_wgrad(("adapt", "actor", "critic"), dz1, hT, M, "train")
         else:
             impl = self._impl()
+            if h.dtype == torch.bfloat16:      # (fewer than 64 rows: CUDA-core products, as at impl 1) the rounded history, exactly in fp32
+                h = h.float()
             dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, impl, want_dextra=True, tag="train")
             nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, tag="train")
             nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, tag="train")
         self._grad[self.std_offset:self.std_offset + self.num_actions].copy_(dstd)
+
+    def _backward_bodies(self, h, priv, dmean, dvalue, dz1, oa, op, M, K0):
+        """The three nets' backward passes down to their first-layer dz, stored transposed into the row slices of dz1 ([adapt | actor |
+        critic] x M), and the tensor-core wgrads behind the first layers, launched as grouped products once all dz exist."""
+        nets, impl = self._nets, 1
+        wgrads = []
+        side = self._side_stream(M)
+        if side is not None:    # critic chain beside actor -> adaptation chain
+            self._fork(side)
+            with torch.cuda.stream(side):
+                nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, tag="train", dz1T=dz1[oa + op:], wgrads=wgrads)
+        dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, impl, want_dextra=True, tag="train", dz1T=dz1[oa:oa + op],
+                                      wgrads=wgrads)
+        if side is None:
+            nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, tag="train", dz1T=dz1[oa + op:], wgrads=wgrads)
+        nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, tag="train", dz1T=dz1[:oa], wgrads=wgrads)
+        if side is not None:
+            self._join(side)
+        self._flush_wgrads(wgrads)
 
     def backward_adaptation(self, h, outs, dpred, hT=None):
         """Gradients of the adaptation module (overwrites its part of flat_grads, [HEAD:n_adapt_params]).  hT: history_kmajor(h, ..) if the
@@ -776,18 +871,26 @@ class ActorCritic(nn.Module):
         M, K0 = h.shape[0], self.num_obs_history
         net = self._nets["adapt"]
         self._grad[self.HEAD:self.n_adapt_params].zero_()
-        if self._impl() == 1 and M >= 64 and _Net._tma_ok(h, h.stride(0)) and net.specs[0][3] == K0:
-            if hT is None:
-                hT = history_kmajor(h, None, net._buf(("adapt", "hT"), K0 + 1, (M + 31) // 32 * 32))
+        if self._impl() >= 1 and M >= 64 and _Net._tma_ok(h, h.stride(0)) and net.specs[0][3] == K0:
             oa = net.specs[0][2]
-            dz1 = net._buf(("adapt", "dz1T"), oa, hT.stride(0))
+            if self._impl() == 2:
+                if hT is None:
+                    hT = history_kmajor_bf16(self._model_input(h, "adapt"), None, net._buf16(("adapt", "hT16"), K0 + 1, M))
+                dz1 = net._buf(("adapt", "dz1T16"), oa, M, hT.stride(0), torch.bfloat16)
+            else:
+                if hT is None:
+                    hT = history_kmajor(h, None, net._buf(("adapt", "hT"), K0 + 1, (M + 31) // 32 * 32))
+                dz1 = net._buf(("adapt", "dz1T"), oa, hT.stride(0))
             net.backward(h, h.stride(0), K0, None, outs, dpred, M, 1, tag="adapt", dz1T=dz1)
             self._first_layer_wgrad(("adapt",), dz1, hT[:K0 + 1], M, "adapt")
         else:
+            if h.dtype == torch.bfloat16:      # (fewer than 64 rows: CUDA-core products, as at impl 1) the rounded history, exactly in fp32
+                h = h.float()
             net.backward(h, h.stride(0), K0, None, outs, dpred, M, self._impl(), tag="adapt")
 
     def adaptation_forward(self, h):
         self.flatten()
+        h = self._model_input(h, "adapt")
         return self._nets["adapt"].forward(h, h.stride(0), self.num_obs_history, None, h.shape[0], self._impl(), "adapt")
 
 

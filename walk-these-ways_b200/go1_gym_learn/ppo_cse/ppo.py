@@ -167,6 +167,8 @@ class PPO:
         tr.observations, tr.privileged_observations = self.storage.snapshot_observations(obs, privileged_obs)
         tr.critic_observations = tr.observations
         tr.observation_histories = obs_history
+        if self.storage.hist_bf16:    # the BF16 slab stores what the policy evaluated
+            tr.history_bf16 = self.actor_critic.model_inputs.get("act")
         return tr.actions
 
     def process_env_step(self, rewards, dones, infos):
@@ -176,7 +178,7 @@ class PPO:
         f32 = lambda x: x.is_cuda and x.is_contiguous() and x.dtype == torch.float32
         h = tr.observation_histories
         fused = f32(rewards) and h.is_cuda and h.dtype == torch.float32 and self.storage.history_rows_fit(h) and f32(tr.env_bins) and f32(tr.values) and \
-            tr.env_bins.numel() == rewards.numel()
+            tr.env_bins.numel() == rewards.numel() and (not self.storage.hist_bf16 or tr.history_bf16 is not None)
         if fused:   # rewards += gamma * values * time_outs (ppo.py:84-86) happens inside the store kernel
             tr.rewards = rewards
             tr.action_sigma_vec = self.actor_critic.std.data

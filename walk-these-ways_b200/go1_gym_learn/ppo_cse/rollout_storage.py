@@ -3,7 +3,7 @@ GAE through the warp-scan kernel, minibatches through the row-gather kernel."""
 import torch
 
 from go1_b200 import capi
-from .actor_critic import history_kmajor
+from .actor_critic import AC_Args, history_kmajor, history_kmajor_bf16
 
 
 class RolloutStorage:
@@ -21,6 +21,7 @@ class RolloutStorage:
             self.action_mean = None
             self.action_sigma = None
             self.env_bins = None
+            self.history_bf16 = None      # AC_Args.gemm_impl = 2: the BF16 history the policy evaluated (ActorCritic.model_inputs["act"])
 
         def clear(self):
             self.__init__()
@@ -33,10 +34,12 @@ class RolloutStorage:
         z = lambda *s, **k: torch.zeros(T, N, *s, device=self.device, **k)
         self.observations = z(*obs_shape)
         self.privileged_observations = z(*privileged_obs_shape)
-        # the history slab [T][N][hist_row_pitch] (the pitch of HistoryWrapper's rows, capi.history_pitch) and its [T][N][K0] view
+        # the history slab [T][N][hist_row_pitch] (the pitch of HistoryWrapper's rows, capi.history_pitch) and its [T][N][K0] view.
+        # AC_Args.gemm_impl = 2: BF16 rows at capi.bf16_pitch (half the bytes), holding exactly the BF16 history the policy evaluated
         K0 = int(obs_history_shape[-1])
-        self.hist_row_pitch = capi.history_pitch(K0)
-        self._hist_slab = z(self.hist_row_pitch)
+        self.hist_bf16 = int(AC_Args.gemm_impl) == 2
+        self.hist_row_pitch = capi.bf16_pitch(K0) if self.hist_bf16 else capi.history_pitch(K0)
+        self._hist_slab = z(self.hist_row_pitch, dtype=torch.bfloat16) if self.hist_bf16 else z(self.hist_row_pitch)
         self.observation_histories = self._hist_slab[..., :K0]
         # Row pitch of the GATHERED minibatch histories: a multiple of 32 floats, so that every 128-byte row of a TMA box of the first-layer
         # products starts on a 128-byte line.  Measured (tools/epi_bench.py): the 24576 x 1280 x 2100 product runs in 180 us with a
@@ -92,7 +95,10 @@ class RolloutStorage:
 
     def history_rows_fit(self, h):
         """The fused transition store copies whole hist_row_pitch-wide rows: h [N][K0] qualifies if it is contiguous (pitch K0) or, for a
-        padded pitch, has exactly that row stride over storage that holds every full row (HistoryWrapper's buffers)."""
+        padded pitch, has exactly that row stride over storage that holds every full row (HistoryWrapper's buffers).  A BF16 slab takes
+        its rows from the policy's BF16 input instead (add_transitions_fused)."""
+        if self.hist_bf16:
+            return True
         P = self.hist_row_pitch
         if P == h.shape[-1]:
             return h.is_contiguous()
@@ -107,8 +113,11 @@ class RolloutStorage:
         u8 = lambda x: x if x.dtype == torch.uint8 else (x.view(torch.uint8) if x.dtype == torch.bool else x.to(torch.uint8))
         dones, touts = u8(tr.dones), (u8(time_outs) if time_outs is not None else None)
         stored = lambda x, slot: None if (x is None or x.data_ptr() == slot.data_ptr()) else x       # already snapshotted by act()
+        h16 = tr.history_bf16 if self.hist_bf16 else None
+        assert not self.hist_bf16 or (h16 is not None and h16.dtype == torch.bfloat16 and h16.shape[0] == self.num_envs), \
+            "a BF16 history slab stores the BF16 history the policy evaluated (PPO.act at AC_Args.gemm_impl = 2)"
         ins = [stored(tr.observations, self.observations[t]), stored(tr.privileged_observations, self.privileged_observations[t]),
-               tr.observation_histories, tr.actions, tr.rewards, tr.values, tr.actions_log_prob, tr.action_mean, tr.action_sigma_vec, tr.env_bins]
+               None if self.hist_bf16 else tr.observation_histories, tr.actions, tr.rewards, tr.values, tr.actions_log_prob, tr.action_mean, tr.action_sigma_vec, tr.env_bins]
         outs = [self.observations[t], self.privileged_observations[t], self.observation_histories[t], self.actions[t], self.rewards[t], self.values[t],
                 self.actions_log_prob[t], self.mu[t], self.sigma[t], self.env_bins[t]]
         for k, x in enumerate(ins):
@@ -120,6 +129,9 @@ class RolloutStorage:
         capi.check(capi.lib().go1_store_transition(arr_in, capi.ptr(dones), capi.ptr(touts), arr_out, capi.ptr(self.dones[t]), self.num_envs,
                                                    self.observations.shape[-1], self.privileged_observations.shape[-1], self.hist_row_pitch,
                                                    self.actions.shape[-1], float(gamma), capi.stream_ptr()), "go1_store_transition")
+        if h16 is not None:
+            capi.check(capi.lib().go1_rollout_store_rows_bf16(capi.ptr(h16), h16.stride(0), capi.ptr(self._hist_slab[t]), self.hist_row_pitch, None,
+                                                              self.num_envs, h16.shape[1], capi.stream_ptr()), "go1_rollout_store_rows_bf16")
         self.step += 1
 
     def clear(self):
@@ -168,21 +180,37 @@ class RolloutStorage:
         if indices is None:
             indices = torch.randperm(num_mini_batches * mini_batch_size, requires_grad=False, device=self.device)
         dones8 = None
+        bf16 = self.hist_bf16
+        if bf16 != (int(AC_Args.gemm_impl) == 2):
+            raise capi.Go1Error("RolloutStorage keeps its history slab in the precision of the AC_Args.gemm_impl it was built under: "
+                                "build the storage again (PPO.init_storage) after changing the mode")
         for epoch in range(num_epochs):
             for i in range(num_mini_batches):
                 idx = indices[i * mini_batch_size:(i + 1) * mini_batch_size].contiguous()
                 obs = self.gather(self.observations, idx)
                 priv_b = self.gather(self.privileged_observations, idx)
-                # whole slab rows: go1_gather_rows reads its source at a row pitch equal to the width it copies
-                hist_b = self.gather(self._hist_slab, idx, key=("hist", i), ldd=self.hist_pitch)[:, :self.observation_histories.shape[-1]]
-                # its K-major transpose [history | 1 | priv | latent rows] for the first layers' weight-gradient products, built once per
-                # update and read by every epoch (ActorCritic.backward_ppo / backward_adaptation); 830 MB for 4 minibatches at 4096 envs
-                M, w, P = hist_b.shape[0], hist_b.shape[1], priv_b.shape[1]
                 cache = self.__dict__.setdefault("_gather_bufs", {})
-                hT = cache.get(("histT", i))
-                if hT is None or hT.shape != (w + 1 + 2 * P, (M + 31) // 32 * 32):
-                    hT = cache[("histT", i)] = torch.empty(w + 1 + 2 * P, (M + 31) // 32 * 32, device=hist_b.device)
-                hist_b.hT = history_kmajor(hist_b, priv_b, hT)
+                K0, P = self.observation_histories.shape[-1], priv_b.shape[1]
+                if bf16:    # AC_Args.gemm_impl = 2: the minibatch history (copied from the BF16 slab) and its K-major copy in BF16
+                    M = idx.shape[0]
+                    shapes = {("hist16", i): (M, capi.bf16_pitch(K0)), ("histT16", i): (K0 + 1 + 2 * P, capi.bf16_pitch(M))}
+                    for k, shp in shapes.items():
+                        if k not in cache or cache[k].shape != shp:
+                            cache[k] = torch.empty(*shp, device=self.device, dtype=torch.bfloat16)
+                    hist_b = cache[("hist16", i)][:, :K0]
+                    capi.check(capi.lib().go1_gather_rows_bf16(capi.ptr(self._hist_slab), self.hist_row_pitch, capi.ptr(idx), capi.ptr(hist_b),
+                                                               hist_b.stride(0), M, K0, capi.stream_ptr()), "gather_rows_bf16")
+                    hist_b.hT = history_kmajor_bf16(hist_b, priv_b, cache[("histT16", i)])
+                else:
+                    # whole slab rows: go1_gather_rows reads its source at a row pitch equal to the width it copies
+                    hist_b = self.gather(self._hist_slab, idx, key=("hist", i), ldd=self.hist_pitch)[:, :K0]
+                    # its K-major transpose [history | 1 | priv | latent rows] for the first layers' weight-gradient products, built once per
+                    # update and read by every epoch (ActorCritic.backward_ppo / backward_adaptation); 830 MB for 4 minibatches at 4096 envs
+                    M = hist_b.shape[0]
+                    hT = cache.get(("histT", i))
+                    if hT is None or hT.shape != (K0 + 1 + 2 * P, (M + 31) // 32 * 32):
+                        hT = cache[("histT", i)] = torch.empty(K0 + 1 + 2 * P, (M + 31) // 32 * 32, device=hist_b.device)
+                    hist_b.hT = history_kmajor(hist_b, priv_b, hT)
                 yield (obs, obs, priv_b, hist_b,
                        self.gather(self.actions, idx), self.gather(self.values, idx), self.gather(self.advantages, idx),
                        self.gather(self.returns, idx), self.gather(self.actions_log_prob, idx), self.gather(self.mu, idx),

@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """Learning-level evidence for the TF32 path (VERDICT r1, weak #2): trains scripts/train.py's configuration for K iterations
-with the tcgen05 TF32 GEMMs (AC_Args.gemm_impl = 1) and with the exact-fp32 CUDA-core GEMMs (impl 0) from the same seeds and
+with the tcgen05 TF32 GEMMs (AC_Args.gemm_impl = 1) and with the exact-fp32 CUDA-core GEMMs (impl 0) -- or, with --impls 1,2, the
+BF16 history products (impl 2) -- from the same seeds and
 writes the reward-term trajectories (one record per `log_freq` iterations, like the reference's metrics.pkl) next to the first
 records of the shipped training log (tests/golden/metrics_envelope.json: Isaac Gym, 4000 envs).
     python walk-these-ways_b200/tools/train_compare.py --iterations 200 --out train_compare.json"""
@@ -20,6 +21,9 @@ KEYS = ["train/episode/rew_total/mean", "train/episode/rew_tracking_lin_vel/mean
         "train/episode/rew_tracking_contacts_shaped_force/mean", "train/episode/rew_tracking_contacts_shaped_vel/mean",
         "train/episode/rew_collision/mean", "train/episode/rew_action_rate/mean", "train/episode/rew_torques/mean",
         "train/episode/command_area_trot/mean", "adaptation_loss/mean", "mean_value_loss/mean", "mean_surrogate_loss/mean", "iterations"]
+
+
+NAMES = {0: "fp32", 1: "tf32", 2: "bf16"}
 
 
 def run(impl, iterations, envs, tag):
@@ -48,12 +52,12 @@ if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--iterations", type=int, default=200)
     ap.add_argument("--envs", type=int, default=4096)
-    ap.add_argument("--impls", default="1,0")
+    ap.add_argument("--impls", default="1,0", help="comma-separated AC_Args.gemm_impl values: 0 fp32, 1 tf32, 2 bf16")
     ap.add_argument("--out", default=os.path.join(tempfile.gettempdir(), "go1_train_compare.json"))
     a = ap.parse_args()
     res = {"iterations": a.iterations, "envs": a.envs}
     for impl in [int(x) for x in a.impls.split(",")]:
-        res["tf32" if impl == 1 else "fp32"] = run(impl, a.iterations, a.envs, f"impl{impl}")
+        res[NAMES[impl]] = run(impl, a.iterations, a.envs, f"impl{impl}")
     with open(os.path.join(ROOT, "tests", "golden", "metrics_envelope.json")) as f:
         env = json.load(f)
     n = a.iterations // 10 + 1
@@ -61,7 +65,7 @@ if __name__ == "__main__":
     os.makedirs(os.path.dirname(a.out), exist_ok=True)
     with open(a.out, "w") as f:
         json.dump(res, f)
-    for name in ("tf32", "fp32", "reference_isaacgym_4000_envs"):
+    for name in ("tf32", "fp32", "bf16", "reference_isaacgym_4000_envs"):
         if name in res:
             r = res[name]
             print(name, "rew_total", [None if x is None else round(x, 3) for x in r["train/episode/rew_total/mean"][::4]],
