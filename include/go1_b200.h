@@ -370,6 +370,26 @@ int go1_gather_rows_bf16(const uint16_t* src, int lds, const int64_t* idx, uint1
 int go1_rollout_store_rows_bf16(const uint16_t* src, int lds, uint16_t* dst_base, int ldd, const int32_t* slot_dev, int rows, int cols, void* stream);
 int go1_transpose_to_bf16(const float* src, int lds, uint16_t* dst, int ldd, int rows, int cols, void* stream);
 int go1_transpose_bf16(const uint16_t* src, int lds, uint16_t* dst, int ldd, int rows, int cols, void* stream);
+/* Up to 16 go1_convert_bf16 copies in ONE launch, dst[r][c] = bf16(src[r][c]) per segment: the BF16 copies of the hidden-layer outputs that
+ * the weight gradients of AC_Args.bf16_backward read and of the hidden weights its dgrads read, made once per minibatch forward.  A bad segment returns non-zero before any launch. */
+typedef struct Go1Bf16Seg { const float* src; int32_t lds; uint16_t* dst; int32_t ldd; int32_t rows, cols; } Go1Bf16Seg;
+int go1_convert_bf16_segments(const Go1Bf16Seg* segs, int n, void* stream);
+/* go1_gemm_bf16_ex with BF16 operands in EITHER major (transA / transB as go1_gemm), read in place: an MN-major operand ([K][M] A, [K][N] B,
+ * the dgrad's W and both operands of a weight gradient) reaches the tensor core as 128B-swizzled TMA boxes through the transpose immediates
+ * of BF16 wgmma, without the shared-to-shared transposition of the TF32 kernel.  The full Go1GemmEpilogue, out_bf16 included.
+ *   c_bf16 = 0: C is fp32 [M][N] (row stride ldc floats), as go1_gemm_bf16_ex.
+ *   c_bf16 = 1: C is a row-major BF16 matrix (uint16_t*, ldc elements, a multiple of 8, >= N, 16-byte aligned): every value is rounded once
+ *               to nearest even after all fp32 terms (the column sums and trailing-input terms see fp32 values, as with out_bf16).  Whole
+ *               16-byte chunks are written: when N % 8 != 0, row padding columns N .. (N rounded up to 8) - 1 may be overwritten.  Not
+ *               with accumulate, store_transposed or out_bf16.
+ * A / B 16-byte aligned with lda / ldb multiples of 8 elements (TMA); anything else returns non-zero before any launch.  Used by the
+ * hidden-layer dgrads and weight gradients of AC_Args.bf16_backward. */
+int go1_gemm_bf16_mn(int transA, int transB, int M, int N, int K, const uint16_t* A, int lda, const uint16_t* B, int ldb,
+                     void* C, int ldc, int c_bf16, const Go1GemmEpilogue* ep, void* stream);
+/* go1_gemm_grouped with BF16 operands in either major (go1_gemm_bf16_mn's kernels, fp32 C): the equal-shape weight gradients of
+ * AC_Args.bf16_backward in one grid. */
+int go1_gemm_bf16_grouped(int transA, int transB, int M, int N, int K, int nprob, const uint16_t* const* A, int lda, const uint16_t* const* B, int ldb,
+                          float* const* C, int ldc, int accumulate, void* stream);
 /* nprob (<= 4) wgmma products of the SAME shape and operand strides in one grid: C[p] (+)= op(A[p]) op(B[p]) (impl 1 only, no fused
  * epilogue operands).  Used for the equal-shape split-K wgrads of the three MLPs (nn.Linear weight gradients, actor_critic.py:38-77). */
 int go1_gemm_grouped(int transA, int transB, int M, int N, int K, int nprob, const float* const* A, int lda, const float* const* B, int ldb,
@@ -434,6 +454,10 @@ int go1_skinny_dgrad_ex(const float* dz, int lddz, const float* W, int ldw, cons
 /* go1_skinny_dgrad_ex with the derivative of any Go1Activation in place of ELU'. */
 int go1_skinny_dgrad_act(const float* dz, int lddz, const float* W, int ldw, const float* y_prev, int ldy, float* dprev, int lddp,
                          float* colsum, int M, int o, int n, int kind, void* stream);
+/* go1_skinny_dgrad_act whose dprev is BF16 (uint16_t, lddp elements), each value rounded once to nearest even after the fp32 column sum:
+ * the head dgrad of AC_Args.bf16_backward.  n, ldw, lddp and ldy multiples of 4, W / y_prev 16-byte and dprev 8-byte aligned. */
+int go1_skinny_dgrad_act_bf16(const float* dz, int lddz, const float* W, int ldw, const float* y_prev, int ldy, uint16_t* dprev, int lddp,
+                              float* colsum, int M, int o, int n, int kind, void* stream);
 /* go1_skinny_wgrad + the layer's bias gradient gb[j] (+)= sum_m dz[m][j] (may be NULL; needs K % 4 == 0 and 16-byte aligned x rows). */
 int go1_skinny_wgrad_ex(const float* dz, int lddz, const float* x, int ldx, float* gW, int ldg, float* gb, int M, int o, int K, int accumulate, void* stream);
 /* wgrad of a narrow (o <= 16) output layer (the 12 / 2 / 1-wide heads): gW[j][k] (+)= sum_m dz[m][j] x[m][k]. */

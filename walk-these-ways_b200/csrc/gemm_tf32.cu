@@ -11,7 +11,8 @@
 // wgrads, the first layers' (1280 x 2105 and 256 x 2101 over M = 24576), read K-major copies instead: the history transposed once
 // per update (go1_transpose, [2105][24576] per minibatch: 207 MB each, 830 MB for the four minibatches at 4096 envs) and dz stored
 // transposed by the dgrad epilogue that produces it (store_transposed).  On an H100 SXM (700 W): 1299 -> 565 us and
-// 206 -> 137 us per launch.  The dgrads' W and the layer-2/3 wgrads are still transposed on the SM.
+// 206 -> 137 us per launch.  The dgrads' W and the layer-2/3 wgrads are still transposed on the SM in TF32; with BF16 operands
+// (gemm_bf16_mn_wgmma, AC_Args.bf16_backward) they are read in place as 128B-swizzled MN-major boxes through wgmma's transpose immediates.
 // Structure (persistent CTAs, one per SM, 384 threads, walking 128 x BN output tiles):
 //   warps 0-7   two consumer warpgroups, 64 rows x BN columns each: wgmma.mma_async m64nBNk8 (4 per k-block) with the accumulator
 //               in registers, then the epilogue: accumulator -> swizzled shared memory -> one 32 x 32 block per warp at a time,
@@ -167,6 +168,10 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void*
                  ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
 }
 
+__device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
+    return (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(lo)) | ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(hi)) << 16);
+}
+
 // act == 2 of one chunk: v[j] *= f'(z) from the saved activation, wherever this chunk's 32 values of it are (see epilogue_chunk)
 template <typename D>
 __device__ __forceinline__ void epilogue_dact(const D dact, const GemmArgs& g, float (&v)[32], const int row, const int col0, const int ncols, const int lane,
@@ -216,7 +221,7 @@ __device__ __forceinline__ float transpose_reduce32(float (&sred)[32], const int
 // Epilogue of one 32-column chunk held in registers (thread = output row, r[j] = column col0 + j).  Called by all 32 lanes
 // of an epilogue warp (the per-column operands -- bias, extra-input weights -- are loaded once per lane and broadcast
 // with shuffles instead of 32 x per-thread global loads, which made the rank-2 term the slowest part of the kernel).
-template <bool ANYKIND>
+template <bool ANYKIND, bool ROW16 = false>
 __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const Cbase, uint32_t (&r)[32], const int row, const int col0, const bool split, const int lane,
                                                const float4 (&ypre)[8], const bool have_pre, const EpiStage& es) {
     if (col0 >= g.N) return;                                    // warp-uniform
@@ -320,6 +325,30 @@ __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const C
             }
         }
     }
+    if (ROW16 && g.c16 && !g.ct) {      // row-major BF16 C (C is then a uint16_t matrix with row stride ldc elements): rounded after every term above
+        if (es.out) {       // the block as 32 rows of 64 bytes, 64B-swizzled (chunk j of row l at j ^ ((l / 2) % 4): conflict-free), one TMA store
+            __syncwarp();   // (it overlays the fp32 rows of the block: every lane has read its row)
+            uint8_t* srow = es.out + lane * 64;
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                uint4 o;
+                o.x = pack_bf16x2(v[8 * j], v[8 * j + 1]); o.y = pack_bf16x2(v[8 * j + 2], v[8 * j + 3]);
+                o.z = pack_bf16x2(v[8 * j + 4], v[8 * j + 5]); o.w = pack_bf16x2(v[8 * j + 6], v[8 * j + 7]);
+                *reinterpret_cast<uint4*>(srow + ((j ^ ((lane >> 1) & 3)) << 4)) = o;
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            __syncwarp();
+            if (lane == 0) {
+                tma_store_2d(es.mapC, es.out, col0, row);
+                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+            }
+        } else if (row_ok) {
+            uint16_t* c16 = reinterpret_cast<uint16_t*>(Cbase) + (size_t)row * g.ldc + col0;
+#pragma unroll
+            for (int j = 0; j < 32; j++) if (j < ncols) c16[j] = __bfloat16_as_ushort(__float2bfloat16_rn(v[j]));
+        }
+        return;
+    }
     if (es.out) {           // warp-uniform: all 32 lanes stage their row (rows / columns beyond M / N are clipped by the TMA store)
         if (g.ct && g.c16) {    // BF16 block of C^T, unswizzled 64-byte rows: store j writes row j, 32 lanes x 2 consecutive bytes (conflict-free)
             __syncwarp();
@@ -380,12 +409,15 @@ __device__ __forceinline__ bool epilogue_prefetch(const GemmArgs& g, const int r
 // ---------------------------------------------------------------------------------------------------------------
 // BF16 = true: the operands are BF16 (K-major only), a k-block is 64 of them (the same 128-byte rows, boxes, ring and multicast as 32
 // floats) and the tensor core runs m64nBNk16 BF16 instructions; the epilogue is the same fp32 code.
+// BF16 with AMN / BMN (gemm_bf16_mn_wgmma, go1_gemm_bf16_mn): an MN-major operand arrives as [64 k][64 mn] boxes, 128B-swizzled (BN = 32:
+// one [64 k][32 n] box, 64B-swizzled), two boxes per 128-wide tile 8 KB apart, and the tensor core reads them in place through its
+// transpose immediates: no shared-to-shared transposition.  ROW16: the epilogue can also store C row-major in BF16 (c16 without ct).
 constexpr int X_BYTES = 65536;
-template <int BN, bool ANYKIND, int CL, bool BF16>
-__global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __grid_constant__ GemmMaps gm,
-                                                                      const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
-                                                                      const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
+template <int BN, bool ANYKIND, int CL, bool BF16, int AMN, int BMN, bool ROW16>
+__device__ __forceinline__ void gemm_wgmma_body(const GemmMaps& gm, const CUtensorMap& mapC, const CUtensorMap& mapY, const GemmArgs& g,
+                                                const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
     static_assert(CL == 1 || (CL == 2 && BN == BM), "CTA pairs share 128-row operand boxes");
+    static_assert((AMN == 0 && BMN == 0 && !ROW16) || (BF16 && CL == 1), "MN-major BF16 operands and the row-major BF16 store: one CTA per tile");
     constexpr int G = EPI_G;
     constexpr int A_BYTES = BM * BK * 4, STAGE_BYTES = (BM + BN) * BK * 4;
     constexpr int MAX_STAGES = 8;
@@ -462,6 +494,14 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
                             tma_load_2d(mapA, &full[s], a, kc, m0);
                             tma_load_2d_multicast(&gm.half, &full[s], b + rank() * (A_BYTES / 2), kc, n0 + (int)rank() * (BN / 2), 0x3);
                         }
+                    } else if (AMN || BMN) {        // BF16: MN-major operands as 64-wide boxes (see above)
+                        const int kc = (kb0 + i) * KE;
+                        if (AMN) { tma_load_2d(mapA, &full[s], a, m0, kc); tma_load_2d(mapA, &full[s], a + A_BYTES / 2, m0 + BM / 2, kc); }
+                        else tma_load_2d(mapA, &full[s], a, kc, m0);
+                        if (BMN) {
+                            tma_load_2d(mapB, &full[s], b, n0, kc);
+                            if (BN == 128) tma_load_2d(mapB, &full[s], b + A_BYTES / 2, n0 + 64, kc);
+                        } else tma_load_2d(mapB, &full[s], b, kc, n0);
                     } else {
                         if (g.amn) tma_load_2d(mapA, &full[s], a, m0, (kb0 + i) * KE);        // box [32 k-rows][128 m]
                         else tma_load_2d(mapA, &full[s], a, (kb0 + i) * KE, m0);              // box [128 m-rows][32 k]
@@ -539,7 +579,13 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
                 cons_sync();
             }
             wg::fence();
-            wg::mma_kblock<BN, BF16>(acc, a + (size_t)wgi * 64 * 128, b, i > 0);
+            if constexpr (AMN || BMN) {
+                const uint64_t da = AMN ? wg::desc_mn128(a + (size_t)wgi * 64 * 128, 8192) : wg::desc(a + (size_t)wgi * 64 * 128);
+                const uint64_t db = BMN ? (BN == 32 ? wg::desc_mn64(b) : wg::desc_mn128(b, 8192)) : wg::desc(b);
+                wg::mma_kblock_bf16<BN, AMN, BMN>(acc, da, db, i > 0);
+            } else {
+                wg::mma_kblock<BN, BF16>(acc, a + (size_t)wgi * 64 * 128, b, i > 0);
+            }
             wg::commit();
             if (!tr && prev >= 0) {
                 wg::wait<1>();
@@ -572,12 +618,26 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __g
             EpiStage es;
             es.out = st_out ? blk : nullptr; es.mapC = &mapC; es.aux = st_aux ? my_aux : nullptr;
             if (st_aux) { mbar_wait(my_bar, aux_phase); aux_phase ^= 1; }
-            epilogue_chunk<ANYKIND>(g, Cbase, r, row, n0 + 32 * c, split, lane, ypre, have_pre && c == grp, es);
+            epilogue_chunk<ANYKIND, ROW16>(g, Cbase, r, row, n0 + 32 * c, split, lane, ypre, have_pre && c == grp, es);
             if (st_aux) { __syncwarp(); request_aux(); }             // every lane has read the operand block: fetch the next one into it
         }
     }
     if (st_out && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");      // all stores of this warp have completed
     if (CL > 1) cluster_sync();
+}
+
+template <int BN, bool ANYKIND, int CL, bool BF16>
+__global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __grid_constant__ GemmMaps gm,
+                                                                      const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
+                                                                      const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
+    gemm_wgmma_body<BN, ANYKIND, CL, BF16, 0, 0, false>(gm, mapC, mapY, g, tiles_m, tiles_n, total_tiles, stages);
+}
+// BF16 operands in the majors AMN / BMN (1: MN-major), fp32 or row-major BF16 output (go1_gemm_bf16_mn / go1_gemm_bf16_grouped)
+template <int BN, bool ANYKIND, int AMN, int BMN>
+__global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_bf16_mn_wgmma(const __grid_constant__ GemmMaps gm,
+                                                                         const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
+                                                                         const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
+    gemm_wgmma_body<BN, ANYKIND, 1, true, AMN, BMN, true>(gm, mapC, mapY, g, tiles_m, tiles_n, total_tiles, stages);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -667,7 +727,8 @@ __global__ void bias_act_strided(float* C, int ldc, const float* bias, int M, in
     *c = v;
 }
 
-template <int BN, bool ANYKIND, int CL, bool BF16>
+// MN < 0: gemm_tf32_wgmma<BN, ANYKIND, CL, BF16>; MN = 0..3: gemm_bf16_mn_wgmma<BN, ANYKIND, MN & 1, MN >> 1> (CL 1, BF16)
+template <int BN, bool ANYKIND, int CL, bool BF16, int MN = -1>
 int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st) {
     constexpr int STAGE_BYTES = (BM + BN) * BK * 4;
     const size_t staging = X_BYTES + (g.tma_aux ? (size_t)NCONS * 4096 : 0);
@@ -677,7 +738,11 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
     if (stages > 8) stages = 8;
     if (stages < 2) return go1_set_error("go1_gemm impl=1: no room for the operand ring");
     const size_t smem = (size_t)stages * STAGE_BYTES + fixed;
-    auto kernel = gemm_tf32_wgmma<BN, ANYKIND, CL, BF16>;
+    static_assert(MN < 0 || (CL == 1 && BF16), "the MN-major BF16 kernel runs one CTA per tile");
+    auto kernel = [] {
+        if constexpr (MN < 0) return gemm_tf32_wgmma<BN, ANYKIND, CL, BF16>;
+        else return gemm_bf16_mn_wgmma<BN, ANYKIND, (MN & 1), (MN >> 1)>;
+    }();
     const int tiles_m = (g.M + BM - 1) / BM, tiles_n = (g.N + BN - 1) / BN;
     g.tiles_per_prob = tiles_m * tiles_n * splits;
     const int total = g.tiles_per_prob * (g.nprob > 1 ? g.nprob : 1);
@@ -1064,11 +1129,23 @@ extern "C" int go1_gemm_timing(int on, double* total_ms, double* total_flop, lon
     return 0;
 }
 
-// T = float: TF32 products (operands in either major); T = uint16_t: BF16 products (K-major operands only, go1_gemm_bf16_ex).  One code path
-// for both: only the operand maps, the k-block width and the tensor-core instruction differ.
+// the MN-major BF16 kernel of layout mn (bit 0: A MN-major, bit 1: B MN-major)
+template <int BN, bool ANYKIND>
+int launch_gemm_mn(int mn, const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st) {
+    switch (mn) {
+        case 0: return launch_gemm<BN, ANYKIND, 1, true, 0>(gm, mc, my, g, splits, st);
+        case 1: return launch_gemm<BN, ANYKIND, 1, true, 1>(gm, mc, my, g, splits, st);
+        case 2: return launch_gemm<BN, ANYKIND, 1, true, 2>(gm, mc, my, g, splits, st);
+        default: return launch_gemm<BN, ANYKIND, 1, true, 3>(gm, mc, my, g, splits, st);
+    }
+}
+
+// T = float: TF32 products (operands in either major); T = uint16_t: BF16 products, K-major operands only (go1_gemm_bf16_ex), or with
+// mn (go1_gemm_bf16_mn / go1_gemm_bf16_grouped) in either major, read in place, and with row16 a row-major BF16 C (Cs[0] is then a
+// uint16_t matrix, ldc in elements).  One code path for all: only the operand maps, the k-block width and the tensor-core instruction differ.
 template <typename T>
 static int gemm_wgmma_impl(int transA, int transB, int M, int N, int K, int nprob, const T* const* As, int lda, const T* const* Bs, int ldb,
-                           float* const* Cs, int ldc, const Go1GemmEpilogue* ep, cudaStream_t st) {
+                           float* const* Cs, int ldc, const Go1GemmEpilogue* ep, cudaStream_t st, bool mn = false, bool row16 = false) {
     constexpr bool BF16 = sizeof(T) == 2;
     constexpr int ES = sizeof(T), KE = 128 / ES;      // operand element size, operand elements per k-block (one 128-byte row)
     float* Cm = Cs[0];
@@ -1076,13 +1153,16 @@ static int gemm_wgmma_impl(int transA, int transB, int M, int N, int K, int npro
     if (act < 0 || act > 2) return go1_set_error("go1_gemm_ex: act must be 0, 1 or 2");
     if (!go1_act_kind_ok(ep->act_kind)) return go1_set_error("go1_gemm_ex: unknown activation kind (Go1Activation)");
     const int amn = transA ? 1 : 0, bmn = transB ? 0 : 1;     // A given as [K][M] / B given as [K][N]: MN-major operands
-    if (BF16 && (amn || bmn)) return go1_set_error("go1_gemm_bf16_ex: both operands must be K-major (transA = 0, transB = 1)");
+    if (BF16 && !mn && (amn || bmn)) return go1_set_error("go1_gemm_bf16_ex: both operands must be K-major (transA = 0, transB = 1)");
     const bool c16 = ep->out_bf16 != nullptr;
+    if (row16 && (c16 || ep->store_transposed || accumulate || nprob != 1 || (ldc & 7) || ldc < N || (((uintptr_t)Cm) & 15)))
+        return go1_set_error("go1_gemm_bf16_mn: c_bf16 needs a 16-byte aligned C with ldc >= N, a multiple of 8, no accumulate, no store_transposed and no out_bf16");
     if (c16 && (!ep->store_transposed || (ep->ld_out_bf16 & 7) || ep->ld_out_bf16 < M || (((uintptr_t)ep->out_bf16) & 15)))
         return go1_set_error("go1_gemm_ex: out_bf16 needs store_transposed, a 16-byte aligned output and ld_out_bf16 >= M, a multiple of 8");
     for (int p = 0; p < nprob; p++)
         if (((lda * ES) & 15) || ((ldb * ES) & 15) || (((uintptr_t)As[p] | (uintptr_t)Bs[p]) & 15) || (!Cs[p] && !c16))
-            return go1_set_error(BF16 ? "go1_gemm_bf16_ex: A/B must be 16-byte aligned with row strides that are multiples of 8 elements (TMA)"
+            return go1_set_error(BF16 ? (mn ? "go1_gemm_bf16_mn: A/B must be 16-byte aligned with row strides that are multiples of 8 elements (TMA)"
+                                            : "go1_gemm_bf16_ex: A/B must be 16-byte aligned with row strides that are multiples of 8 elements (TMA)")
                                       : "go1_gemm impl=1: A/B must be 16-byte aligned with row strides that are multiples of 4 floats (TMA)");
     GemmArgs g;
     g.nprob = nprob; g.tiles_per_prob = 0;
@@ -1090,7 +1170,7 @@ static int gemm_wgmma_impl(int transA, int transB, int M, int N, int K, int npro
     g.C = Cm; g.bias = bias; g.M = M; g.N = N; g.K = K; g.ldc = ldc; g.act = act; g.kind = ep->act_kind; g.accumulate = accumulate;
     g.ex = ep->extra; g.ldex = ep->ld_extra; g.wex = ep->w_extra; g.ldwex = ep->ld_w_extra; g.nex = ep->extra ? ep->num_extra : 0;
     g.aux = ep->dact_y; g.ldaux = ep->ld_dact_y;
-    g.amn = amn; g.bmn = bmn; g.lead = ep->lead_cols; g.colsum = ep->colsum; g.ct = ep->store_transposed ? 1 : 0; g.c16 = c16 ? 1 : 0;
+    g.amn = amn; g.bmn = bmn; g.lead = ep->lead_cols; g.colsum = ep->colsum; g.ct = ep->store_transposed ? 1 : 0; g.c16 = (c16 || row16) ? 1 : 0;
     g.nbx = ep->num_bwd_extra; g.bx = ep->bwd_extra; g.bwx = ep->bwd_w_extra; g.gwx = ep->g_w_extra; g.dx = ep->d_extra;
     g.ldbx = ep->ld_bwd_extra; g.ldbwx = ep->ld_bwd_w_extra; g.ldgwx = ep->ld_g_w_extra; g.lddx = ep->ld_d_extra;
     if (g.nbx < 0 || g.nbx > 4 || (g.nbx > 0 && ((g.gwx && !g.bx) || (!g.gwx && !g.dx) || (g.dx && !g.bwx)))) return go1_set_error("go1_gemm_ex: bad fused trailing-input backward arguments");
@@ -1104,22 +1184,29 @@ static int gemm_wgmma_impl(int transA, int transB, int M, int N, int K, int npro
     constexpr int SPLIT_MIN_KB = 16;          // least k-blocks per split
     const int BN = (N > 64) ? 128 : (N > 32 ? 64 : 32);
     const int tiles = ((M + BM - 1) / BM) * ((N + BN - 1) / BN) * nprob;
-    const bool plain = g.nex == 0 && act != 2 && g.lead <= 0 && !g.colsum && g.nbx == 0 && !g.ct;
+    const bool plain = g.nex == 0 && act != 2 && g.lead <= 0 && !g.colsum && g.nbx == 0 && !g.ct && !row16;
     const int splits = plain ? split_count(tiles, num_kb, SPLIT_MIN_KB, sm_count()) : 1;
     g.kb_per_split = (num_kb + splits - 1) / splits;
     GemmMaps gm;
-    // K-major: rows = M (or N), cols = K, box BK x tile rows.  MN-major: rows = K, cols = M (or N), box tile width x BK k-rows.
+    // K-major: rows = M (or N), cols = K, box BK x tile rows.  MN-major: rows = K, cols = M (or N), box tile width x BK k-rows; BF16:
+    // 64 k-rows x 64 mn, 128B-swizzled (BN = 32: 64 k-rows x 32 n, 64B-swizzled), read in place by the tensor core.
     for (int p = 0; p < nprob; p++) {
-        if (int e = amn ? make_map_mn(&gm.a[p], (const float*)As[p], K, M, lda, BM) : make_map(&gm.a[p], As[p], M, K, lda, BM, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES)) return e;
-        if (int e = bmn ? make_map_mn(&gm.b[p], (const float*)Bs[p], K, N, ldb, BN) : make_map(&gm.b[p], Bs[p], N, K, ldb, BN, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES)) return e;
+        int e = 0;
+        if (BF16 && amn) e = make_map(&gm.a[p], As[p], K, M, lda, KE, BM / 2, CU_TENSOR_MAP_SWIZZLE_128B, ES);
+        else e = amn ? make_map_mn(&gm.a[p], (const float*)As[p], K, M, lda, BM) : make_map(&gm.a[p], As[p], M, K, lda, BM, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES);
+        if (e) return e;
+        if (BF16 && bmn) e = make_map(&gm.b[p], Bs[p], K, N, ldb, KE, BN == 32 ? 32 : 64, BN == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B, ES);
+        else e = bmn ? make_map_mn(&gm.b[p], (const float*)Bs[p], K, N, ldb, BN) : make_map(&gm.b[p], Bs[p], N, K, ldb, BN, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES);
+        if (e) return e;
     }
+    const int mnk = BF16 && (amn || bmn || row16) ? (amn | (bmn << 1)) : -1;      // >= 0: gemm_bf16_mn_wgmma of that layout
     for (int p = nprob; p < GEMM_MAXP; p++) { gm.a[p] = gm.a[0]; gm.b[p] = gm.b[0]; }
     const CUtensorMap& ma = gm.a[0];
     // CTA pairs (cluster of 2) share one operand box of every k-block by multicast: K-major operands, one problem, 128 x 128 tiles and an
     // even tile count along N (pairs share A) or else along M (pairs share B).  Same tiles, instructions and order of the sums as one CTA.
     // No derivative operand (act 2, the dgrads, whose W is MN-major anyway): without its prefetch registers the pair kernels spill less.
     const int tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN;
-    const int cluster = (!amn && !bmn && nprob == 1 && act != 2 && BN == 128 && (tiles_n % 2 == 0 || tiles_m % 2 == 0)) ? 2 : 1;
+    const int cluster = (mnk < 0 && !amn && !bmn && nprob == 1 && act != 2 && BN == 128 && (tiles_n % 2 == 0 || tiles_m % 2 == 0)) ? 2 : 1;
     gm.half = ma;
     if (cluster == 2) {
         if (int e = tiles_n % 2 == 0 ? make_map(&gm.half, As[0], M, K, lda, BM / 2, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES)
@@ -1134,14 +1221,19 @@ static int gemm_wgmma_impl(int transA, int transB, int M, int N, int K, int npro
     const bool timed = g_time_on && cudaStreamIsCapturing(st, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone;
     if (timed) {
         cudaEventRecord(timing_event(), st); g_time_flop += 2.0 * (double)M * (double)N * (double)K * nprob;
-        g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, BN, g.colsum ? 1 : 0, cluster, 0, 0, nprob, BF16 ? 1 : 0});
+        g_time_recs.push_back({M * nprob, N, K, amn, bmn, act, g.nex, splits, BN, g.colsum ? 1 : 0, cluster, 0, 0, nprob, BF16 ? (mn ? 2 : 1) : 0});
     }
     int e;
     // staged epilogue: C blocks leave the accumulator staging by TMA store, the derivative operand arrives through TMA loads.  The direct
     // row-per-lane stores serve the rest: split-K partial tiles, accumulate, grouped launches, N < 32 and a misaligned C.
     CUtensorMap mc = ma, my = ma;
     g.tma_store = g.tma_aux = 0;
-    if (c16) {          // (a BF16 transposed store: checked above) 32 x 32 blocks of 64-byte rows, unswizzled
+    if (row16) {        // row-major BF16 C: 32 x 32 blocks of 64-byte rows, 64B-swizzled (N < 32: direct stores)
+        if (N >= 32) {
+            if (int e2 = make_map(&mc, Cm, M, N, ldc, 32, 32, CU_TENSOR_MAP_SWIZZLE_64B, 2)) return e2;
+            g.tma_store = 1;
+        }
+    } else if (c16) {   // (a BF16 transposed store: checked above) 32 x 32 blocks of 64-byte rows, unswizzled
         if (int e2 = make_map(&mc, ep->out_bf16, N, M, ep->ld_out_bf16, 32, 32, CU_TENSOR_MAP_SWIZZLE_NONE, 2)) return e2;
         g.tma_store = 1;
     } else if (nprob == 1 && splits == 1 && !accumulate && (g.ct ? M : N) >= 32 && (ldc & 3) == 0 && (((uintptr_t)Cm) & 15) == 0) {
@@ -1155,7 +1247,11 @@ static int gemm_wgmma_impl(int transA, int transB, int M, int N, int K, int npro
         }
     }
     const bool any = g.act != 0 && g.kind != GO1_ACT_ELU;
-    if (cluster == 2) e = any ? launch_gemm<128, true, 2, BF16>(gm, mc, my, g, splits, st) : launch_gemm<128, false, 2, BF16>(gm, mc, my, g, splits, st);
+    if (mnk >= 0) {
+        if (BN == 128) e = any ? launch_gemm_mn<128, true>(mnk, gm, mc, my, g, splits, st) : launch_gemm_mn<128, false>(mnk, gm, mc, my, g, splits, st);
+        else if (BN == 64) e = any ? launch_gemm_mn<64, true>(mnk, gm, mc, my, g, splits, st) : launch_gemm_mn<64, false>(mnk, gm, mc, my, g, splits, st);
+        else e = any ? launch_gemm_mn<32, true>(mnk, gm, mc, my, g, splits, st) : launch_gemm_mn<32, false>(mnk, gm, mc, my, g, splits, st);
+    } else if (cluster == 2) e = any ? launch_gemm<128, true, 2, BF16>(gm, mc, my, g, splits, st) : launch_gemm<128, false, 2, BF16>(gm, mc, my, g, splits, st);
     else if (BN == 128) e = any ? launch_gemm<128, true, 1, BF16>(gm, mc, my, g, splits, st) : launch_gemm<128, false, 1, BF16>(gm, mc, my, g, splits, st);
     else if (BN == 64) e = any ? launch_gemm<64, true, 1, BF16>(gm, mc, my, g, splits, st) : launch_gemm<64, false, 1, BF16>(gm, mc, my, g, splits, st);
     else e = any ? launch_gemm<32, true, 1, BF16>(gm, mc, my, g, splits, st) : launch_gemm<32, false, 1, BF16>(gm, mc, my, g, splits, st);
@@ -1178,6 +1274,26 @@ extern "C" int go1_gemm_bf16_ex(int transA, int transB, int M, int N, int K, con
     if (!A || !B || !ep || M <= 0 || N <= 0 || K <= 0) return go1_set_error("go1_gemm_bf16_ex: bad arguments");
     if (!ep->out_bf16 && (!Cm || ldc < N)) return go1_set_error("go1_gemm_bf16_ex: bad output");
     return gemm_wgmma_impl<uint16_t>(transA, transB, M, N, K, 1, &A, lda, &B, ldb, &Cm, ldc, ep, (cudaStream_t)stream);
+}
+// BF16 operands in either major, read in place (MN-major ones through the tensor core's transpose immediates); C fp32, or with c_bf16 a
+// row-major BF16 matrix (uint16_t, ldc elements); the full fused epilogue (include/go1_b200.h)
+extern "C" int go1_gemm_bf16_mn(int transA, int transB, int M, int N, int K, const uint16_t* A, int lda, const uint16_t* B, int ldb,
+                                void* Cm, int ldc, int c_bf16, const Go1GemmEpilogue* ep, void* stream) {
+    if (!A || !B || !ep || M <= 0 || N <= 0 || K <= 0 || (transA & ~1) || (transB & ~1) || (c_bf16 & ~1)) return go1_set_error("go1_gemm_bf16_mn: bad arguments");
+    if (!ep->out_bf16 && (!Cm || ldc < (ep->store_transposed ? M : N))) return go1_set_error("go1_gemm_bf16_mn: bad output");
+    float* C = (float*)Cm;
+    return gemm_wgmma_impl<uint16_t>(transA, transB, M, N, K, 1, &A, lda, &B, ldb, &C, ldc, ep, (cudaStream_t)stream, true, c_bf16 != 0);
+}
+// go1_gemm_grouped with BF16 operands in either major (the equal-shape weight gradients of AC_Args.bf16_backward)
+extern "C" int go1_gemm_bf16_grouped(int transA, int transB, int M, int N, int K, int nprob, const uint16_t* const* A, int lda, const uint16_t* const* B, int ldb,
+                                     float* const* C, int ldc, int accumulate, void* stream) {
+    if (!A || !B || !C || nprob < 1 || nprob > GEMM_MAXP || M <= 0 || N <= 0 || K <= 0 || (transA & ~1) || (transB & ~1))
+        return go1_set_error("go1_gemm_bf16_grouped: 1..4 problems");
+    for (int p = 0; p < nprob; p++) if (!A[p] || !B[p] || !C[p]) return go1_set_error("go1_gemm_bf16_grouped: bad arguments");
+    if (ldc < N) return go1_set_error("go1_gemm_bf16_grouped: bad output");
+    Go1GemmEpilogue ep = {};
+    ep.accumulate = accumulate;
+    return gemm_wgmma_impl<uint16_t>(transA, transB, M, N, K, nprob, A, lda, B, ldb, C, ldc, &ep, (cudaStream_t)stream, true, false);
 }
 // nprob (<= 4) products of the same shape and operand strides in ONE grid: C[p] (+)= op(A[p]) op(B[p]).  Meant for the equal-shape
 // split-K wgrads of the three MLPs (128 x 256 x 24576 three times, 256 x 512 x 24576 twice per optimizer step): one launch fills the

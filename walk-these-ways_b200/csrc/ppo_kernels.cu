@@ -5,6 +5,7 @@
 //   (ppo.py:168-186), global grad-norm + clip + Adam (ppo.py:155-158), row gather
 //   (rollout_storage.py:98-137).
 #include <cuda_runtime.h>
+#include <cuda_bf16.h>
 #include <math.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -1123,8 +1124,9 @@ __global__ void skinny_dgrad_kernel(const float* __restrict__ dz, int lddz, cons
 // float4 variant: a warp owns rows (stride 8 inside the block's row slab), a lane owns 4 consecutive columns of a 128-column group and keeps
 // its O x 4 weights in registers; the row's o output gradients are fetched by the first o lanes and shuffle-broadcast.  Optionally the
 // column sums of the values written (= the bias gradient of the layer below) are reduced here as well: per-lane partial sums, one
-// shared-memory reduction per block, one set of atomics per block.
-template <int O, int KIND>
+// shared-memory reduction per block, one set of atomics per block.  OUT16: dprev is a BF16 matrix (uint16_t, lddp elements) that gets the
+// values rounded to nearest even; the column sums see the fp32 values (go1_skinny_dgrad_act_bf16).
+template <int O, int KIND, bool OUT16 = false>
 __global__ void __launch_bounds__(256) skinny_dgrad4_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ W, int ldw, const float* __restrict__ y, int ldy,
                                                             float* __restrict__ dprev, int lddp, float* __restrict__ colsum, int M, int o, int n, int rows_per_block) {
     __shared__ float4 s_sum[8][32];
@@ -1151,7 +1153,13 @@ __global__ void __launch_bounds__(256) skinny_dgrad4_kernel(const float* __restr
             v0 = fmaf(d, wr[t][0], v0); v1 = fmaf(d, wr[t][1], v1); v2 = fmaf(d, wr[t][2], v2); v3 = fmaf(d, wr[t][3], v3);
         }
         if (y) { v0 *= act_deriv<KIND>(yy.x); v1 *= act_deriv<KIND>(yy.y); v2 *= act_deriv<KIND>(yy.z); v3 *= act_deriv<KIND>(yy.w); }
-        if (col_ok) *reinterpret_cast<float4*>(dprev + (size_t)m * lddp + c) = make_float4(v0, v1, v2, v3);
+        if (OUT16) {
+            if (col_ok) {
+                uint16_t* d16 = reinterpret_cast<uint16_t*>(dprev) + (size_t)m * lddp + c;
+                *reinterpret_cast<uint2*>(d16) = make_uint2((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v0)) | ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v1)) << 16),
+                                                            (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v2)) | ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v3)) << 16));
+            }
+        } else if (col_ok) *reinterpret_cast<float4*>(dprev + (size_t)m * lddp + c) = make_float4(v0, v1, v2, v3);
         cs.x += v0; cs.y += v1; cs.z += v2; cs.w += v3;
     }
     if (colsum) {
@@ -1187,6 +1195,25 @@ extern "C" int go1_skinny_dgrad_act(const float* dz, int lddz, const float* W, i
     const size_t tot = (size_t)M * n;
     skinny_dgrad_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, M, o, n, kind); go1_count_launch(1);
     return cuda_rc("go1_skinny_dgrad");
+}
+// go1_skinny_dgrad_act with a BF16 dprev (AC_Args.bf16_backward: the head's dgrad stores the hidden dz the BF16 products read)
+extern "C" int go1_skinny_dgrad_act_bf16(const float* dz, int lddz, const float* W, int ldw, const float* y_prev, int ldy, uint16_t* dprev, int lddp,
+                                         float* colsum, int M, int o, int n, int kind, void* stream) {
+    if (!dz || !W || !dprev || M <= 0 || o <= 0 || o > 16 || n <= 0) return go1_set_error("go1_skinny_dgrad_act_bf16: bad arguments");
+    if (!go1_act_kind_ok(kind)) return go1_set_error("go1_skinny_dgrad_act_bf16: unknown activation kind (Go1Activation)");
+    if ((n & 3) || (ldw & 3) || (lddp & 3) || lddp < n || (y_prev && (ldy & 3)) || ((((uintptr_t)W) | ((uintptr_t)(y_prev ? y_prev : W))) & 15) || (((uintptr_t)dprev) & 7))
+        return go1_set_error("go1_skinny_dgrad_act_bf16: n, ldw, lddp, ldy multiples of 4; W / y_prev 16-byte and dprev 8-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int cb = (n + 127) / 128;
+    int rpb = (M * cb + 2 * 132 - 1) / (2 * 132);
+    rpb = (rpb + 7) / 8 * 8; if (rpb < 8) rpb = 8;
+    dim3 grid(cb, (M + rpb - 1) / rpb);
+    float* out = reinterpret_cast<float*>(dprev);
+#define LAUNCH(O, KD) skinny_dgrad4_kernel<O, KD, true><<<grid, 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, out, lddp, colsum, M, o, n, rpb)
+    GO1_ACT_SWITCH(kind, KD, if (o <= 2) LAUNCH(2, KD); else if (o <= 4) LAUNCH(4, KD); else LAUNCH(16, KD);)
+#undef LAUNCH
+    go1_count_launch(1);
+    return cuda_rc("go1_skinny_dgrad_act_bf16");
 }
 extern "C" int go1_skinny_dgrad_ex(const float* dz, int lddz, const float* W, int ldw, const float* y_prev, int ldy, float* dprev, int lddp,
                                    float* colsum, int M, int o, int n, void* stream) {

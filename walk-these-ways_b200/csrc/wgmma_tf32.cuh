@@ -1,7 +1,8 @@
 // wgmma_tf32.cuh — sm_90a warpgroup MMA (wgmma.mma_async, TF32 or BF16 operands from shared memory, fp32 accumulators in registers).
 //
 // One TF32 instruction multiplies a 64 x 8 slice of A by an 8 x N slice of B (BF16: 64 x 16 by 16 x N), both K-major in shared memory
-// (TF32 wgmma has no transposed-operand form: MN-major data must be brought to K-major first).  Accumulator fragment of thread t of the warpgroup
+// (TF32 wgmma has no transposed-operand form: MN-major data must be brought to K-major first; BF16 reads MN-major tiles through its transpose
+// immediates: mma_kblock_bf16).  Accumulator fragment of thread t of the warpgroup
 // (warp w = t / 32, lane l): d[4 j + 0 / 1] = C[16 w + l / 4][8 j + 2 (l % 4) + 0 / 1], d[4 j + 2 / 3] = the same columns of row + 8.
 #pragma once
 #include <stdint.h>
@@ -56,6 +57,49 @@ template <int N, bool BF16 = false> __device__ __forceinline__ void mma_kblock(f
     const uint64_t da = desc(a), db = desc(b);
 #pragma unroll
     for (int k = 0; k < 4; k++) mma<N, BF16>(d, da + 2 * k, db + 2 * k, (accumulate || k > 0) ? 1u : 0u);
+}
+
+// MN-major 16-bit operand tiles, as TMA writes a [64 k][64 mn] box with CU_TENSOR_MAP_SWIZZLE_128B (128-byte rows along MN, 16-byte
+// chunks XOR-swizzled by k % 8).  PTX ISA's MN-major canonical layout: the 8-k-row groups are the stride byte offset apart (1024 B) and the
+// next 64 mn (the next box) the leading byte offset apart (lbo).  One k16 instruction step is 16 k-rows = 2048 B: +128 in the descriptor.
+__device__ __forceinline__ uint64_t desc_mn128(const void* smem, uint32_t lbo) {
+    uint64_t d = 0;
+    d |= (uint64_t)(((uint32_t)__cvta_generic_to_shared(smem) >> 4) & 0x3FFF);
+    d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
+    d |= (uint64_t)(1024 >> 4) << 32;
+    d |= (uint64_t)1 << 62;                                                         // SWIZZLE_128B
+    return d;
+}
+// The 32-wide form, a [64 k][32 mn] box with CU_TENSOR_MAP_SWIZZLE_64B (64-byte rows): 8-k-row groups 512 B apart, a k16 step is 1024 B (+64).
+__device__ __forceinline__ uint64_t desc_mn64(const void* smem) {
+    uint64_t d = 0;
+    d |= (uint64_t)(((uint32_t)__cvta_generic_to_shared(smem) >> 4) & 0x3FFF);
+    d |= (uint64_t)1 << 16;
+    d |= (uint64_t)(512 >> 4) << 32;
+    d |= (uint64_t)2 << 62;                                                         // SWIZZLE_64B
+    return d;
+}
+
+// BF16 instructions with the transpose immediates TA / TB (1: that operand is MN-major in shared memory)
+#define GO1_WG_MMAT(INSTR, R, A, B, P, TA, TB, ...) \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" P ", 0;\n\t" INSTR " " R ", %" A ", %" B ", p, 1, 1, %" TA ", %" TB ";\n\t}" \
+                 : __VA_ARGS__ : "l"(da), "l"(db), "r"(accumulate), "n"(TRA), "n"(TRB))
+template <int N> struct MmaBf16T;
+template <> struct MmaBf16T<32> { template <int TRA, int TRB> static __device__ __forceinline__ void run(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+    GO1_WG_MMAT("wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16", GO1_WG_R16, "16", "17", "18", "19", "20", GO1_WG_D16); } };
+template <> struct MmaBf16T<64> { template <int TRA, int TRB> static __device__ __forceinline__ void run(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+    GO1_WG_MMAT("wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16", GO1_WG_R32, "32", "33", "34", "35", "36", GO1_WG_D32); } };
+template <> struct MmaBf16T<128> { template <int TRA, int TRB> static __device__ __forceinline__ void run(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    GO1_WG_MMAT("wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16", GO1_WG_R64, "64", "65", "66", "67", "68", GO1_WG_D64); } };
+#undef GO1_WG_MMAT
+
+// One BF16 k-block (64 k) of a 64 x N product whose operands are K-major (TA / TB = 0: da / db from desc, +2 per k16) or MN-major
+// (1: da from desc_mn128, db from desc_mn128 or, N = 32, desc_mn64; +128 / +64 per k16).
+template <int N, int TA, int TB>
+__device__ __forceinline__ void mma_kblock_bf16(float (&d)[N / 2], const uint64_t da, const uint64_t db, bool accumulate) {
+    constexpr uint32_t sa = TA ? 128 : 2, sb = TB ? (N == 32 ? 64 : 128) : 2;
+#pragma unroll
+    for (int k = 0; k < 4; k++) MmaBf16T<N>::template run<TA, TB>(d, da + sa * k, db + sb * k, (accumulate || k > 0) ? 1u : 0u);
 }
 
 }  // namespace wg

@@ -171,6 +171,22 @@ def copy_segments(pairs):
     check(lib().go1_copy_segments(arr, n, stream_ptr()), "go1_copy_segments")
 
 
+class Go1Bf16Seg(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("lds", _i), ("dst", C.c_void_p), ("ldd", _i), ("rows", _i), ("cols", _i)]
+
+
+def convert_bf16_segments(pairs):
+    """dst.copy_(src.to(torch.bfloat16)) for (dst, src) pairs -- BF16 dst, float32 src, 2-D CUDA tensors with unit inner stride -- in one
+    go1_convert_bf16_segments launch per 16 pairs."""
+    for k0 in range(0, len(pairs), 16):
+        chunk = pairs[k0:k0 + 16]
+        arr = (Go1Bf16Seg * len(chunk))()
+        for sg, (dst, src) in zip(arr, chunk):
+            assert dst.shape == src.shape and dst.dim() == 2 and dst.stride(1) == 1 and src.stride(1) == 1
+            sg.src, sg.lds, sg.dst, sg.ldd, sg.rows, sg.cols = src.data_ptr(), src.stride(0), dst.data_ptr(), dst.stride(0), dst.shape[0], dst.shape[1]
+        check(lib().go1_convert_bf16_segments(arr, len(chunk), stream_ptr()), "go1_convert_bf16_segments")
+
+
 class Go1Error(RuntimeError):
     pass
 
@@ -229,6 +245,10 @@ def lib():
         "go1_transpose_to_bf16": ([vp, ip, vp, ip, ip, ip, vp], ip),
         "go1_transpose_bf16": ([vp, ip, vp, ip, ip, ip, vp], ip),
         "go1_gemm_grouped": ([ip, ip, ip, ip, ip, ip, C.POINTER(vp), ip, C.POINTER(vp), ip, C.POINTER(vp), ip, ip, vp], ip),
+        "go1_gemm_bf16_mn": ([ip, ip, ip, ip, ip, vp, ip, vp, ip, vp, ip, ip, C.POINTER(Go1GemmEpilogue), vp], ip),
+        "go1_gemm_bf16_grouped": ([ip, ip, ip, ip, ip, ip, C.POINTER(vp), ip, C.POINTER(vp), ip, C.POINTER(vp), ip, ip, vp], ip),
+        "go1_convert_bf16_segments": ([C.POINTER(Go1Bf16Seg), ip, vp], ip),
+        "go1_skinny_dgrad_act_bf16": ([vp, ip, vp, ip, vp, ip, vp, ip, vp, ip, ip, ip, ip, vp], ip),
         "go1_copy_segments": ([C.POINTER(Go1CopySeg), ip, vp], ip),
         "go1_skinny_forward": ([vp, ip, vp, ip, vp, vp, ip, ip, ip, ip, vp], ip),
         "go1_skinny_wgrad": ([vp, ip, vp, ip, vp, ip, ip, ip, ip, ip, vp], ip),

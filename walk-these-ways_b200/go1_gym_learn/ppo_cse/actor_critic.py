@@ -31,6 +31,8 @@ class AC_Args(PrefixProto, cli=False):
     use_decoder = False
     gemm_impl = 1       # 1 = wgmma TF32 tensor cores (default; torch 1.10, the reference's pin, also ran these matmuls in TF32), 0 = fp32 CUDA cores (exact),
                         # 2 = as 1, but the products that reduce over the observation history (the first layers) take BF16 operands (fp32 accumulation)
+    bf16_backward = False   # with gemm_impl = 2 only: the hidden layers' dgrads and weight gradients run on BF16 too (MN-major operands read in place);
+                            # hidden-layer dz is then held in BF16 (see ActorCritic.backward_ppo)
 
 
 def _mlp(in_dim, hidden, out_dim, activation):
@@ -137,6 +139,9 @@ class _Net:
     def _packed16(self, li, K):
         """(copy, pitch): W[:, :K] of layer li in BF16 (rounded to nearest even), row pitch capi.bf16_pitch(K), rebuilt once per weight version
         (AC_Args.gemm_impl = 2: the first layers' operand)."""
+        return self._cached(("pack16", li), self._packed16_build(li, K)), capi.bf16_pitch(K)
+
+    def _packed16_build(self, li, K):
         wo, bo, o, i = self.specs[li]
         W = self.flat[wo:wo + o * i]
         KPk = capi.bf16_pitch(K)
@@ -145,7 +150,22 @@ class _Net:
             dst = old if old is not None else _empty(o, KPk, device=W.device, dtype=torch.bfloat16)[:, :K]
             capi.check(capi.lib().go1_convert_bf16(W.data_ptr(), i, capi.ptr(dst), KPk, o, K, capi.stream_ptr()), "convert_bf16")
             return dst
-        return self._cached(("pack16", li), build), KPk
+        return build
+
+    def packed16_pairs(self):
+        """The (dst, src) conversions that bring the BF16 weight copies of layers 1.. (the MN-major B operands of backward_bf16's dgrads)
+        up to the current weight version.  Their cache entries are marked current here; the caller launches the conversions
+        (ActorCritic._convert_outputs: in the one launch that also makes the output copies, instead of one launch per layer)."""
+        ver, pairs = self.owner.weights_version, []
+        for li in range(1, len(self.specs)):
+            key = ("pack16", li)
+            hit = self._cache.get(key)
+            if hit is None or hit[0] != ver:
+                wo, bo, o, i = self.specs[li]
+                dst = hit[1] if hit is not None else _empty(o, capi.bf16_pitch(i), device=self.flat.device, dtype=torch.bfloat16)[:, :i]
+                pairs.append((dst, self.flat[wo:wo + o * i].view(o, i)))
+                self._cache[key] = (ver, dst, self._packed16_build(li, i))
+        return pairs
 
     def _weight_tma(self, li):
         """(W, row stride) of layer li for a TMA operand: in place when its rows allow it, else the packed copy."""
@@ -177,9 +197,9 @@ class _Net:
         return x.data_ptr() if torch.is_tensor(x) else x
 
     def _gemm(self, ta, tb, M, N, K, A, lda, B, ldb, Cm, ldc, bias=None, act=0, acc=0, impl=0, extra=None, w_extra=0, ld_w_extra=0, dact_y=None, lead_cols=0,
-              colsum=None, bwd_extra=None, store_transposed=0, bf16=False, out16=None):
+              colsum=None, bwd_extra=None, store_transposed=0, bf16=False, out16=None, mn=False):
         """go1_gemm_ex (impl 0 / 1), or go1_gemm_bf16_ex with bf16: A and B BF16.  out16: a BF16 tensor that receives the transposed result
-        (store_transposed) in place of Cm."""
+        (store_transposed) in place of Cm.  mn: go1_gemm_bf16_mn (BF16 operands in either major; a BF16 Cm is stored row-major in BF16)."""
         ep = self._ep
         ep.out_bf16, ep.ld_out_bf16 = (out16.data_ptr(), out16.stride(0)) if out16 is not None else (None, 0)
         ep.lead_cols = lead_cols
@@ -202,7 +222,10 @@ class _Net:
             ep.dact_y, ep.ld_dact_y = dact_y.data_ptr(), dact_y.stride(0)
         else:
             ep.dact_y = None
-        if bf16:
+        if mn:
+            c16 = 1 if torch.is_tensor(Cm) and Cm.dtype == torch.bfloat16 else 0
+            capi.check(capi.lib().go1_gemm_bf16_mn(ta, tb, M, N, K, self._p(A), lda, self._p(B), ldb, self._p(Cm), ldc, c16, ep, capi.stream_ptr()), "go1_gemm_bf16_mn")
+        elif bf16:
             capi.check(capi.lib().go1_gemm_bf16_ex(ta, tb, M, N, K, self._p(A), lda, self._p(B), ldb, self._p(Cm), ldc, ep, capi.stream_ptr()), "go1_gemm_bf16")
         else:
             capi.check(capi.lib().go1_gemm_ex(ta, tb, M, N, K, self._p(A), lda, self._p(B), ldb, self._p(Cm), ldc, ep, impl, capi.stream_ptr()), "go1_gemm")
@@ -408,6 +431,94 @@ class _Net:
                 bias_done = False
             dz = dprev if dprev is not None else out16
 
+    def bf16_inputs(self, outs):
+        """[(layer, width)] of the hidden outputs whose BF16 copies backward_bf16 reads: the input of every weight gradient behind the first
+        layer that runs on BF16 (every hidden layer's, and the head's when it is wider than the skinny kernels' 16 columns)."""
+        n = len(self.specs)
+        return [(li - 1, self.specs[li][3]) for li in range(1, n) if li < n - 1 or self.specs[li][2] > 16]
+
+    def backward_bf16(self, x, ldx, K0, extra, outs, y16, dout, M, dz1T, want_dextra=False, tag="a", wgrads=None):
+        """backward() of AC_Args.bf16_backward (M >= 64; dz1T: the BF16 transposed first-layer dz, whose wgrad the caller makes).  The head
+        gradient dout (fp32, from the loss kernels) goes through the head's fp32 skinny dgrad and that output is converted to BF16 (a head
+        wider than 16 columns: dout itself is converted and the head's products run on BF16); every dgrad behind it is a go1_gemm_bf16_mn
+        product of the BF16 dz and a BF16 copy of W (_packed16, read MN-major) whose epilogue multiplies by f'(y) from the fp32 saved output,
+        reduces the bias gradient from the fp32 values and rounds the stored dz to BF16 (row-major, or dz1T transposed).  Weight gradients behind the
+        first layer read the BF16 dz and y16[l] (the BF16 copy of outs[l], ActorCritic._convert_outputs), both MN-major; a head of at most
+        16 columns keeps its fp32 skinny kernels.  Returns d(extra) [M][E] if requested."""
+        L, st = capi.lib(), capi.stream_ptr()
+        n = len(self.specs)
+        dextra, extra_done, dz1T16 = None, False, None
+        wo, bo, o, i = self.specs[-1]
+        gW, gb = self.grad[wo:wo + o * i], self.grad[bo:bo + o]
+        inp = outs[n - 2]
+        if o <= 16:             # the head: weight and bias gradient in one fp32 pass over its input, as at gemm_impl 2
+            if i % 4 == 0 and self._tma_ok(inp, inp.stride(0)):
+                capi.check(L.go1_skinny_wgrad_ex(capi.ptr(dout), dout.stride(0), capi.ptr(inp), inp.stride(0), gW.data_ptr(), i, gb.data_ptr(), M, o, i, 1, st), "skinny_wgrad")
+            else:
+                capi.check(L.go1_colsum(capi.ptr(dout), dout.stride(0), capi.ptr(gb), M, o, 0, st), "colsum")
+                capi.check(L.go1_skinny_wgrad(capi.ptr(dout), dout.stride(0), capi.ptr(inp), inp.stride(0), gW.data_ptr(), i, M, o, i, 1, st), "skinny_wgrad")
+        else:
+            capi.check(L.go1_colsum(capi.ptr(dout), dout.stride(0), capi.ptr(gb), M, o, 0, st), "colsum")
+        if o <= 16 and n > 2:
+            # the head's dgrad on its fp32 skinny kernel, as at gemm_impl 2, storing BF16 (a K <= 16 tensor-core product pays for a whole
+            # 64-deep k-block and measured slower: 35-45 us per launch at M = 24576); the bias gradient below it from the fp32 values
+            pwo, pbo, po, pi = self.specs[n - 2]
+            W, gb_prev, yprev = self.flat[wo:wo + o * i], self.grad[pbo:pbo + po], outs[n - 2]
+            dz = self._buf16((tag, "d16", n - 2), M, i)
+            if i % 4 == 0 and self._tma_ok(W, i) and self._tma_ok(yprev, yprev.stride(0)):
+                capi.check(L.go1_skinny_dgrad_act_bf16(capi.ptr(dout), dout.stride(0), capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(dz),
+                                                       dz.stride(0), gb_prev.data_ptr(), M, o, i, self.kind, st), "skinny_dgrad_bf16")
+            else:           # rows the vector kernel cannot read: fp32 first, then its column sums and BF16 copy
+                d32 = self._hbuf((tag, "dskinny"), M, i)
+                capi.check(L.go1_skinny_dgrad_act(capi.ptr(dout), dout.stride(0), capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(d32),
+                                                  d32.stride(0), None, M, o, i, self.kind, st), "skinny_dgrad")
+                capi.check(L.go1_colsum(capi.ptr(d32), d32.stride(0), capi.ptr(gb_prev), M, i, 0, st), "colsum")
+                capi.convert_bf16_segments([(dz, d32)])
+            first = n - 2
+        else:       # a head wider than 16 (or a one-hidden-layer net, whose head dgrad stores dz1T): BF16 head gradient, tensor-core products
+            dz = self._buf16((tag, "dhead16"), M, o)
+            capi.convert_bf16_segments([(dz, dout)])
+            first = n - 1
+        for li in range(first, 0, -1):
+            wo, bo, o, i = self.specs[li]
+            gW = self.grad[wo:wo + o * i]
+            if li < n - 1 or o > 16:    # wgrad dW[o][i] = dz^T y_{li-1}: both operands MN-major, split-K partial tiles add into the zeroed gradient
+                yb = y16[li - 1]
+                if wgrads is not None:
+                    wgrads.append((o, i, M, dz.stride(0), yb.stride(0), i, dz, yb, gW))
+                else:
+                    self._gemm(1, 0, o, i, M, dz, dz.stride(0), yb, yb.stride(0), gW, i, None, 0, 1, 1, mn=True)
+            # dgrad dz_prev[M][i] = (dz[M][o] W[o][i]) * f'(y_prev), W read MN-major from its BF16 copy
+            pwo, pbo, po, pi = self.specs[li - 1]
+            gb_prev, yprev = self.grad[pbo:pbo + po], outs[li - 1]
+            W16, ldw16 = self._packed16(li, i)
+            bx, out16, colsum = None, None, gb_prev
+            if li == 1:
+                colsum = None           # the first layer's bias gradient is the caller's (the augmented row of its wgrad)
+                if extra is not None and pi - K0 > 4 and want_dextra:
+                    # a wide trailing input's d(extra) is a pass over the stored dz (go1_mlp_extra_backward): fp32 first, the BF16 copy after it
+                    dz1T16, dprev = dz1T, self._buf((tag, "dz1T32"), i, M, capi.row_pitch(M))
+                else:
+                    out16, dprev = dz1T, None
+                if extra is not None and 1 <= pi - K0 <= 4 and want_dextra:
+                    extra_done = True   # d(extra) of a narrow trailing input in this epilogue
+                    dextra = self._buf((tag, "dextra"), M, pi - K0).zero_()
+                    bx = (extra, self.flat.data_ptr() + 4 * (pwo + K0), pi, None, pi, dextra)
+            else:
+                dprev = self._buf16((tag, "d16", li - 1), M, i)
+            self._gemm(0, 0, M, i, o, dz, dz.stride(0), W16, ldw16, dprev, dprev.stride(0) if dprev is not None else 0, None, 2, 0, 1, dact_y=yprev,
+                       colsum=colsum, bwd_extra=bx, store_transposed=1 if li == 1 else 0, out16=out16, mn=True)
+            dz = dprev
+        if extra is not None and not extra_done and want_dextra:
+            E = self.specs[0][3] - K0
+            dextra = self._buf((tag, "dextra"), M, E)
+            W = self.flat[self.specs[0][0]:]
+            capi.check(L.go1_mlp_extra_backward(capi.ptr(dz), dz.stride(0), 1, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, self.specs[0][3],
+                                                None, self.specs[0][3], capi.ptr(dextra), E, M, self.specs[0][2], E, 0, st), "extra_backward")
+        if dz1T16 is not None:
+            capi.check(L.go1_convert_bf16(capi.ptr(dz), dz.stride(0), capi.ptr(dz1T16), dz1T16.stride(0), self.specs[0][2], M, st), "convert_bf16")
+        return dextra
+
 
 class ActorCritic(nn.Module):
     is_recurrent = False
@@ -543,7 +654,33 @@ class ActorCritic(nn.Module):
         impl = int(AC_Args.gemm_impl)
         if impl not in (0, 1, 2):
             raise ValueError(f"AC_Args.gemm_impl = {AC_Args.gemm_impl!r}: expected 0 (fp32 CUDA cores), 1 (TF32 tensor cores) or 2 (BF16 history products)")
+        if AC_Args.bf16_backward and impl != 2:
+            raise ValueError(f"AC_Args.bf16_backward = True needs AC_Args.gemm_impl = 2 (it is {impl})")
         return impl
+
+    def _bf16_backward(self):
+        """AC_Args.bf16_backward, validated with the mode (_impl)."""
+        return self._impl() == 2 and bool(AC_Args.bf16_backward)
+
+    def _convert_outputs(self, named_outs, M, defer=False):
+        """{net name: {layer: BF16 copy}} of the hidden outputs that the nets' backward_bf16 weight gradients read, made together with the
+        BF16 copies of the weights their dgrads read (stale after every optimizer step) by ONE go1_convert_bf16_segments launch per
+        minibatch forward (two beyond 16 matrices; named_outs: [(net name, outs)]).  defer: only the weight copies are converted here;
+        returns (copies, output pairs) and the caller converts the outputs (_backward_bodies: on the side stream, beside the dgrads)."""
+        wpairs, ypairs, y16 = [], [], {}
+        for name, outs in named_outs:
+            net, y16[name] = self._nets[name], {}
+            wpairs += net.packed16_pairs()
+            for l, w in net.bf16_inputs(outs):
+                y16[name][l] = net._buf16(("y16", name, l), M, w)
+                ypairs.append((y16[name][l], outs[l]))
+        if defer:
+            if wpairs:
+                capi.convert_bf16_segments(wpairs)
+            return y16, ypairs
+        if wpairs + ypairs:
+            capi.convert_bf16_segments(wpairs + ypairs)
+        return y16
 
     def _check_input(self, h):
         if not h.is_cuda:
@@ -764,16 +901,19 @@ class ActorCritic(nn.Module):
         import ctypes as C
         groups = {}
         for it in wgrads:
-            groups.setdefault(it[:6], []).append(it)
+            groups.setdefault(it[:6] + (it[6].dtype,), []).append(it)
         L, st = capi.lib(), capi.stream_ptr()
-        for (o, K, M, ldz, ld_in, i), items in groups.items():
+        for (o, K, M, ldz, ld_in, i, dt), items in groups.items():
             for k0 in range(0, len(items), 4):
                 chunk = items[k0:k0 + 4]
                 n = len(chunk)
                 A = (C.c_void_p * n)(*[it[6].data_ptr() for it in chunk])
                 B = (C.c_void_p * n)(*[it[7].data_ptr() for it in chunk])
                 Cc = (C.c_void_p * n)(*[it[8].data_ptr() for it in chunk])
-                capi.check(L.go1_gemm_grouped(1, 0, o, K, M, n, A, ldz, B, ld_in, Cc, i, 1, st), "go1_gemm_grouped")
+                if dt == torch.bfloat16:        # AC_Args.bf16_backward: BF16 dz and layer inputs, both MN-major
+                    capi.check(L.go1_gemm_bf16_grouped(1, 0, o, K, M, n, A, ldz, B, ld_in, Cc, i, 1, st), "go1_gemm_bf16_grouped")
+                else:
+                    capi.check(L.go1_gemm_grouped(1, 0, o, K, M, n, A, ldz, B, ld_in, Cc, i, 1, st), "go1_gemm_grouped")
 
     def _first_layers_fusable(self, h, priv):
         """The first layers of the three nets can run their backward as one K-major product over hT (history_kmajor)."""
@@ -823,7 +963,8 @@ class ActorCritic(nn.Module):
             capi.check(capi.lib().go1_transpose_to_bf16(capi.ptr(self._latent), self._latent.stride(0), capi.ptr(hT[K0 + 1 + E:]), hT.stride(0), M, E,
                                                         capi.stream_ptr()), "transpose_to_bf16")
             dz1 = nets["adapt"]._buf(("train", "dz1catT16"), oa + op + oc, M, hT.stride(0), torch.bfloat16)
-            self._backward_bodies(h, priv, dmean, dvalue, dz1, oa, op, M, K0)
+            y16 = self._convert_outputs((("adapt", self._a_out), ("actor", self._p_out), ("critic", self._c_out)), M, defer=True) if self._bf16_backward() else None
+            self._backward_bodies(h, priv, dmean, dvalue, dz1, oa, op, M, K0, y16)
             self._first_layer_wgrad(("adapt", "actor", "critic"), dz1, hT, M, "train")
         elif self._first_layers_fusable(h, priv):
             # the three first layers share their input: ONE transposed dz [o_a+o_p+o_c][M] (each net's layer-2 dgrad stores its
@@ -846,21 +987,35 @@ class ActorCritic(nn.Module):
             nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, tag="train")
         self._grad[self.std_offset:self.std_offset + self.num_actions].copy_(dstd)
 
-    def _backward_bodies(self, h, priv, dmean, dvalue, dz1, oa, op, M, K0):
+    def _backward_bodies(self, h, priv, dmean, dvalue, dz1, oa, op, M, K0, y16=None):
         """The three nets' backward passes down to their first-layer dz, stored transposed into the row slices of dz1 ([adapt | actor |
-        critic] x M), and the tensor-core wgrads behind the first layers, launched as grouped products once all dz exist."""
+        critic] x M), and the tensor-core wgrads behind the first layers, launched as grouped products once all dz exist.  y16: (the BF16
+        output copies of AC_Args.bf16_backward, the conversions that make them) from _convert_outputs(defer=True): the nets run
+        backward_bf16.  Only those grouped wgrads read the copies, so the conversion runs first on the critic's side stream, beside the
+        actor and adaptation dgrads (measured 2.2 ms of the 35 ms of kernel time of an update at 4096 envs, bandwidth-bound)."""
         nets, impl = self._nets, 1
         wgrads = []
+        ypairs = []
+        if y16 is not None:
+            y16, ypairs = y16
+
+        def bwd(name, extra, outs, dout, dz1T, want_dextra=False):
+            if y16 is not None:
+                return nets[name].backward_bf16(h, h.stride(0), K0, extra, outs, y16[name], dout, M, dz1T, want_dextra=want_dextra, tag="train", wgrads=wgrads)
+            return nets[name].backward(h, h.stride(0), K0, extra, outs, dout, M, impl, want_dextra=want_dextra, tag="train", dz1T=dz1T, wgrads=wgrads)
         side = self._side_stream(M)
         if side is not None:    # critic chain beside actor -> adaptation chain
             self._fork(side)
             with torch.cuda.stream(side):
-                nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, tag="train", dz1T=dz1[oa + op:], wgrads=wgrads)
-        dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, impl, want_dextra=True, tag="train", dz1T=dz1[oa:oa + op],
-                                      wgrads=wgrads)
+                if ypairs:
+                    capi.convert_bf16_segments(ypairs)
+                bwd("critic", priv, self._c_out, dvalue, dz1[oa + op:])
+        elif ypairs:
+            capi.convert_bf16_segments(ypairs)
+        dlat = bwd("actor", self._latent, self._p_out, dmean, dz1[oa:oa + op], want_dextra=True)
         if side is None:
-            nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, impl, tag="train", dz1T=dz1[oa + op:], wgrads=wgrads)
-        nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, tag="train", dz1T=dz1[:oa], wgrads=wgrads)
+            bwd("critic", priv, self._c_out, dvalue, dz1[oa + op:])
+        bwd("adapt", None, self._a_out, dlat, dz1[:oa])
         if side is not None:
             self._join(side)
         self._flush_wgrads(wgrads)
@@ -877,6 +1032,11 @@ class ActorCritic(nn.Module):
                 if hT is None:
                     hT = history_kmajor_bf16(self._model_input(h, "adapt"), None, net._buf16(("adapt", "hT16"), K0 + 1, M))
                 dz1 = net._buf(("adapt", "dz1T16"), oa, M, hT.stride(0), torch.bfloat16)
+                if self._bf16_backward():
+                    y16 = self._convert_outputs((("adapt", outs),), M)["adapt"]
+                    net.backward_bf16(h, h.stride(0), K0, None, outs, y16, dpred, M, dz1, tag="adapt")
+                    self._first_layer_wgrad(("adapt",), dz1, hT[:K0 + 1], M, "adapt")
+                    return
             else:
                 if hT is None:
                     hT = history_kmajor(h, None, net._buf(("adapt", "hT"), K0 + 1, (M + 31) // 32 * 32))

@@ -1,5 +1,7 @@
 #!/usr/bin/env python
-"""Per-shape table of a GO1_GEMM_TIMING_CSV dump (one PPO update): launches, total / mean microseconds, TFLOP/s, share."""
+"""Per-shape table of a GO1_GEMM_TIMING_CSV dump (one PPO update): launches, total / mean microseconds, TFLOP/s, share.  The bf16 column
+tells the operand paths apart: 0 TF32, 1 BF16 K-major (go1_gemm_bf16_ex), 2 BF16 in either major (go1_gemm_bf16_mn / _grouped, the products
+of AC_Args.bf16_backward)."""
 import collections, csv, sys
 
 
@@ -8,11 +10,11 @@ def main(path):
     agg = collections.OrderedDict()
     for r in rows:
         k = (r['M'], r['N'], r['K'], r['a_mn_major'], r['b_mn_major'], r['act'], r['num_extra'], r['splits'], r['kernel'], r['colsum'], r['n3'], r['heads'],
-             r['problems'])
+             r['problems'], r.get('bf16', '0'))
         a = agg.setdefault(k, [0, 0.0]); a[0] += 1; a[1] += float(r['us'])
     tot = sum(v[1] for v in agg.values())
     print(f"total {tot / 1e3:.2f} ms over {len(rows)} launches")
-    print("M N K amn bmn act nex splits kern colsum n3 heads problems | n total_us avg_us TF/s share%")
+    print("M N K amn bmn act nex splits kern colsum n3 heads problems bf16 | n total_us avg_us TF/s share%")
     for k, v in sorted(agg.items(), key=lambda kv: -kv[1][1]):
         M, N, K = int(k[0]), int(k[1]), int(k[2])
         fl = 2 * M * N * K

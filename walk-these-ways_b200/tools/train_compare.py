@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Learning-level evidence for the TF32 path (VERDICT r1, weak #2): trains scripts/train.py's configuration for K iterations
 with the tcgen05 TF32 GEMMs (AC_Args.gemm_impl = 1) and with the exact-fp32 CUDA-core GEMMs (impl 0) -- or, with --impls 1,2, the
-BF16 history products (impl 2) -- from the same seeds and
+BF16 history products (impl 2), or with 2b impl 2 plus AC_Args.bf16_backward -- from the same seeds and
 writes the reward-term trajectories (one record per `log_freq` iterations, like the reference's metrics.pkl) next to the first
 records of the shipped training log (tests/golden/metrics_envelope.json: Isaac Gym, 4000 envs).
     python walk-these-ways_b200/tools/train_compare.py --iterations 200 --out train_compare.json"""
@@ -23,12 +23,14 @@ KEYS = ["train/episode/rew_total/mean", "train/episode/rew_tracking_lin_vel/mean
         "train/episode/command_area_trot/mean", "adaptation_loss/mean", "mean_value_loss/mean", "mean_surrogate_loss/mean", "iterations"]
 
 
-NAMES = {0: "fp32", 1: "tf32", 2: "bf16"}
+NAMES = {"0": "fp32", "1": "tf32", "2": "bf16", "2b": "bf16_backward"}
 
 
-def run(impl, iterations, envs, tag):
+def run(impl, iterations, envs, tag, bf16_backward=False):
     import numpy as np
     from ml_logger import logger
+    from go1_gym_learn.ppo_cse.actor_critic import AC_Args
+    AC_Args.bf16_backward = bf16_backward
     torch.manual_seed(0); np.random.seed(0)
     env, runner = bench.build_training(envs, "cuda:0", impl, "flat")
     from go1_gym_learn.ppo_cse import RunnerArgs
@@ -45,6 +47,7 @@ def run(impl, iterations, envs, tag):
     out["env_steps_per_s_incl_logging"] = round(iterations * 24 * envs / dt)
     del env, runner
     torch.cuda.empty_cache()
+    AC_Args.bf16_backward = False
     return out
 
 
@@ -52,12 +55,12 @@ if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--iterations", type=int, default=200)
     ap.add_argument("--envs", type=int, default=4096)
-    ap.add_argument("--impls", default="1,0", help="comma-separated AC_Args.gemm_impl values: 0 fp32, 1 tf32, 2 bf16")
+    ap.add_argument("--impls", default="1,0", help="comma-separated AC_Args.gemm_impl values: 0 fp32, 1 tf32, 2 bf16; 2b = 2 with AC_Args.bf16_backward")
     ap.add_argument("--out", default=os.path.join(tempfile.gettempdir(), "go1_train_compare.json"))
     a = ap.parse_args()
     res = {"iterations": a.iterations, "envs": a.envs}
-    for impl in [int(x) for x in a.impls.split(",")]:
-        res[NAMES[impl]] = run(impl, a.iterations, a.envs, f"impl{impl}")
+    for m in a.impls.split(","):
+        res[NAMES[m]] = run(int(m.rstrip("b")), a.iterations, a.envs, f"impl{m}", bf16_backward=m.endswith("b"))
     with open(os.path.join(ROOT, "tests", "golden", "metrics_envelope.json")) as f:
         env = json.load(f)
     n = a.iterations // 10 + 1
@@ -65,7 +68,7 @@ if __name__ == "__main__":
     os.makedirs(os.path.dirname(a.out), exist_ok=True)
     with open(a.out, "w") as f:
         json.dump(res, f)
-    for name in ("tf32", "fp32", "bf16", "reference_isaacgym_4000_envs"):
+    for name in ("tf32", "fp32", "bf16", "bf16_backward", "reference_isaacgym_4000_envs"):
         if name in res:
             r = res[name]
             print(name, "rew_total", [None if x is None else round(x, 3) for x in r["train/episode/rew_total/mean"][::4]],
