@@ -51,28 +51,33 @@ def _empty(*shape, device, dtype=torch.float32):
         return torch.empty(*shape, device=device, dtype=dtype)
 
 
-def history_kmajor(h, priv, out):
-    """The first layers' input transposed, K-major for their weight-gradient products: out[K0 + 1 + 2E][>= M] (row pitch a multiple of
-    4 floats) gets h's K0 columns as rows 0..K0-1, ones in row K0 and priv's E columns in rows K0 + 1.. (priv None: only K0 + 1 rows).
-    Rows K0 + 1 + E.. are left for the latent, which ActorCritic.backward_ppo writes for each minibatch."""
-    M, K0 = h.shape[0], h.shape[1]
-    L, st = capi.lib(), capi.stream_ptr()
-    capi.check(L.go1_transpose(capi.ptr(h), h.stride(0), capi.ptr(out), out.stride(0), M, K0, st), "transpose")
-    out[K0, :M].fill_(1.0)
-    if priv is not None:
-        capi.check(L.go1_transpose(capi.ptr(priv), priv.stride(0), capi.ptr(out[K0 + 1:]), out.stride(0), M, priv.shape[1], st), "transpose")
+_TRANSPOSE = {(torch.float32, torch.float32): "go1_transpose", (torch.bfloat16, torch.bfloat16): "go1_transpose_bf16",
+              (torch.float32, torch.bfloat16): "go1_transpose_to_bf16"}
+
+
+def _transpose(x, out):
+    """out[:cols][:M] = x^T for x [M][cols] (unit inner strides); an fp32 x into a BF16 out is rounded to nearest even."""
+    name = _TRANSPOSE[(x.dtype, out.dtype)]
+    capi.check(getattr(capi.lib(), name)(capi.ptr(x), x.stride(0), capi.ptr(out), out.stride(0), x.shape[0], x.shape[1], capi.stream_ptr()), name)
+
+
+def _to_bf16(x, out):
+    """out = x rounded to BF16 (nearest even) in one go1_convert_bf16 launch; x fp32 [rows][cols], out BF16, unit inner strides."""
+    capi.check(capi.lib().go1_convert_bf16(capi.ptr(x), x.stride(0), capi.ptr(out), out.stride(0), x.shape[0], x.shape[1], capi.stream_ptr()), "convert_bf16")
     return out
 
 
-def history_kmajor_bf16(h16, priv, out):
-    """history_kmajor for AC_Args.gemm_impl = 2: h16 is the BF16 history [M][K0], out a BF16 [K0 + 1 + 2E][>= M] buffer (row pitch a
-    multiple of 8 elements); the history rows are copied, the ones row is exact and priv is rounded to BF16 (nearest even)."""
-    M, K0 = h16.shape[0], h16.shape[1]
-    L, st = capi.lib(), capi.stream_ptr()
-    capi.check(L.go1_transpose_bf16(capi.ptr(h16), h16.stride(0), capi.ptr(out), out.stride(0), M, K0, st), "transpose_bf16")
+def history_kmajor(h, priv, out):
+    """The first layers' input transposed, K-major for their weight-gradient products: out[K0 + 1 + 2E][>= M] gets h's K0 columns as rows
+    0..K0-1, ones in row K0 and priv's E columns in rows K0 + 1.. (priv None: only K0 + 1 rows).  Rows K0 + 1 + E.. are left for the
+    latent, which ActorCritic.backward_ppo writes for each minibatch.  out is fp32 with h fp32 (row pitch a multiple of 4 floats), or BF16
+    with the BF16 history of AC_Args.gemm_impl = 2 (row pitch a multiple of 8 elements): the history rows are copied, the ones row is
+    exact and priv is rounded to BF16 (nearest even)."""
+    M, K0 = h.shape[0], h.shape[1]
+    _transpose(h, out)
     out[K0, :M].fill_(1.0)
     if priv is not None:
-        capi.check(L.go1_transpose_to_bf16(capi.ptr(priv), priv.stride(0), capi.ptr(out[K0 + 1:]), out.stride(0), M, priv.shape[1], st), "transpose_to_bf16")
+        _transpose(priv, out[K0 + 1:])
     return out
 
 
@@ -128,43 +133,37 @@ class _Net:
         """A hidden activation or gradient buffer: TMA-readable rows whatever the width."""
         return self._buf(key, M, width, capi.row_pitch(width))
 
-    def _packed(self, li, K):
-        """(copy, pitch): W[:, :K] of layer li in a TMA-readable copy whose row pitch is a multiple of 128 bytes (any K: the kernels read the
-        K tail as zeros), rebuilt once per weight version."""
+    def _packed(self, li, K, dtype=torch.float32):
+        """(copy, pitch): W[:, :K] of layer li in a TMA-readable copy, rebuilt once per weight version: fp32 with a row pitch that is a
+        multiple of 128 bytes (any K: the kernels read the K tail as zeros), or BF16 (rounded to nearest even) with row pitch
+        capi.bf16_pitch(K) (AC_Args.gemm_impl = 2: the first layers' operand; AC_Args.bf16_backward: the dgrads' MN-major B operand)."""
+        W = self._cached((li, K, dtype), self._packer(li, K, dtype))
+        return W, W.stride(0)
+
+    def _packer(self, li, K, dtype):
+        """The builder of _packed's cache entry.  pairs: a list that receives the BF16 conversion (dst, src) in place of launching it."""
         wo, bo, o, i = self.specs[li]
-        W = self.flat[wo:wo + o * i]
-        KPk = (K + 31) // 32 * 32
-        return self._cached(("pack", li), lambda old: (old if old is not None else _empty(o, KPk, device=W.device)[:, :K]).copy_(W.view(o, i)[:, :K])), KPk
+        W = self.flat[wo:wo + o * i].view(o, i)[:, :K]
+        pitch = capi.bf16_pitch(K) if dtype == torch.bfloat16 else (K + 31) // 32 * 32
 
-    def _packed16(self, li, K):
-        """(copy, pitch): W[:, :K] of layer li in BF16 (rounded to nearest even), row pitch capi.bf16_pitch(K), rebuilt once per weight version
-        (AC_Args.gemm_impl = 2: the first layers' operand)."""
-        return self._cached(("pack16", li), self._packed16_build(li, K)), capi.bf16_pitch(K)
-
-    def _packed16_build(self, li, K):
-        wo, bo, o, i = self.specs[li]
-        W = self.flat[wo:wo + o * i]
-        KPk = capi.bf16_pitch(K)
-
-        def build(old):
-            dst = old if old is not None else _empty(o, KPk, device=W.device, dtype=torch.bfloat16)[:, :K]
-            capi.check(capi.lib().go1_convert_bf16(W.data_ptr(), i, capi.ptr(dst), KPk, o, K, capi.stream_ptr()), "convert_bf16")
+        def build(old, pairs=None):
+            dst = old if old is not None else _empty(o, pitch, device=W.device, dtype=dtype)[:, :K]
+            if dtype != torch.bfloat16:
+                return dst.copy_(W)
+            if pairs is None:
+                return _to_bf16(W, dst)
+            pairs.append((dst, W))
             return dst
         return build
 
     def packed16_pairs(self):
-        """The (dst, src) conversions that bring the BF16 weight copies of layers 1.. (the MN-major B operands of backward_bf16's dgrads)
-        up to the current weight version.  Their cache entries are marked current here; the caller launches the conversions
+        """The (dst, src) conversions that bring the BF16 weight copies of layers 1.. (the MN-major B operands of the AC_Args.bf16_backward
+        dgrads) up to the current weight version.  Their cache entries are marked current here; the caller launches the conversions
         (ActorCritic._convert_outputs: in the one launch that also makes the output copies, instead of one launch per layer)."""
-        ver, pairs = self.owner.weights_version, []
+        pairs = []
         for li in range(1, len(self.specs)):
-            key = ("pack16", li)
-            hit = self._cache.get(key)
-            if hit is None or hit[0] != ver:
-                wo, bo, o, i = self.specs[li]
-                dst = hit[1] if hit is not None else _empty(o, capi.bf16_pitch(i), device=self.flat.device, dtype=torch.bfloat16)[:, :i]
-                pairs.append((dst, self.flat[wo:wo + o * i].view(o, i)))
-                self._cache[key] = (ver, dst, self._packed16_build(li, i))
+            i = self.specs[li][3]
+            self._cached((li, i, torch.bfloat16), self._packer(li, i, torch.bfloat16), pairs)
         return pairs
 
     def _weight_tma(self, li):
@@ -173,16 +172,18 @@ class _Net:
         W = self.flat[wo:wo + o * i]
         return (W, i) if self._tma_ok(W, i) else self._packed(li, i)
 
-    def _cached(self, key, build):
-        """A packed copy of weights, rebuilt when the weights changed (weights_version).  The entry keeps its builder so that
-        ActorCritic.ensure_packed() can refresh every copy eagerly before a CUDA graph that reads them is replayed: the graphs contain
-        no packing kernels (the rollout replays one 24 times per weight version)."""
+    def _cached(self, key, build, pairs=None):
+        """A packed copy of weights, keyed by (layer, K, dtype), rebuilt when the weights changed (weights_version).  The entry keeps its
+        builder so that ActorCritic.ensure_packed() can refresh every copy eagerly before a CUDA graph that reads them is replayed: the
+        graphs contain no packing kernels (the rollout replays one 24 times per weight version).  pairs: passed to the builder (_packer),
+        which defers its BF16 conversion there."""
         ver = self.owner.weights_version
         hit = self._cache.get(key)
         if hit is None or hit[0] != ver:
             if torch.cuda.is_current_stream_capturing():
                 raise capi.Go1Error("stale packed weights during graph capture: call ActorCritic.ensure_packed() first")
-            hit = (ver, build(hit[1] if hit else None), build)
+            old = hit[1] if hit else None
+            hit = (ver, build(old) if pairs is None else build(old, pairs), build)
             self._cache[key] = hit
         return hit[1]
 
@@ -196,10 +197,11 @@ class _Net:
     def _p(x):
         return x.data_ptr() if torch.is_tensor(x) else x
 
-    def _gemm(self, ta, tb, M, N, K, A, lda, B, ldb, Cm, ldc, bias=None, act=0, acc=0, impl=0, extra=None, w_extra=0, ld_w_extra=0, dact_y=None, lead_cols=0,
-              colsum=None, bwd_extra=None, store_transposed=0, bf16=False, out16=None, mn=False):
-        """go1_gemm_ex (impl 0 / 1), or go1_gemm_bf16_ex with bf16: A and B BF16.  out16: a BF16 tensor that receives the transposed result
-        (store_transposed) in place of Cm.  mn: go1_gemm_bf16_mn (BF16 operands in either major; a BF16 Cm is stored row-major in BF16)."""
+    def _gemm(self, ta, tb, M, N, K, A, lda, B, ldb, Cm, ldc, impl=1, *, bias=None, act=0, acc=0, extra=None, w_extra=0, ld_w_extra=0, dact_y=None,
+              lead_cols=0, colsum=None, bwd_extra=None, store_transposed=0, out16=None):
+        """The entry point follows the operands: fp32 A and B -> go1_gemm_ex (impl 0 / 1); BF16 A and B, both K-major -> go1_gemm_bf16_ex;
+        BF16 in any other major -> go1_gemm_bf16_mn (a BF16 Cm is stored row-major in BF16).  out16: a BF16 tensor that receives the
+        transposed result (store_transposed) in place of Cm."""
         ep = self._ep
         ep.out_bf16, ep.ld_out_bf16 = (out16.data_ptr(), out16.stride(0)) if out16 is not None else (None, 0)
         ep.lead_cols = lead_cols
@@ -222,13 +224,14 @@ class _Net:
             ep.dact_y, ep.ld_dact_y = dact_y.data_ptr(), dact_y.stride(0)
         else:
             ep.dact_y = None
-        if mn:
-            c16 = 1 if torch.is_tensor(Cm) and Cm.dtype == torch.bfloat16 else 0
-            capi.check(capi.lib().go1_gemm_bf16_mn(ta, tb, M, N, K, self._p(A), lda, self._p(B), ldb, self._p(Cm), ldc, c16, ep, capi.stream_ptr()), "go1_gemm_bf16_mn")
-        elif bf16:
-            capi.check(capi.lib().go1_gemm_bf16_ex(ta, tb, M, N, K, self._p(A), lda, self._p(B), ldb, self._p(Cm), ldc, ep, capi.stream_ptr()), "go1_gemm_bf16")
+        L, args = capi.lib(), (ta, tb, M, N, K, A.data_ptr(), lda, self._p(B), ldb, self._p(Cm), ldc)
+        if A.dtype != torch.bfloat16:
+            capi.check(L.go1_gemm_ex(*args, ep, impl, capi.stream_ptr()), "go1_gemm")
+        elif (ta, tb) == (0, 1):
+            capi.check(L.go1_gemm_bf16_ex(*args, ep, capi.stream_ptr()), "go1_gemm_bf16")
         else:
-            capi.check(capi.lib().go1_gemm_ex(ta, tb, M, N, K, self._p(A), lda, self._p(B), ldb, self._p(Cm), ldc, ep, impl, capi.stream_ptr()), "go1_gemm")
+            c16 = 1 if torch.is_tensor(Cm) and Cm.dtype == torch.bfloat16 else 0
+            capi.check(L.go1_gemm_bf16_mn(*args, c16, ep, capi.stream_ptr()), "go1_gemm_bf16_mn")
 
     @staticmethod
     def _tma_ok(x, ld):
@@ -266,21 +269,20 @@ class _Net:
                 raise capi.Go1Error("BF16 observation histories are the input of AC_Args.gemm_impl = 2 only")
             tc = impl >= 1 and self._tma_ok(inp, ld_in)
             if bf16:
-                Wm, ldw = self._packed16(li, K)
+                Wm, ldw = self._packed(li, K, torch.bfloat16)
             elif tc and (not self._tma_ok(W, i) or (li == 0 and K >= 1024 and i % 32 != 0)):
                 # for the long first-layer rows the packed copy's aligned pitch alone is worth 30 % (misaligned 128-byte box rows cost an
                 # extra L2 sector each)
                 Wm, ldw = self._packed(li, K)
             ldy = y.stride(0)
             if first_extra and i - K0 > 4:      # wide trailing input: y = x W[:, :K0]^T + b, then y = act(y + extra W[:, K0:]^T)
-                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, ldy, b, 0, 0, 1 if tc else 0, bf16=bf16)
+                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, ldy, 1 if tc else 0, bias=b)
                 capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(y), ldy, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i, M, o, i - K0,
                                                             capi.act_arg(self.kind, act), capi.stream_ptr()), "go1_mlp_extra_forward")
             elif first_extra:   # y = act(x W[:, :K0]^T + extra W[:, K0:]^T + b): the (at most 4) trailing columns ride in the epilogue
-                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, ldy, b, act, 0, 1 if tc else 0, extra=extra, w_extra=W.data_ptr() + 4 * K0, ld_w_extra=i,
-                           bf16=bf16)
+                self._gemm(0, 1, M, o, K0, inp, ld_in, Wm, ldw, y, ldy, 1 if tc else 0, bias=b, act=act, extra=extra, w_extra=W.data_ptr() + 4 * K0, ld_w_extra=i)
             else:
-                self._gemm(0, 1, M, o, K, inp, ld_in, Wm, ldw, y, ldy, b, act, 0, 1 if tc else 0, bf16=bf16)
+                self._gemm(0, 1, M, o, K, inp, ld_in, Wm, ldw, y, ldy, 1 if tc else 0, bias=b, act=act)
             outs.append(y)
             inp, ld_in = y, y.stride(0)
         return outs
@@ -324,7 +326,7 @@ class _Net:
         capi.check(capi.lib().go1_mlp_tail_forward_grouped(arr, 1, M, k1, n2, n3, capi.stream_ptr()), "go1_mlp_tail_forward")
         return outs
 
-    def backward(self, x, ldx, K0, extra, outs, dout, M, impl, want_dextra=False, tag="a", dz1T=None, wgrads=None):
+    def backward(self, x, ldx, K0, extra, outs, dout, M, impl, want_dextra=False, tag="a", dz1T=None, wgrads=None, y16=None):
         """dout: gradient w.r.t. the network output [M][out] (the last layer has no activation).  Adds the weight and bias gradients into
         the flat grad buffer, which the caller has zeroed (ActorCritic.backward_ppo / backward_adaptation): split-K partial tiles and the
         bias gradients reduced in epilogues are atomic sums.  dz of every hidden layer comes out of the dgrad GEMM already multiplied by
@@ -333,13 +335,20 @@ class _Net:
         gradient and trailing-input weight gradients are left to the caller (ActorCritic._first_layer_wgrad: augmented rows of the
         transposed input).  A BF16 dz1T (AC_Args.gemm_impl = 2) receives the rounded dz; the bias, d(extra) and trailing-input reductions
         see the fp32 values.  wgrads: optional list that collects the tensor-core wgrads instead of launching them (ActorCritic._flush_wgrads
-        launches equal shapes as grouped products).  Returns d(extra) [M][E] if requested."""
+        launches equal shapes as grouped products).  Returns d(extra) [M][E] if requested.
+
+        y16 (AC_Args.bf16_backward, M >= 64, with a BF16 dz1T): {layer: BF16 copy of outs[layer]} for the layers bf16_inputs lists
+        (ActorCritic._convert_outputs).  Hidden-layer dz is then held in BF16: the head gradient is converted once the head's fp32 skinny
+        kernels have read it (unless _skinny_head_dgrad), every dgrad behind it reads the BF16 copy of W (_packed) MN-major, multiplies by
+        f'(y) from the fp32 saved output, reduces the bias gradient from the fp32 values and rounds the stored dz, and the weight
+        gradients of the layers in y16 read the BF16 dz and layer input, both MN-major."""
         L, st = capi.lib(), capi.stream_ptr()
+        n = len(self.specs)
         dz, dextra = dout, None
         bias_done = False      # this layer's bias gradient was reduced by the dgrad that made its dz, or is left to the caller
         extra_done = False     # likewise the first layer's trailing-input gradients
         dz1T16 = None          # a BF16 dz1T filled from the fp32 dz once go1_mlp_extra_backward has read that
-        for li in range(len(self.specs) - 1, -1, -1):
+        for li in range(n - 1, -1, -1):
             wo, bo, o, i = self.specs[li]
             W = self.flat[wo:wo + o * i]
             gW, gb = self.grad[wo:wo + o * i], self.grad[bo:bo + o]
@@ -349,14 +358,16 @@ class _Net:
             else:
                 inp, ld_in, K = outs[li - 1], outs[li - 1].stride(0), i
             wgrad_done = li == 0 and dz1T is not None       # made by the caller
-            if impl >= 1 and M >= 64 and not self._tma_ok(dz, ldz) and (o > 16 or (li == 1 and dz1T is not None)):
+            if y16 is None and impl >= 1 and M >= 64 and not self._tma_ok(dz, ldz) and (o > 16 or (li == 1 and dz1T is not None)):
                 # a head gradient whose rows TMA cannot read ([M][1] values, [M][E] latents) where a tensor-core product must read it: the
                 # wgrad and dgrad of a head wider than the skinny kernels take, or a one-hidden-layer net's dgrad that stores the first-layer
                 # dz transposed
                 dzp = self._buf((tag, "dhead"), M, o, capi.row_pitch(o))
                 dzp.copy_(dz)
                 dz, ldz = dzp, dzp.stride(0)
-            skinny = not wgrad_done and o <= 16              # the narrow layers (heads): one bandwidth-bound pass instead of a padded GEMM tile
+            # the narrow layers (heads): one bandwidth-bound pass instead of a padded GEMM tile; with y16 the layers listed there take
+            # their wgrad on BF16 tensor cores whatever their width
+            skinny = not wgrad_done and (o <= 16 if y16 is None else li - 1 not in y16)
             # ---- 1. bias gradient: reduced by the dgrad that made dz, by the skinny wgrad, or by go1_colsum
             if not bias_done:
                 if skinny and K % 4 == 0 and self._tma_ok(inp, ld_in):
@@ -366,16 +377,22 @@ class _Net:
                 else:
                     capi.check(L.go1_colsum(capi.ptr(dz), ldz, capi.ptr(gb), M, o, 0, st), "colsum")
             # ---- 2. wgrad: dW[o][K] = dz^T[o][M] inp[M][K]
-            if wgrad_done:
-                pass
-            elif skinny:
+            if skinny and not wgrad_done:
                 capi.check(L.go1_skinny_wgrad(capi.ptr(dz), ldz, capi.ptr(inp), ld_in, gW.data_ptr(), i, M, o, K, 1, st), "skinny_wgrad")
-            else:       # impl 1: both operands MN-major, read in place by the wgmma kernel; split-K partial tiles add into the zeroed gradient
+                wgrad_done = True
+            if y16 is not None and li == n - 1 and not self._skinny_head_dgrad(li, True):
+                # the BF16 head gradient of the tensor-core products, once the fp32 kernels have read the fp32 one
+                dz = self._buf16((tag, "dhead16"), M, o)
+                capi.convert_bf16_segments([(dz, dout)])
+                ldz = dz.stride(0)
+            if not wgrad_done:      # both operands MN-major, read in place by the wgmma kernel; split-K partial tiles add into the zeroed gradient
+                if y16 is not None:
+                    inp, ld_in = y16[li - 1], y16[li - 1].stride(0)
                 tc = impl >= 1 and M >= 64 and self._tma_ok(dz, ldz) and self._tma_ok(inp, ld_in)
                 if tc and wgrads is not None:
                     wgrads.append((o, K, M, ldz, ld_in, i, dz, inp, gW))
                 else:
-                    self._gemm(1, 0, o, K, M, dz, ldz, inp, ld_in, gW, i, None, 0, 1 if tc else 0, 1 if tc else 0)
+                    self._gemm(1, 0, o, K, M, dz, ldz, inp, ld_in, gW, i, 1 if tc else 0, acc=1 if tc else 0)
             if li == 0:
                 # trailing-input gradients the layer-2 dgrad epilogue did not reduce: d(extra) from dz in either layout, the weight
                 # gradient only from a row-major dz (a transposed one is _first_layer_wgrad's augmented product)
@@ -387,13 +404,18 @@ class _Net:
                     capi.check(L.go1_mlp_extra_backward(capi.ptr(dz), ldz, 0 if dz1T is None else 1, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, i,
                                                         gwx, i, capi.ptr(dextra) if want_dextra else None, E, M, o, E, 0, st), "extra_backward")
                 if dz1T16 is not None:
-                    capi.check(L.go1_convert_bf16(capi.ptr(dz), ldz, capi.ptr(dz1T16), dz1T16.stride(0), o, M, st), "convert_bf16")
+                    _to_bf16(dz, dz1T16)
                 return dextra
             # ---- 3. dgrad (+ fused activation derivative): dz_prev[M][i] = (dz[M][o] W[o][i]) * f'(y_prev)
             pwo, pbo, po, pi = self.specs[li - 1]
             gb_prev, yprev = self.grad[pbo:pbo + po], outs[li - 1]
             to_T = li == 1 and dz1T is not None
-            dprev = dz1T if to_T else self._hbuf((tag, "d", li - 1), M, i)
+            if to_T:
+                dprev = dz1T
+            elif y16 is not None:
+                dprev = self._buf16((tag, "d16", li - 1), M, i)
+            else:
+                dprev = self._hbuf((tag, "d", li - 1), M, i)
             out16 = None
             if to_T and dz1T.dtype == torch.bfloat16:
                 if extra is not None and pi - K0 > 4 and want_dextra:
@@ -402,10 +424,10 @@ class _Net:
                 else:
                     out16, dprev = dz1T, None
             ldp = dprev.stride(0) if dprev is not None else 0
-            if impl >= 1 and self._tma_ok(dz, ldz) and M >= 64:      # (the 12-wide actor head included: 19 us here, 22 us on the skinny pass)
-                # W read MN-major (in place, or its packed copy when its rows are not 16-byte multiples); the bias gradient of layer li-1
-                # (column sums of dprev) rides in the epilogue
-                Wd, ldwd = self._weight_tma(li)
+            if impl >= 1 and self._tma_ok(dz, ldz) and M >= 64 and not self._skinny_head_dgrad(li, y16 is not None):
+                # W read MN-major (in place, or its packed copy when its rows are not 16-byte multiples; with y16 its BF16 copy); the bias
+                # gradient of layer li-1 (column sums of dprev) rides in the epilogue
+                Wd, ldwd = self._weight_tma(li) if y16 is None else self._packed(li, i, torch.bfloat16)
                 bx = None
                 if li == 1 and extra is not None and 1 <= pi - K0 <= 4:
                     # dprev is the first layer's dz: d(extra), and the trailing-input weight gradient unless _first_layer_wgrad makes it,
@@ -416,7 +438,7 @@ class _Net:
                     gwx = None if to_T else self.grad.data_ptr() + 4 * (pwo + K0)
                     if dextra is not None or gwx is not None:
                         bx = (extra, self.flat.data_ptr() + 4 * (pwo + K0), pi, gwx, pi, dextra)
-                self._gemm(0, 0, M, i, o, dz, ldz, Wd, ldwd, dprev, ldp, None, 2, 0, 1, dact_y=yprev, colsum=None if to_T else gb_prev, bwd_extra=bx,
+                self._gemm(0, 0, M, i, o, dz, ldz, Wd, ldwd, dprev, ldp, 1, act=2, dact_y=yprev, colsum=None if to_T else gb_prev, bwd_extra=bx,
                            store_transposed=1 if to_T else 0, out16=out16)
                 bias_done = True
             elif to_T:
@@ -424,100 +446,36 @@ class _Net:
             elif o <= 16:
                 # the bias gradient of layer li-1 (column sums of dprev) is reduced in the same pass where the operands allow it
                 bias_done = impl >= 1 and i % 4 == 0 and self._tma_ok(W, i) and self._tma_ok(dprev, ldp) and self._tma_ok(yprev, yprev.stride(0))
-                capi.check(L.go1_skinny_dgrad_act(capi.ptr(dz), ldz, capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(dprev), ldp,
-                                                  gb_prev.data_ptr() if bias_done else None, M, o, i, self.kind, st), "skinny_dgrad")
+                if dprev.dtype == torch.bfloat16 and bias_done:
+                    capi.check(L.go1_skinny_dgrad_act_bf16(capi.ptr(dz), ldz, capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(dprev), ldp,
+                                                           gb_prev.data_ptr(), M, o, i, self.kind, st), "skinny_dgrad_bf16")
+                else:
+                    d32 = self._hbuf((tag, "dskinny"), M, i) if dprev.dtype == torch.bfloat16 else dprev
+                    capi.check(L.go1_skinny_dgrad_act(capi.ptr(dz), ldz, capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(d32), d32.stride(0),
+                                                      gb_prev.data_ptr() if bias_done else None, M, o, i, self.kind, st), "skinny_dgrad")
+                    if d32 is not dprev:    # rows the vector kernel cannot read: the column sums and the BF16 copy of the fp32 dz
+                        capi.check(L.go1_colsum(capi.ptr(d32), d32.stride(0), capi.ptr(gb_prev), M, i, 0, st), "colsum")
+                        capi.convert_bf16_segments([(dprev, d32)])
+                        bias_done = True
             else:
-                self._gemm(0, 0, M, i, o, dz, ldz, W, i, dprev, ldp, None, 2, 0, 0, dact_y=yprev)
+                self._gemm(0, 0, M, i, o, dz, ldz, W, i, dprev, ldp, 0, act=2, dact_y=yprev)
                 bias_done = False
             dz = dprev if dprev is not None else out16
 
+    def _skinny_head_dgrad(self, li, bf16):
+        """With BF16 hidden-layer dz (AC_Args.bf16_backward) a head of at most 16 columns in a net of more than one hidden layer takes its
+        dgrad on the skinny kernel, storing BF16: a K <= 16 tensor-core product pays for a whole 64-deep k-block and measured slower (35-45
+        us per launch at M = 24576).  At gemm_impl 1 and 2 a head whose gradient rows TMA can read takes its dgrad on the tensor cores
+        (the 12-wide actor head: 19 us there, 22 us on the skinny pass)."""
+        n = len(self.specs)
+        return bf16 and li == n - 1 and n > 2 and self.specs[li][2] <= 16
+
     def bf16_inputs(self, outs):
-        """[(layer, width)] of the hidden outputs whose BF16 copies backward_bf16 reads: the input of every weight gradient behind the first
-        layer that runs on BF16 (every hidden layer's, and the head's when it is wider than the skinny kernels' 16 columns)."""
+        """[(layer, width)] of the hidden outputs whose BF16 copies backward reads at AC_Args.bf16_backward: the input of every weight
+        gradient behind the first layer that runs on BF16 (every hidden layer's, and the head's when it is wider than the skinny kernels'
+        16 columns)."""
         n = len(self.specs)
         return [(li - 1, self.specs[li][3]) for li in range(1, n) if li < n - 1 or self.specs[li][2] > 16]
-
-    def backward_bf16(self, x, ldx, K0, extra, outs, y16, dout, M, dz1T, want_dextra=False, tag="a", wgrads=None):
-        """backward() of AC_Args.bf16_backward (M >= 64; dz1T: the BF16 transposed first-layer dz, whose wgrad the caller makes).  The head
-        gradient dout (fp32, from the loss kernels) goes through the head's fp32 skinny dgrad and that output is converted to BF16 (a head
-        wider than 16 columns: dout itself is converted and the head's products run on BF16); every dgrad behind it is a go1_gemm_bf16_mn
-        product of the BF16 dz and a BF16 copy of W (_packed16, read MN-major) whose epilogue multiplies by f'(y) from the fp32 saved output,
-        reduces the bias gradient from the fp32 values and rounds the stored dz to BF16 (row-major, or dz1T transposed).  Weight gradients behind the
-        first layer read the BF16 dz and y16[l] (the BF16 copy of outs[l], ActorCritic._convert_outputs), both MN-major; a head of at most
-        16 columns keeps its fp32 skinny kernels.  Returns d(extra) [M][E] if requested."""
-        L, st = capi.lib(), capi.stream_ptr()
-        n = len(self.specs)
-        dextra, extra_done, dz1T16 = None, False, None
-        wo, bo, o, i = self.specs[-1]
-        gW, gb = self.grad[wo:wo + o * i], self.grad[bo:bo + o]
-        inp = outs[n - 2]
-        if o <= 16:             # the head: weight and bias gradient in one fp32 pass over its input, as at gemm_impl 2
-            if i % 4 == 0 and self._tma_ok(inp, inp.stride(0)):
-                capi.check(L.go1_skinny_wgrad_ex(capi.ptr(dout), dout.stride(0), capi.ptr(inp), inp.stride(0), gW.data_ptr(), i, gb.data_ptr(), M, o, i, 1, st), "skinny_wgrad")
-            else:
-                capi.check(L.go1_colsum(capi.ptr(dout), dout.stride(0), capi.ptr(gb), M, o, 0, st), "colsum")
-                capi.check(L.go1_skinny_wgrad(capi.ptr(dout), dout.stride(0), capi.ptr(inp), inp.stride(0), gW.data_ptr(), i, M, o, i, 1, st), "skinny_wgrad")
-        else:
-            capi.check(L.go1_colsum(capi.ptr(dout), dout.stride(0), capi.ptr(gb), M, o, 0, st), "colsum")
-        if o <= 16 and n > 2:
-            # the head's dgrad on its fp32 skinny kernel, as at gemm_impl 2, storing BF16 (a K <= 16 tensor-core product pays for a whole
-            # 64-deep k-block and measured slower: 35-45 us per launch at M = 24576); the bias gradient below it from the fp32 values
-            pwo, pbo, po, pi = self.specs[n - 2]
-            W, gb_prev, yprev = self.flat[wo:wo + o * i], self.grad[pbo:pbo + po], outs[n - 2]
-            dz = self._buf16((tag, "d16", n - 2), M, i)
-            if i % 4 == 0 and self._tma_ok(W, i) and self._tma_ok(yprev, yprev.stride(0)):
-                capi.check(L.go1_skinny_dgrad_act_bf16(capi.ptr(dout), dout.stride(0), capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(dz),
-                                                       dz.stride(0), gb_prev.data_ptr(), M, o, i, self.kind, st), "skinny_dgrad_bf16")
-            else:           # rows the vector kernel cannot read: fp32 first, then its column sums and BF16 copy
-                d32 = self._hbuf((tag, "dskinny"), M, i)
-                capi.check(L.go1_skinny_dgrad_act(capi.ptr(dout), dout.stride(0), capi.ptr(W), i, capi.ptr(yprev), yprev.stride(0), capi.ptr(d32),
-                                                  d32.stride(0), None, M, o, i, self.kind, st), "skinny_dgrad")
-                capi.check(L.go1_colsum(capi.ptr(d32), d32.stride(0), capi.ptr(gb_prev), M, i, 0, st), "colsum")
-                capi.convert_bf16_segments([(dz, d32)])
-            first = n - 2
-        else:       # a head wider than 16 (or a one-hidden-layer net, whose head dgrad stores dz1T): BF16 head gradient, tensor-core products
-            dz = self._buf16((tag, "dhead16"), M, o)
-            capi.convert_bf16_segments([(dz, dout)])
-            first = n - 1
-        for li in range(first, 0, -1):
-            wo, bo, o, i = self.specs[li]
-            gW = self.grad[wo:wo + o * i]
-            if li < n - 1 or o > 16:    # wgrad dW[o][i] = dz^T y_{li-1}: both operands MN-major, split-K partial tiles add into the zeroed gradient
-                yb = y16[li - 1]
-                if wgrads is not None:
-                    wgrads.append((o, i, M, dz.stride(0), yb.stride(0), i, dz, yb, gW))
-                else:
-                    self._gemm(1, 0, o, i, M, dz, dz.stride(0), yb, yb.stride(0), gW, i, None, 0, 1, 1, mn=True)
-            # dgrad dz_prev[M][i] = (dz[M][o] W[o][i]) * f'(y_prev), W read MN-major from its BF16 copy
-            pwo, pbo, po, pi = self.specs[li - 1]
-            gb_prev, yprev = self.grad[pbo:pbo + po], outs[li - 1]
-            W16, ldw16 = self._packed16(li, i)
-            bx, out16, colsum = None, None, gb_prev
-            if li == 1:
-                colsum = None           # the first layer's bias gradient is the caller's (the augmented row of its wgrad)
-                if extra is not None and pi - K0 > 4 and want_dextra:
-                    # a wide trailing input's d(extra) is a pass over the stored dz (go1_mlp_extra_backward): fp32 first, the BF16 copy after it
-                    dz1T16, dprev = dz1T, self._buf((tag, "dz1T32"), i, M, capi.row_pitch(M))
-                else:
-                    out16, dprev = dz1T, None
-                if extra is not None and 1 <= pi - K0 <= 4 and want_dextra:
-                    extra_done = True   # d(extra) of a narrow trailing input in this epilogue
-                    dextra = self._buf((tag, "dextra"), M, pi - K0).zero_()
-                    bx = (extra, self.flat.data_ptr() + 4 * (pwo + K0), pi, None, pi, dextra)
-            else:
-                dprev = self._buf16((tag, "d16", li - 1), M, i)
-            self._gemm(0, 0, M, i, o, dz, dz.stride(0), W16, ldw16, dprev, dprev.stride(0) if dprev is not None else 0, None, 2, 0, 1, dact_y=yprev,
-                       colsum=colsum, bwd_extra=bx, store_transposed=1 if li == 1 else 0, out16=out16, mn=True)
-            dz = dprev
-        if extra is not None and not extra_done and want_dextra:
-            E = self.specs[0][3] - K0
-            dextra = self._buf((tag, "dextra"), M, E)
-            W = self.flat[self.specs[0][0]:]
-            capi.check(L.go1_mlp_extra_backward(capi.ptr(dz), dz.stride(0), 1, capi.ptr(extra), extra.stride(0), W.data_ptr() + 4 * K0, self.specs[0][3],
-                                                None, self.specs[0][3], capi.ptr(dextra), E, M, self.specs[0][2], E, 0, st), "extra_backward")
-        if dz1T16 is not None:
-            capi.check(L.go1_convert_bf16(capi.ptr(dz), dz.stride(0), capi.ptr(dz1T16), dz1T16.stride(0), self.specs[0][2], M, st), "convert_bf16")
-        return dextra
 
 
 class ActorCritic(nn.Module):
@@ -663,7 +621,7 @@ class ActorCritic(nn.Module):
         return self._impl() == 2 and bool(AC_Args.bf16_backward)
 
     def _convert_outputs(self, named_outs, M, defer=False):
-        """{net name: {layer: BF16 copy}} of the hidden outputs that the nets' backward_bf16 weight gradients read, made together with the
+        """{net name: {layer: BF16 copy}} of the hidden outputs that the nets' BF16 weight gradients read (_Net.backward's y16), made together with the
         BF16 copies of the weights their dgrads read (stale after every optimizer step) by ONE go1_convert_bf16_segments launch per
         minibatch forward (two beyond 16 matrices; named_outs: [(net name, outs)]).  defer: only the weight copies are converted here;
         returns (copies, output pairs) and the caller converts the outputs (_backward_bodies: on the side stream, beside the dgrads)."""
@@ -695,8 +653,7 @@ class ActorCritic(nn.Module):
         if self._impl() != 2 or h.dtype == torch.bfloat16:
             return h
         M, K0 = h.shape[0], self.num_obs_history
-        h16 = self._nets["adapt"]._buf16((tag, "h16"), M, K0)
-        capi.check(capi.lib().go1_convert_bf16(capi.ptr(h), h.stride(0), capi.ptr(h16), h16.stride(0), M, K0, capi.stream_ptr()), "convert_bf16")
+        h16 = _to_bf16(h, self._nets["adapt"]._buf16((tag, "h16"), M, K0))
         self.model_inputs[tag] = h16
         return h16
 
@@ -752,22 +709,18 @@ class ActorCritic(nn.Module):
                                 (x[Pa:Pa + oc], Wc[:, K0:])])
             return old
 
-        Wcat, bcat, xcat = na._cached(("l1cat", "all"), build_all)
-        bf16 = impl == 2
-        if bf16:                # the block in BF16 (rounded to nearest even; the padding rows stay zero), refreshed with the fp32 one
-            def build_all16(old):
-                W32 = na._cached(("l1cat", "all"), build_all)[0]
-                W16 = old if old is not None else _empty(NC, capi.bf16_pitch(K0), device=flat.device, dtype=torch.bfloat16)[:, :K0]
-                capi.check(capi.lib().go1_convert_bf16(capi.ptr(W32), W32.stride(0), capi.ptr(W16), W16.stride(0), NC, K0, capi.stream_ptr()), "convert_bf16")
-                return W16
-            Wcat = na._cached(("l1cat16", "all"), build_all16)
+        Wcat, bcat, xcat = na._cached(("l1cat", K0, torch.float32), build_all)
+        if impl == 2:           # the block in BF16 (rounded to nearest even; the padding rows stay zero), refreshed with the fp32 one
+            Wcat = na._cached(("l1cat", K0, torch.bfloat16), lambda old: _to_bf16(
+                na._cached(("l1cat", K0, torch.float32), build_all)[0],
+                old if old is not None else _empty(NC, capi.bf16_pitch(K0), device=flat.device, dtype=torch.bfloat16)[:, :K0]))
         y = na._buf((tag, "y1cat"), M, NC)
         ya, yc, yp = y[:, :oa], y[:, Pa:Pa + oc], y[:, Pa + Pc:Pa + Pc + op]
         if E <= 4:
-            na._gemm(0, 1, M, NC, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1,
-                     extra=priv, w_extra=xcat.data_ptr(), ld_w_extra=E, lead_cols=Pa + Pc, bf16=bf16)
+            na._gemm(0, 1, M, NC, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bias=bcat, act=1,
+                     extra=priv, w_extra=xcat.data_ptr(), ld_w_extra=E, lead_cols=Pa + Pc)
         else:       # wide privileged input: only the adaptation slice is finished in the epilogue; the critic slice gets priv here
-            na._gemm(0, 1, M, NC, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bcat, 1, 0, 1, lead_cols=Pa, bf16=bf16)
+            na._gemm(0, 1, M, NC, K0, h, h.stride(0), Wcat, Wcat.stride(0), y, y.stride(0), bias=bcat, act=1, lead_cols=Pa)
             capi.check(capi.lib().go1_mlp_extra_forward(capi.ptr(yc), yc.stride(0), capi.ptr(priv), priv.stride(0), Wc.data_ptr() + 4 * K0, K0 + E,
                                                         M, oc, E, capi.act_arg(self.act_kind, 1), capi.stream_ptr()), "go1_mlp_extra_forward")
         ts = npol.tail_start
@@ -932,7 +885,7 @@ class ActorCritic(nn.Module):
         KP = (KA + 31) // 32 * 32
         n0 = nets["adapt"]
         gcat = n0._buf((tag, "gWcat"), dz1T.shape[0], KP)
-        n0._gemm(0, 1, dz1T.shape[0], KA, M, dz1T, dz1T.stride(0), hT, hT.stride(0), gcat, KP, None, 0, 0, 1, bf16=dz1T.dtype == torch.bfloat16)
+        n0._gemm(0, 1, dz1T.shape[0], KA, M, dz1T, dz1T.stride(0), hT, hT.stride(0), gcat, KP)
         row, pairs = 0, []
         for name in names:
             xcol = {"adapt": None, "actor": K0 + 1 + E, "critic": K0 + 1}[name]
@@ -945,38 +898,34 @@ class ActorCritic(nn.Module):
             row += o
         capi.copy_segments(pairs)
 
+    def _kmajor_buf(self, key, rows, M):
+        """A [rows][M] K-major operand of the first layers' weight-gradient product: BF16 at AC_Args.gemm_impl = 2 (row pitch
+        capi.bf16_pitch(M)), else fp32 (128-byte aligned rows)."""
+        if self._impl() == 2:
+            return self._nets["adapt"]._buf16(key, rows, M)
+        return self._nets["adapt"]._buf(key, rows, M, (M + 31) // 32 * 32)
+
     def backward_ppo(self, h, priv, dmean, dvalue, dstd, hT=None):
         """Gradients of the PPO loss into flat_grads[HEAD:] (overwrites; the loss scalars in the head are left alone). h/priv are the
         minibatch inputs of the forward pass just run with tag='train'; dmean [M,A], dvalue [M,1], dstd [A].
-        hT: history_kmajor(h, priv) if the caller keeps one (RolloutStorage builds it once per update; at AC_Args.gemm_impl = 2
-        history_kmajor_bf16 of the BF16 history); built here otherwise.  Its latent rows are written here."""
+        hT: history_kmajor(h, priv) if the caller keeps one (RolloutStorage builds it once per update; BF16 at AC_Args.gemm_impl = 2,
+        from the BF16 history); built here otherwise.  Its latent rows are written here."""
         M, K0 = h.shape[0], self.num_obs_history
         nets = self._nets
-        bf16 = self._impl() == 2
         self._grad[self.HEAD:].zero_()      # one fill; every kernel below adds into it (atomics in the epilogues and split-K products)
-        if self._first_layers_fusable(h, priv) and bf16:
-            # the BF16 history products: dz1 stored in BF16 by the layer-2 dgrads, the wgrad over the BF16 hT
-            oa, op, oc = nets["adapt"].specs[0][2], nets["actor"].specs[0][2], nets["critic"].specs[0][2]
-            E = self.num_privileged_obs
-            if hT is None:
-                hT = history_kmajor_bf16(self._model_input(h, "train"), priv, nets["adapt"]._buf16(("train", "hT16"), K0 + 1 + 2 * E, M))
-            capi.check(capi.lib().go1_transpose_to_bf16(capi.ptr(self._latent), self._latent.stride(0), capi.ptr(hT[K0 + 1 + E:]), hT.stride(0), M, E,
-                                                        capi.stream_ptr()), "transpose_to_bf16")
-            dz1 = nets["adapt"]._buf(("train", "dz1catT16"), oa + op + oc, M, hT.stride(0), torch.bfloat16)
-            y16 = self._convert_outputs((("adapt", self._a_out), ("actor", self._p_out), ("critic", self._c_out)), M, defer=True) if self._bf16_backward() else None
-            self._backward_bodies(h, priv, dmean, dvalue, dz1, oa, op, M, K0, y16)
-            self._first_layer_wgrad(("adapt", "actor", "critic"), dz1, hT, M, "train")
-        elif self._first_layers_fusable(h, priv):
+        if self._first_layers_fusable(h, priv):
             # the three first layers share their input: ONE transposed dz [o_a+o_p+o_c][M] (each net's layer-2 dgrad stores its
-            # first-layer dz into its row slice) and ONE tensor-core wgrad with K-major operands (_first_layer_wgrad)
+            # first-layer dz into its row slice) and ONE tensor-core wgrad with K-major operands (_first_layer_wgrad); at gemm_impl 2
+            # both operands are BF16, the dz rounded by the dgrads that store it
             oa, op, oc = nets["adapt"].specs[0][2], nets["actor"].specs[0][2], nets["critic"].specs[0][2]
             E = self.num_privileged_obs
             if hT is None:
-                hT = history_kmajor(h, priv, nets["adapt"]._buf(("train", "hT"), K0 + 1 + 2 * E, (M + 31) // 32 * 32))
-            L, st = capi.lib(), capi.stream_ptr()
-            capi.check(L.go1_transpose(capi.ptr(self._latent), self._latent.stride(0), capi.ptr(hT[K0 + 1 + E:]), hT.stride(0), M, E, st), "transpose")
-            dz1 = nets["adapt"]._buf(("train", "dz1catT"), oa + op + oc, hT.stride(0))
-            self._backward_bodies(h, priv, dmean, dvalue, dz1, oa, op, M, K0)
+                hT = history_kmajor(self._model_input(h, "train"), priv, self._kmajor_buf(("train", "hT"), K0 + 1 + 2 * E, M))
+            _transpose(self._latent, hT[K0 + 1 + E:])
+            dz1 = nets["adapt"]._buf(("train", "dz1catT"), oa + op + oc, M, hT.stride(0), hT.dtype)
+            named_outs = (("adapt", self._a_out), ("actor", self._p_out), ("critic", self._c_out))
+            y16, ypairs = self._convert_outputs(named_outs, M, defer=True) if self._bf16_backward() else ({}, [])
+            self._backward_bodies(h, priv, dmean, dvalue, dz1, oa, op, M, K0, y16, ypairs)
             self._first_layer_wgrad(("adapt", "actor", "critic"), dz1, hT, M, "train")
         else:
             impl = self._impl()
@@ -987,35 +936,31 @@ class ActorCritic(nn.Module):
             nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, impl, tag="train")
         self._grad[self.std_offset:self.std_offset + self.num_actions].copy_(dstd)
 
-    def _backward_bodies(self, h, priv, dmean, dvalue, dz1, oa, op, M, K0, y16=None):
+    def _backward_bodies(self, h, priv, dmean, dvalue, dz1, oa, op, M, K0, y16, ypairs):
         """The three nets' backward passes down to their first-layer dz, stored transposed into the row slices of dz1 ([adapt | actor |
-        critic] x M), and the tensor-core wgrads behind the first layers, launched as grouped products once all dz exist.  y16: (the BF16
-        output copies of AC_Args.bf16_backward, the conversions that make them) from _convert_outputs(defer=True): the nets run
-        backward_bf16.  Only those grouped wgrads read the copies, so the conversion runs first on the critic's side stream, beside the
-        actor and adaptation dgrads (measured 2.2 ms of the 35 ms of kernel time of an update at 4096 envs, bandwidth-bound)."""
-        nets, impl = self._nets, 1
-        wgrads = []
-        ypairs = []
-        if y16 is not None:
-            y16, ypairs = y16
+        critic] x M), and the tensor-core wgrads behind the first layers, launched as grouped products once all dz exist.  y16, ypairs:
+        AC_Args.bf16_backward's {net name: BF16 output copies} and the conversions that make them (_convert_outputs(defer=True)), else
+        empty.  Only the grouped wgrads read the copies, so the conversion runs first on the critic's side stream, beside the actor and
+        adaptation dgrads (measured 2.2 ms of the 35 ms of kernel time of an update at 4096 envs, bandwidth-bound)."""
+        nets, wgrads = self._nets, []
 
-        def bwd(name, extra, outs, dout, dz1T, want_dextra=False):
-            if y16 is not None:
-                return nets[name].backward_bf16(h, h.stride(0), K0, extra, outs, y16[name], dout, M, dz1T, want_dextra=want_dextra, tag="train", wgrads=wgrads)
-            return nets[name].backward(h, h.stride(0), K0, extra, outs, dout, M, impl, want_dextra=want_dextra, tag="train", dz1T=dz1T, wgrads=wgrads)
+        def critic():
+            nets["critic"].backward(h, h.stride(0), K0, priv, self._c_out, dvalue, M, 1, tag="train", dz1T=dz1[oa + op:], wgrads=wgrads,
+                                    y16=y16.get("critic"))
         side = self._side_stream(M)
         if side is not None:    # critic chain beside actor -> adaptation chain
             self._fork(side)
             with torch.cuda.stream(side):
                 if ypairs:
                     capi.convert_bf16_segments(ypairs)
-                bwd("critic", priv, self._c_out, dvalue, dz1[oa + op:])
+                critic()
         elif ypairs:
             capi.convert_bf16_segments(ypairs)
-        dlat = bwd("actor", self._latent, self._p_out, dmean, dz1[oa:oa + op], want_dextra=True)
+        dlat = nets["actor"].backward(h, h.stride(0), K0, self._latent, self._p_out, dmean, M, 1, want_dextra=True, tag="train", dz1T=dz1[oa:oa + op],
+                                      wgrads=wgrads, y16=y16.get("actor"))
         if side is None:
-            bwd("critic", priv, self._c_out, dvalue, dz1[oa + op:])
-        bwd("adapt", None, self._a_out, dlat, dz1[:oa])
+            critic()
+        nets["adapt"].backward(h, h.stride(0), K0, None, self._a_out, dlat, M, 1, tag="train", dz1T=dz1[:oa], wgrads=wgrads, y16=y16.get("adapt"))
         if side is not None:
             self._join(side)
         self._flush_wgrads(wgrads)
@@ -1027,21 +972,11 @@ class ActorCritic(nn.Module):
         net = self._nets["adapt"]
         self._grad[self.HEAD:self.n_adapt_params].zero_()
         if self._impl() >= 1 and M >= 64 and _Net._tma_ok(h, h.stride(0)) and net.specs[0][3] == K0:
-            oa = net.specs[0][2]
-            if self._impl() == 2:
-                if hT is None:
-                    hT = history_kmajor_bf16(self._model_input(h, "adapt"), None, net._buf16(("adapt", "hT16"), K0 + 1, M))
-                dz1 = net._buf(("adapt", "dz1T16"), oa, M, hT.stride(0), torch.bfloat16)
-                if self._bf16_backward():
-                    y16 = self._convert_outputs((("adapt", outs),), M)["adapt"]
-                    net.backward_bf16(h, h.stride(0), K0, None, outs, y16, dpred, M, dz1, tag="adapt")
-                    self._first_layer_wgrad(("adapt",), dz1, hT[:K0 + 1], M, "adapt")
-                    return
-            else:
-                if hT is None:
-                    hT = history_kmajor(h, None, net._buf(("adapt", "hT"), K0 + 1, (M + 31) // 32 * 32))
-                dz1 = net._buf(("adapt", "dz1T"), oa, hT.stride(0))
-            net.backward(h, h.stride(0), K0, None, outs, dpred, M, 1, tag="adapt", dz1T=dz1)
+            if hT is None:
+                hT = history_kmajor(self._model_input(h, "adapt"), None, self._kmajor_buf(("adapt", "hT"), K0 + 1, M))
+            dz1 = net._buf(("adapt", "dz1T"), net.specs[0][2], M, hT.stride(0), hT.dtype)
+            y16 = self._convert_outputs((("adapt", outs),), M)["adapt"] if self._bf16_backward() else None
+            net.backward(h, h.stride(0), K0, None, outs, dpred, M, 1, tag="adapt", dz1T=dz1, y16=y16)
             self._first_layer_wgrad(("adapt",), dz1, hT[:K0 + 1], M, "adapt")
         else:
             if h.dtype == torch.bfloat16:      # (fewer than 64 rows: CUDA-core products, as at impl 1) the rounded history, exactly in fp32

@@ -3,7 +3,7 @@ GAE through the warp-scan kernel, minibatches through the row-gather kernel."""
 import torch
 
 from go1_b200 import capi
-from .actor_critic import AC_Args, history_kmajor, history_kmajor_bf16
+from .actor_critic import AC_Args, history_kmajor
 
 
 class RolloutStorage:
@@ -165,14 +165,19 @@ class RolloutStorage:
         w = flat.shape[1]
         ldd = ldd or w
         if out is None and key is not None:
-            cache = self.__dict__.setdefault("_gather_bufs", {})
-            out = cache.get(key)
-            if out is None or out.shape != (idx.shape[0], ldd):
-                out = cache[key] = torch.empty(idx.shape[0], ldd, device=flat.device)
+            out = self._buffer(key, (idx.shape[0], ldd), torch.float32)
         if out is None:
             out = torch.empty(idx.shape[0], ldd, device=flat.device)
         capi.check(capi.lib().go1_gather_rows(capi.ptr(flat), capi.ptr(idx), capi.ptr(out), idx.shape[0], w, ldd, capi.stream_ptr()), "gather")
         return out if ldd == w else out[:, :w]
+
+    def _buffer(self, key, shape, dtype):
+        """A destination buffer kept across updates (reallocated when the minibatch shape changes)."""
+        cache = self.__dict__.setdefault("_gather_bufs", {})
+        out = cache.get(key)
+        if out is None or out.shape != shape or out.dtype != dtype:
+            out = cache[key] = torch.empty(*shape, device=self.device, dtype=dtype)
+        return out
 
     def mini_batch_generator(self, num_mini_batches, num_epochs=8, indices=None):
         batch_size = self.num_envs * self.num_transitions_per_env
@@ -189,28 +194,19 @@ class RolloutStorage:
                 idx = indices[i * mini_batch_size:(i + 1) * mini_batch_size].contiguous()
                 obs = self.gather(self.observations, idx)
                 priv_b = self.gather(self.privileged_observations, idx)
-                cache = self.__dict__.setdefault("_gather_bufs", {})
-                K0, P = self.observation_histories.shape[-1], priv_b.shape[1]
-                if bf16:    # AC_Args.gemm_impl = 2: the minibatch history (copied from the BF16 slab) and its K-major copy in BF16
-                    M = idx.shape[0]
-                    shapes = {("hist16", i): (M, capi.bf16_pitch(K0)), ("histT16", i): (K0 + 1 + 2 * P, capi.bf16_pitch(M))}
-                    for k, shp in shapes.items():
-                        if k not in cache or cache[k].shape != shp:
-                            cache[k] = torch.empty(*shp, device=self.device, dtype=torch.bfloat16)
-                    hist_b = cache[("hist16", i)][:, :K0]
+                K0, P, M = self.observation_histories.shape[-1], priv_b.shape[1], idx.shape[0]
+                if bf16:    # AC_Args.gemm_impl = 2: the minibatch history, copied from the BF16 slab, and its K-major copy in BF16
+                    hist_b = self._buffer(("hist16", i), (M, capi.bf16_pitch(K0)), torch.bfloat16)[:, :K0]
+                    kmajor = (K0 + 1 + 2 * P, capi.bf16_pitch(M)), torch.bfloat16
                     capi.check(capi.lib().go1_gather_rows_bf16(capi.ptr(self._hist_slab), self.hist_row_pitch, capi.ptr(idx), capi.ptr(hist_b),
                                                                hist_b.stride(0), M, K0, capi.stream_ptr()), "gather_rows_bf16")
-                    hist_b.hT = history_kmajor_bf16(hist_b, priv_b, cache[("histT16", i)])
                 else:
                     # whole slab rows: go1_gather_rows reads its source at a row pitch equal to the width it copies
                     hist_b = self.gather(self._hist_slab, idx, key=("hist", i), ldd=self.hist_pitch)[:, :K0]
-                    # its K-major transpose [history | 1 | priv | latent rows] for the first layers' weight-gradient products, built once per
-                    # update and read by every epoch (ActorCritic.backward_ppo / backward_adaptation); 830 MB for 4 minibatches at 4096 envs
-                    M = hist_b.shape[0]
-                    hT = cache.get(("histT", i))
-                    if hT is None or hT.shape != (K0 + 1 + 2 * P, (M + 31) // 32 * 32):
-                        hT = cache[("histT", i)] = torch.empty(K0 + 1 + 2 * P, (M + 31) // 32 * 32, device=hist_b.device)
-                    hist_b.hT = history_kmajor(hist_b, priv_b, hT)
+                    kmajor = (K0 + 1 + 2 * P, (M + 31) // 32 * 32), torch.float32
+                # its K-major transpose [history | 1 | priv | latent rows] for the first layers' weight-gradient products, built once per
+                # update and read by every epoch (ActorCritic.backward_ppo / backward_adaptation); 830 MB for 4 minibatches at 4096 envs in fp32
+                hist_b.hT = history_kmajor(hist_b, priv_b, self._buffer(("histT", i), *kmajor))
                 yield (obs, obs, priv_b, hist_b,
                        self.gather(self.actions, idx), self.gather(self.values, idx), self.gather(self.advantages, idx),
                        self.gather(self.returns, idx), self.gather(self.actions_log_prob, idx), self.gather(self.mu, idx),
