@@ -264,6 +264,20 @@ int go1_curriculum_pack(Go1Sim* sim, const Go1CurriculumConfig* cfg, const Go1Cu
  * category after the other.  Same arithmetic either way. */
 void go1_curriculum_set_grouped(int on);
 
+/* Deterministic learner (AC_Args.deterministic).  1: every learner entry point launched from then on sums its cross-CTA reductions
+ * (split-K partial tiles, column sums, trailing-input terms, loss / statistics scalars, weight gradients of the narrow layers) in a
+ * fixed order: per-CTA partials are stored to a workspace with plain stores and added up by a separate launch, so identical inputs
+ * give bit-identical outputs on the same build, GPU model and launch configuration.  0 (default): the atomics of the default mode.
+ * The mode is library-wide and read at launch; the workspace is one buffer per stream, grown outside CUDA graph capture only (a
+ * launch that needs more during capture fails) and never freed, so captured graphs keep valid pointers. */
+void go1_set_deterministic(int on);
+int go1_deterministic(void);
+/* Bytes held by the deterministic-mode workspaces of all streams. */
+int64_t go1_deterministic_workspace_bytes(void);
+/* Grows the workspace of `stream` to the size of the largest one: called before a CUDA graph is captured on a stream of its own, after the
+ * captured work ran eagerly on another stream (the capture then finds the workspace it needs). */
+int go1_deterministic_reserve(void* stream);
+
 /* go1_sim_reset_idx with the env count read from device memory (*k_dev <= num_envs) and an optional per-call
  * accumulator for extras["train/episode"] (NULL = the bound episode_acc). */
 int go1_sim_reset_idx_dev(Go1Sim* sim, const int32_t* env_ids, const int32_t* k_dev, const float* new_commands,

@@ -35,6 +35,7 @@
 #include "../../include/go1_b200.h"
 #include "wgmma_tf32.cuh"
 #include "activation.cuh"
+#include "deterministic.cuh"
 
 extern int go1_set_error(const char* m);
 void go1_count_launch(int n);
@@ -152,6 +153,13 @@ struct GemmArgs {
     float* Cg[4]; int nprob, tiles_per_prob;
 };
 constexpr int GEMM_MAXP = 4;
+// Deterministic mode (go1_set_deterministic): where the plain kernels add into their targets with atomics, the DET instantiations store
+// partials to the stream's workspace and go1_det_sum adds them in a fixed order:
+//   split    [problem][split][M][ldc]  the split-K partial tiles (slab = M x ldc floats)
+//   cs       [M / 32][N]               colsum: the column sums of each 32-row block
+//   gwx      [M / 32][N][nbx]          the trailing-input weight gradient of each 32-row block
+//   dx       [N / 32][M][nbx]          the trailing-input gradient of each 32-column chunk
+struct DetArgs { float* split; size_t slab; int nsplit; float* cs; float* gwx; float* dx; };
 // half: the 64-row box of the operand a CTA pair shares (cluster launches: see gemm_tf32_wgmma)
 struct GemmMaps { CUtensorMap a[GEMM_MAXP], b[GEMM_MAXP], half; };
 
@@ -221,13 +229,29 @@ __device__ __forceinline__ float transpose_reduce32(float (&sred)[32], const int
 // Epilogue of one 32-column chunk held in registers (thread = output row, r[j] = column col0 + j).  Called by all 32 lanes
 // of an epilogue warp (the per-column operands -- bias, extra-input weights -- are loaded once per lane and broadcast
 // with shuffles instead of 32 x per-thread global loads, which made the rank-2 term the slowest part of the kernel).
-template <bool ANYKIND, bool ROW16 = false>
+template <bool ANYKIND, bool ROW16 = false, bool DET = false>
 __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const Cbase, uint32_t (&r)[32], const int row, const int col0, const bool split, const int lane,
-                                               const float4 (&ypre)[8], const bool have_pre, const EpiStage& es) {
+                                               const float4 (&ypre)[8], const bool have_pre, const EpiStage& es, const DetArgs* det = nullptr) {
     if (col0 >= g.N) return;                                    // warp-uniform
     const int ncols = min(32, g.N - col0);
     const bool row_ok = row < g.M;
     float* crow = Cbase + (size_t)(row_ok ? row : 0) * g.ldc + col0;
+    if constexpr (DET) {
+        if (split) {        // split-K partial tile: stored into this split's slab of the workspace (Cbase)
+            if (row_ok) {
+                if ((ncols == 32) && ((g.ldc & 3) == 0) && ((((uintptr_t)Cbase) & 15) == 0) && ((col0 & 3) == 0)) {
+#pragma unroll
+                    for (int j = 0; j < 8; j++)
+                        reinterpret_cast<float4*>(crow)[j] = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
+                                                                         __uint_as_float(r[4 * j + 3]));
+                } else {
+#pragma unroll
+                    for (int j = 0; j < 32; j++) if (j < ncols) crow[j] = __uint_as_float(r[j]);
+                }
+            }
+            return;
+        }
+    }
     if (split) {            // split-K partial tile: reduce into C; 16-byte vector reductions cut the L2 atomic operations 4x
         if (row_ok) {
             if ((ncols == 32) && ((g.ldc & 3) == 0) && ((((uintptr_t)Cbase) & 15) == 0) && ((col0 & 3) == 0)) {
@@ -300,7 +324,9 @@ __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const C
 #pragma unroll
         for (int j = 0; j < 32; j++) sred[j] = (row_ok && j < ncols) ? v[j] : 0.f;
         const float s = transpose_reduce32(sred, lane);
-        if (lane < ncols) atomicAdd(g.colsum + col0 + lane, s);
+        // (DET: a 32-row block that starts at or beyond M -- the last tile's, when M % 128 is 1..96 -- has no slot among the M / 32 partials)
+        if constexpr (DET) { if (lane < ncols && row - lane < g.M) det->cs[(size_t)(row >> 5) * g.N + col0 + lane] = s; }
+        else if (lane < ncols) atomicAdd(g.colsum + col0 + lane, s);
     }
     if (g.nbx > 0) {        // warp-uniform.  C is the dz of a first layer with nbx trailing inputs: their weight gradient (column sums weighted by the
         const int cjx = col0 + lane;                     // row's trailing inputs) and input gradient (row dots with the trailing-input weights)
@@ -313,14 +339,16 @@ __device__ __forceinline__ void epilogue_chunk(const GemmArgs& g, float* const C
 #pragma unroll
                 for (int j = 0; j < 32; j++) sred[j] = (row_ok && j < ncols) ? v[j] * e : 0.f;
                 const float s = transpose_reduce32(sred, lane);
-                if (lane < ncols) atomicAdd(g.gwx + (size_t)cjx * g.ldgwx + t, s);
+                if constexpr (DET) { if (lane < ncols && row - lane < g.M) det->gwx[((size_t)(row >> 5) * g.N + cjx) * g.nbx + t] = s; }
+                else if (lane < ncols) atomicAdd(g.gwx + (size_t)cjx * g.ldgwx + t, s);
                 }
                 if (g.dx) {
                     const float wl = lane < ncols ? __ldg(g.bwx + (size_t)cjx * g.ldbwx + t) : 0.f;
                     float acc = 0.f;
 #pragma unroll
                     for (int j = 0; j < 32; j++) acc = fmaf(v[j], __shfl_sync(0xffffffffu, wl, j), acc);      // wl = 0 beyond ncols
-                    if (row_ok) atomicAdd(g.dx + (size_t)row * g.lddx + t, acc);
+                    if constexpr (DET) { if (row_ok) det->dx[((size_t)(col0 >> 5) * g.M + row) * g.nbx + t] = acc; }
+                    else if (row_ok) atomicAdd(g.dx + (size_t)row * g.lddx + t, acc);
                 }
             }
         }
@@ -413,9 +441,9 @@ __device__ __forceinline__ bool epilogue_prefetch(const GemmArgs& g, const int r
 // one [64 k][32 n] box, 64B-swizzled), two boxes per 128-wide tile 8 KB apart, and the tensor core reads them in place through its
 // transpose immediates: no shared-to-shared transposition.  ROW16: the epilogue can also store C row-major in BF16 (c16 without ct).
 constexpr int X_BYTES = 65536;
-template <int BN, bool ANYKIND, int CL, bool BF16, int AMN, int BMN, bool ROW16>
+template <int BN, bool ANYKIND, int CL, bool BF16, int AMN, int BMN, bool ROW16, bool DET = false>
 __device__ __forceinline__ void gemm_wgmma_body(const GemmMaps& gm, const CUtensorMap& mapC, const CUtensorMap& mapY, const GemmArgs& g,
-                                                const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
+                                                const int tiles_m, const int tiles_n, const int total_tiles, const int stages, const DetArgs* det = nullptr) {
     static_assert(CL == 1 || (CL == 2 && BN == BM), "CTA pairs share 128-row operand boxes");
     static_assert((AMN == 0 && BMN == 0 && !ROW16) || (BF16 && CL == 1), "MN-major BF16 operands and the row-major BF16 store: one CTA per tile");
     constexpr int G = EPI_G;
@@ -599,7 +627,10 @@ __device__ __forceinline__ void gemm_wgmma_body(const GemmMaps& gm, const CUtens
         if (tr) cons_sync();            // both warpgroups are done with the transposed tiles that the staging overlays
 
         const int row = m0 + 32 * q + lane;
-        float* const Cbase = CL == 1 && g.nprob > 1 ? g.Cg[t / g.tiles_per_prob] : g.C;
+        float* Cbase = CL == 1 && g.nprob > 1 ? g.Cg[t / g.tiles_per_prob] : g.C;
+        if constexpr (DET) {    // split-K: the slab of (problem, split) in the workspace
+            if (split) Cbase = det->split + (size_t)((CL == 1 && g.nprob > 1 ? t / g.tiles_per_prob : 0) * det->nsplit + kb0 / g.kb_per_split) * det->slab;
+        }
         float4 ypre[8];
         const bool have_pre = CL == 1 && !st_aux && (grp < BN / 32) && epilogue_prefetch(g, row, n0 + 32 * grp, split, ypre);
         store_fragment<BN / 8>(acc, xwg, 0, w, lane, [](float2 v, int, int) { return v; });
@@ -618,7 +649,7 @@ __device__ __forceinline__ void gemm_wgmma_body(const GemmMaps& gm, const CUtens
             EpiStage es;
             es.out = st_out ? blk : nullptr; es.mapC = &mapC; es.aux = st_aux ? my_aux : nullptr;
             if (st_aux) { mbar_wait(my_bar, aux_phase); aux_phase ^= 1; }
-            epilogue_chunk<ANYKIND, ROW16>(g, Cbase, r, row, n0 + 32 * c, split, lane, ypre, have_pre && c == grp, es);
+            epilogue_chunk<ANYKIND, ROW16, DET>(g, Cbase, r, row, n0 + 32 * c, split, lane, ypre, have_pre && c == grp, es, det);
             if (st_aux) { __syncwarp(); request_aux(); }             // every lane has read the operand block: fetch the next one into it
         }
     }
@@ -638,6 +669,19 @@ __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_bf16_mn_wgmma(const 
                                                                          const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
                                                                          const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
     gemm_wgmma_body<BN, ANYKIND, 1, true, AMN, BMN, true>(gm, mapC, mapY, g, tiles_m, tiles_n, total_tiles, stages);
+}
+// the two kernels of the deterministic mode (DetArgs): the same products, their cross-CTA sums left to go1_det_sum
+template <int BN, bool ANYKIND, int CL, bool BF16>
+__global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma_det(const __grid_constant__ GemmMaps gm,
+                                                                          const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
+                                                                          const int tiles_m, const int tiles_n, const int total_tiles, const int stages, const DetArgs det) {
+    gemm_wgmma_body<BN, ANYKIND, CL, BF16, 0, 0, false, true>(gm, mapC, mapY, g, tiles_m, tiles_n, total_tiles, stages, &det);
+}
+template <int BN, bool ANYKIND, int AMN, int BMN>
+__global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_bf16_mn_wgmma_det(const __grid_constant__ GemmMaps gm,
+                                                                             const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
+                                                                             const int tiles_m, const int tiles_n, const int total_tiles, const int stages, const DetArgs det) {
+    gemm_wgmma_body<BN, ANYKIND, 1, true, AMN, BMN, true, true>(gm, mapC, mapY, g, tiles_m, tiles_n, total_tiles, stages, &det);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -727,9 +771,10 @@ __global__ void bias_act_strided(float* C, int ldc, const float* bias, int M, in
     *c = v;
 }
 
-// MN < 0: gemm_tf32_wgmma<BN, ANYKIND, CL, BF16>; MN = 0..3: gemm_bf16_mn_wgmma<BN, ANYKIND, MN & 1, MN >> 1> (CL 1, BF16)
-template <int BN, bool ANYKIND, int CL, bool BF16, int MN = -1>
-int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st) {
+// MN < 0: gemm_tf32_wgmma<BN, ANYKIND, CL, BF16>; MN = 0..3: gemm_bf16_mn_wgmma<BN, ANYKIND, MN & 1, MN >> 1> (CL 1, BF16); det: their _det
+// kernels (deterministic mode)
+template <int BN, bool ANYKIND, int CL, bool BF16, int MN = -1, bool DET = false>
+int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st, const DetArgs* det = nullptr) {
     constexpr int STAGE_BYTES = (BM + BN) * BK * 4;
     const size_t staging = X_BYTES + (g.tma_aux ? (size_t)NCONS * 4096 : 0);
     const size_t fixed = staging + (2 * 8 + NCONS) * 8 + 16 + 1024;
@@ -740,8 +785,13 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
     const size_t smem = (size_t)stages * STAGE_BYTES + fixed;
     static_assert(MN < 0 || (CL == 1 && BF16), "the MN-major BF16 kernel runs one CTA per tile");
     auto kernel = [] {
-        if constexpr (MN < 0) return gemm_tf32_wgmma<BN, ANYKIND, CL, BF16>;
-        else return gemm_bf16_mn_wgmma<BN, ANYKIND, (MN & 1), (MN >> 1)>;
+        if constexpr (DET) {
+            if constexpr (MN < 0) return gemm_tf32_wgmma_det<BN, ANYKIND, CL, BF16>;
+            else return gemm_bf16_mn_wgmma_det<BN, ANYKIND, (MN & 1), (MN >> 1)>;
+        } else {
+            if constexpr (MN < 0) return gemm_tf32_wgmma<BN, ANYKIND, CL, BF16>;
+            else return gemm_bf16_mn_wgmma<BN, ANYKIND, (MN & 1), (MN >> 1)>;
+        }
     }();
     const int tiles_m = (g.M + BM - 1) / BM, tiles_n = (g.N + BN - 1) / BN;
     g.tiles_per_prob = tiles_m * tiles_n * splits;
@@ -771,10 +821,18 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
     // persistent grid: one CTA per SM (the ring and the staging fill its shared memory), CL x (pair-)tile slots for clusters
     const int units = total / CL;
     cfg.gridDim = dim3(CL * (units < slots ? units : slots));
-    if (CL == 1) kernel<<<cfg.gridDim, cfg.blockDim, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages);
-    else {
-        cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, gm, mc, my, g, tiles_m, tiles_n, total, stages);
-        if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
+    if constexpr (DET) {
+        if (CL == 1) kernel<<<cfg.gridDim, cfg.blockDim, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages, *det);
+        else {
+            cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, gm, mc, my, g, tiles_m, tiles_n, total, stages, *det);
+            if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
+        }
+    } else {
+        if (CL == 1) kernel<<<cfg.gridDim, cfg.blockDim, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages);
+        else {
+            cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, gm, mc, my, g, tiles_m, tiles_n, total, stages);
+            if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
+        }
     }
     go1_count_launch(1);
     return 0;
@@ -1130,14 +1188,31 @@ extern "C" int go1_gemm_timing(int on, double* total_ms, double* total_flop, lon
 }
 
 // the MN-major BF16 kernel of layout mn (bit 0: A MN-major, bit 1: B MN-major)
-template <int BN, bool ANYKIND>
-int launch_gemm_mn(int mn, const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st) {
+template <int BN, bool ANYKIND, bool DET>
+int launch_gemm_mn(int mn, const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st, const DetArgs* det) {
     switch (mn) {
-        case 0: return launch_gemm<BN, ANYKIND, 1, true, 0>(gm, mc, my, g, splits, st);
-        case 1: return launch_gemm<BN, ANYKIND, 1, true, 1>(gm, mc, my, g, splits, st);
-        case 2: return launch_gemm<BN, ANYKIND, 1, true, 2>(gm, mc, my, g, splits, st);
-        default: return launch_gemm<BN, ANYKIND, 1, true, 3>(gm, mc, my, g, splits, st);
+        case 0: return launch_gemm<BN, ANYKIND, 1, true, 0, DET>(gm, mc, my, g, splits, st, det);
+        case 1: return launch_gemm<BN, ANYKIND, 1, true, 1, DET>(gm, mc, my, g, splits, st, det);
+        case 2: return launch_gemm<BN, ANYKIND, 1, true, 2, DET>(gm, mc, my, g, splits, st, det);
+        default: return launch_gemm<BN, ANYKIND, 1, true, 3, DET>(gm, mc, my, g, splits, st, det);
     }
+}
+// the kernel of (mnk, cluster, BN, any) in the default or the deterministic instantiation
+template <bool BF16, bool DET>
+int launch_gemm_any(int mnk, int cluster, int BN, bool any, const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st,
+                    const DetArgs* det) {
+    if (mnk >= 0) {
+        if constexpr (BF16) {
+            if (BN == 128) return any ? launch_gemm_mn<128, true, DET>(mnk, gm, mc, my, g, splits, st, det) : launch_gemm_mn<128, false, DET>(mnk, gm, mc, my, g, splits, st, det);
+            if (BN == 64) return any ? launch_gemm_mn<64, true, DET>(mnk, gm, mc, my, g, splits, st, det) : launch_gemm_mn<64, false, DET>(mnk, gm, mc, my, g, splits, st, det);
+            return any ? launch_gemm_mn<32, true, DET>(mnk, gm, mc, my, g, splits, st, det) : launch_gemm_mn<32, false, DET>(mnk, gm, mc, my, g, splits, st, det);
+        }
+        return go1_set_error("go1_gemm: MN-major BF16 layout without BF16 operands");
+    }
+    if (cluster == 2) return any ? launch_gemm<128, true, 2, BF16, -1, DET>(gm, mc, my, g, splits, st, det) : launch_gemm<128, false, 2, BF16, -1, DET>(gm, mc, my, g, splits, st, det);
+    if (BN == 128) return any ? launch_gemm<128, true, 1, BF16, -1, DET>(gm, mc, my, g, splits, st, det) : launch_gemm<128, false, 1, BF16, -1, DET>(gm, mc, my, g, splits, st, det);
+    if (BN == 64) return any ? launch_gemm<64, true, 1, BF16, -1, DET>(gm, mc, my, g, splits, st, det) : launch_gemm<64, false, 1, BF16, -1, DET>(gm, mc, my, g, splits, st, det);
+    return any ? launch_gemm<32, true, 1, BF16, -1, DET>(gm, mc, my, g, splits, st, det) : launch_gemm<32, false, 1, BF16, -1, DET>(gm, mc, my, g, splits, st, det);
 }
 
 // T = float: TF32 products (operands in either major); T = uint16_t: BF16 products, K-major operands only (go1_gemm_bf16_ex), or with
@@ -1212,8 +1287,21 @@ static int gemm_wgmma_impl(int transA, int transB, int M, int N, int K, int npro
         if (int e = tiles_n % 2 == 0 ? make_map(&gm.half, As[0], M, K, lda, BM / 2, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES)
                                      : make_map(&gm.half, Bs[0], N, K, ldb, BN / 2, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES)) return e;
     }
+    // deterministic mode: the launches whose CTAs add into shared targets run their _det kernels, whose partials go to the stream's workspace
+    const bool det = go1_det_on() && (splits > 1 || g.colsum || (g.nbx > 0 && (g.gwx || g.dx)));
+    DetArgs da = {};
+    if (det) {
+        const size_t nrb = (size_t)(M + 31) / 32, ncb = (size_t)(N + 31) / 32;
+        const size_t r4 = 3;        // region sizes rounded up to 16 bytes
+        const size_t n_split = splits > 1 ? ((size_t)nprob * splits * M * ldc + r4) & ~r4 : 0, n_cs = g.colsum ? (nrb * N + r4) & ~r4 : 0;
+        const size_t n_gwx = g.nbx > 0 && g.gwx ? (nrb * N * g.nbx + r4) & ~r4 : 0, n_dx = g.nbx > 0 && g.dx ? (ncb * M * g.nbx + r4) & ~r4 : 0;
+        float* ws = (float*)go1_det_workspace(st, sizeof(float) * (n_split + n_cs + n_gwx + n_dx));
+        if (!ws) return 1;
+        da.split = ws; da.slab = (size_t)M * ldc; da.nsplit = splits;
+        da.cs = ws + n_split; da.gwx = da.cs + n_cs; da.dx = da.gwx + n_gwx;
+    }
     if (splits > 1) {
-        if (!accumulate)
+        if (!accumulate && !det)
             for (int p = 0; p < nprob; p++) { const size_t tot = (size_t)M * N; zero_strided<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cs[p], ldc, M, N); go1_count_launch(1); }
         g.bias = nullptr; g.act = 0;
     }
@@ -1247,15 +1335,18 @@ static int gemm_wgmma_impl(int transA, int transB, int M, int N, int K, int npro
         }
     }
     const bool any = g.act != 0 && g.kind != GO1_ACT_ELU;
-    if (mnk >= 0) {
-        if (BN == 128) e = any ? launch_gemm_mn<128, true>(mnk, gm, mc, my, g, splits, st) : launch_gemm_mn<128, false>(mnk, gm, mc, my, g, splits, st);
-        else if (BN == 64) e = any ? launch_gemm_mn<64, true>(mnk, gm, mc, my, g, splits, st) : launch_gemm_mn<64, false>(mnk, gm, mc, my, g, splits, st);
-        else e = any ? launch_gemm_mn<32, true>(mnk, gm, mc, my, g, splits, st) : launch_gemm_mn<32, false>(mnk, gm, mc, my, g, splits, st);
-    } else if (cluster == 2) e = any ? launch_gemm<128, true, 2, BF16>(gm, mc, my, g, splits, st) : launch_gemm<128, false, 2, BF16>(gm, mc, my, g, splits, st);
-    else if (BN == 128) e = any ? launch_gemm<128, true, 1, BF16>(gm, mc, my, g, splits, st) : launch_gemm<128, false, 1, BF16>(gm, mc, my, g, splits, st);
-    else if (BN == 64) e = any ? launch_gemm<64, true, 1, BF16>(gm, mc, my, g, splits, st) : launch_gemm<64, false, 1, BF16>(gm, mc, my, g, splits, st);
-    else e = any ? launch_gemm<32, true, 1, BF16>(gm, mc, my, g, splits, st) : launch_gemm<32, false, 1, BF16>(gm, mc, my, g, splits, st);
+    e = det ? launch_gemm_any<BF16, true>(mnk, cluster, BN, any, gm, mc, my, g, splits, st, &da)
+            : launch_gemm_any<BF16, false>(mnk, cluster, BN, any, gm, mc, my, g, splits, st, nullptr);
     if (e) return e;
+    if (det) {      // the partials, in a fixed order, into C (split-K: overwriting it unless accumulate) and the epilogue's targets (adding)
+        if (splits > 1)
+            for (int p = 0; p < nprob; p++)
+                if (int e2 = go1_det_sum(da.split + (size_t)p * splits * da.slab, splits, da.slab, Cs[p], M, N, ldc, accumulate, st, ldc)) return e2;
+        const int nrb = (M + 31) / 32, ncb = (N + 31) / 32;
+        if (g.colsum) { if (int e2 = go1_det_sum(da.cs, nrb, N, g.colsum, 1, N, N, 1, st)) return e2; }
+        if (g.nbx > 0 && g.gwx) { if (int e2 = go1_det_sum(da.gwx, nrb, (size_t)N * g.nbx, g.gwx, N, g.nbx, g.ldgwx, 1, st)) return e2; }
+        if (g.nbx > 0 && g.dx) { if (int e2 = go1_det_sum(da.dx, ncb, (size_t)M * g.nbx, g.dx, M, g.nbx, g.lddx, 1, st)) return e2; }
+    }
     if (splits > 1 && (bias || act))
         for (int p = 0; p < nprob; p++) { const size_t tot = (size_t)M * N; bias_act_strided<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cs[p], ldc, bias, M, N, act, ep->act_kind); go1_count_launch(1); }
     if (timed) cudaEventRecord(timing_event(), st);

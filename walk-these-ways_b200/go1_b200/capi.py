@@ -4,6 +4,7 @@ The product has no CPU fallback: importing this module works anywhere (so the bu
 on a CPU box), but every compute call goes through the CUDA library and raises Go1Error if the
 library is missing or no CUDA device is present.
 """
+import contextlib
 import ctypes as C
 import os
 
@@ -218,6 +219,8 @@ def lib():
         "go1_sim_set_commands": ([vp, vp, ip, vp, vp], ip),
         "go1_sim_set_step_block": ([ip], None),
         "go1_sizeof_curriculum": ([ip], ip), "go1_curriculum_set_grouped": ([ip], None),
+        "go1_set_deterministic": ([ip], None), "go1_deterministic": ([], ip), "go1_deterministic_workspace_bytes": ([], i64),
+        "go1_deterministic_reserve": ([vp], ip),
         "go1_curriculum_resample": ([vp, C.POINTER(Go1CurriculumConfig), C.POINTER(Go1CurriculumBuffers), ip, vp], ip),
         "go1_curriculum_pack": ([vp, C.POINTER(Go1CurriculumConfig), C.POINTER(Go1CurriculumBuffers), vp], ip),
         "go1_sim_reset_idx_dev": ([vp, vp, vp, vp, vp, ip, i64, vp, vp], ip),
@@ -278,6 +281,26 @@ def lib():
         raise Go1Error("Go1Curriculum* mirrors out of date")
     _lib = L
     return L
+
+
+@contextlib.contextmanager
+def deterministic(on):
+    """The library's deterministic mode (go1_set_deterministic) set to `on` for the launches inside the block and restored afterwards.  Nothing
+    is called when the library is already in that mode, nor to keep the default mode before the library has been loaded."""
+    on = 1 if on else 0
+    if _lib is None and not on:
+        yield
+        return
+    L = lib()
+    prev = L.go1_deterministic()
+    if prev == on:
+        yield
+        return
+    L.go1_set_deterministic(on)
+    try:
+        yield
+    finally:
+        L.go1_set_deterministic(prev)
 
 
 def check(rc, what=""):

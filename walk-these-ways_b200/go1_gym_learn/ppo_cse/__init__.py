@@ -243,8 +243,12 @@ class Runner:
                 elif g is None:
                     graph = torch.cuda.CUDAGraph()
                     ac.ensure_packed()
+                    cap = {}
+                    if ac.deterministic:    # captured on a stream of its own whose workspace (go1_set_deterministic) is sized before the capture
+                        cap["stream"] = self.__dict__.setdefault("_det_capture_stream", torch.cuda.Stream())
+                        capi.check(L.go1_deterministic_reserve(cap["stream"].cuda_stream), "go1_deterministic_reserve")
                     n0 = L.go1_kernel_launch_count()
-                    with torch.cuda.graph(graph):
+                    with torch.cuda.graph(graph, **cap):
                         actions = self._graph_step_body(sg)
                     n_kernels = L.go1_kernel_launch_count() - n0
                     L.go1_kernel_launch_add(-n_kernels)

@@ -12,7 +12,9 @@ the reference's names, .act / .evaluate / .act_student / .act_teacher / .get_act
     the product for 4 < E <= 64);
   * no autograd graph: the backward pass is written out (see `backward_ppo`, `backward_adaptation`).
 """
+import functools
 import numbers
+import os
 
 import torch
 import torch.nn as nn
@@ -33,6 +35,17 @@ class AC_Args(PrefixProto, cli=False):
                         # 2 = as 1, but the products that reduce over the observation history (the first layers) take BF16 operands (fp32 accumulation)
     bf16_backward = False   # with gemm_impl = 2 only: the hidden layers' dgrads and weight gradients run on BF16 too (MN-major operands read in place);
                             # hidden-layer dz is then held in BF16 (see ActorCritic.backward_ppo)
+    deterministic = os.environ.get("GO1_DETERMINISTIC", "0") != "0"   # fixed-order learner reductions: bit-identical runs from identical inputs (go1_set_deterministic)
+
+
+def in_mode(method):
+    """Runs an ActorCritic / PPO / RolloutStorage method in the deterministic mode of the object (its `deterministic` attribute): the library
+    mode is set around the call and restored afterwards, so that learners of either mode can be used side by side."""
+    @functools.wraps(method)
+    def wrapped(self, *a, **k):
+        with capi.deterministic(self.deterministic):
+            return method(self, *a, **k)
+    return wrapped
 
 
 def _mlp(in_dim, hidden, out_dim, activation):
@@ -512,11 +525,13 @@ class ActorCritic(nn.Module):
         self.sample_seed = 0
         self.injected_eps = None      # parity tests inject the N(0,1) draws
         self.weights_version = 0      # bumped by every optimizer step / load: invalidates the packed first-layer weight copies
-        import os
         self.update_streams = os.environ.get("GO1_UPDATE_STREAMS", "1") != "0"     # critic chain on a second stream during the update (measured -1.3 ms / iteration)
         self._side = None
         self.model_inputs = {}        # AC_Args.gemm_impl = 2: tag -> the BF16 history the last call with that tag read (see _model_input)
         self.fuse_tail = os.environ.get("GO1_FUSE_TAIL", "1") != "0"     # layers behind a first layer in one wgmma launch (go1_mlp_tail_forward_grouped: actor + critic bodies in one grid)
+        # AC_Args.deterministic, or torch.use_deterministic_algorithms(True): every launch of this learner (and of its PPO and RolloutStorage)
+        # sums its cross-CTA reductions in a fixed order (in_mode)
+        self.deterministic = bool(AC_Args.deterministic) or torch.are_deterministic_algorithms_enabled()
 
     # ------------------------------------------------------------------ flat storage
     def _ordered_params(self):
@@ -657,6 +672,7 @@ class ActorCritic(nn.Module):
         self.model_inputs[tag] = h16
         return h16
 
+    @in_mode
     def update_distribution(self, observation_history, tag="act"):
         self.flatten()
         h = self._model_input(observation_history, tag)
@@ -667,6 +683,7 @@ class ActorCritic(nn.Module):
         self._mean = self._p_out[-1]
         self._latent = latent
 
+    @in_mode
     def forward_all(self, observation_history, privileged_observations, tag="act"):
         """update_distribution + evaluate in one pass.  With the tensor-core path the first layers of the three MLPs --
         which all read obs_history -- run as ONE product [M][256+512+512] = h Wcat^T: bias + activation (+ the critic's E <= 4
@@ -773,6 +790,7 @@ class ActorCritic(nn.Module):
         self._ev_join.record(side)
         torch.cuda.current_stream().wait_event(self._ev_join)
 
+    @in_mode
     def act_and_evaluate(self, observation_history, privileged_observations):
         """PPO.act's two calls (actor_critic.act + evaluate, ppo.py:67-68) on one fused forward pass."""
         self.forward_all(observation_history, privileged_observations, "act")
@@ -787,6 +805,7 @@ class ActorCritic(nn.Module):
     def stddev(self):
         return self.action_std
 
+    @in_mode
     def act(self, observation_history, **kwargs):
         self.update_distribution(observation_history)
         return self._sample(observation_history)
@@ -819,6 +838,7 @@ class ActorCritic(nn.Module):
     def act_inference(self, ob, policy_info={}):
         return self.act_student(ob["obs_history"], policy_info=policy_info)
 
+    @in_mode
     def act_student(self, observation_history, policy_info={}):
         if observation_history.shape[0] == 0:
             return observation_history.new_zeros(0, self.num_actions)
@@ -826,6 +846,7 @@ class ActorCritic(nn.Module):
         policy_info["latents"] = self._latent.detach().cpu().numpy()
         return self._mean
 
+    @in_mode
     def act_teacher(self, observation_history, privileged_info, policy_info={}):
         if observation_history.shape[0] == 0:
             return observation_history.new_zeros(0, self.num_actions)
@@ -835,6 +856,7 @@ class ActorCritic(nn.Module):
         policy_info["latents"] = privileged_info
         return out[-1]
 
+    @in_mode
     def evaluate(self, observation_history, privileged_observations, tag="act", **kwargs):
         self.flatten()
         h = self._model_input(observation_history, tag)
@@ -842,6 +864,7 @@ class ActorCritic(nn.Module):
         self._value = self._c_out[-1]
         return self._value
 
+    @in_mode
     def get_student_latent(self, observation_history):
         self.flatten()
         h = self._model_input(observation_history, "latent")
@@ -905,6 +928,7 @@ class ActorCritic(nn.Module):
             return self._nets["adapt"]._buf16(key, rows, M)
         return self._nets["adapt"]._buf(key, rows, M, (M + 31) // 32 * 32)
 
+    @in_mode
     def backward_ppo(self, h, priv, dmean, dvalue, dstd, hT=None):
         """Gradients of the PPO loss into flat_grads[HEAD:] (overwrites; the loss scalars in the head are left alone). h/priv are the
         minibatch inputs of the forward pass just run with tag='train'; dmean [M,A], dvalue [M,1], dstd [A].
@@ -965,6 +989,7 @@ class ActorCritic(nn.Module):
             self._join(side)
         self._flush_wgrads(wgrads)
 
+    @in_mode
     def backward_adaptation(self, h, outs, dpred, hT=None):
         """Gradients of the adaptation module (overwrites its part of flat_grads, [HEAD:n_adapt_params]).  hT: history_kmajor(h, ..) if the
         caller keeps one (built here otherwise); the first layer's weight and bias gradients are the K-major product over its first K0 + 1 rows."""
@@ -983,6 +1008,7 @@ class ActorCritic(nn.Module):
                 h = h.float()
             net.backward(h, h.stride(0), K0, None, outs, dpred, M, self._impl(), tag="adapt")
 
+    @in_mode
     def adaptation_forward(self, h):
         self.flatten()
         h = self._model_input(h, "adapt")

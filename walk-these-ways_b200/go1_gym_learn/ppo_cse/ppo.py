@@ -7,7 +7,7 @@ from go1_b200 import capi
 from go1_gym_learn.ppo_cse import ActorCritic
 from go1_gym_learn.ppo_cse import RolloutStorage
 from go1_gym_learn.ppo_cse import caches
-from go1_gym_learn.ppo_cse.actor_critic import _Net
+from go1_gym_learn.ppo_cse.actor_critic import _Net, in_mode
 from params_proto import PrefixProto
 
 
@@ -81,8 +81,11 @@ class PPO:
     _scalars = property(lambda self: self.actor_critic.flat_grads[0:8])
     _mse_scalars = property(lambda self: self.actor_critic.flat_grads[8:10])
 
+    deterministic = property(lambda self: self.actor_critic.deterministic)      # the mode of in_mode: the ActorCritic's
+
     def init_storage(self, num_envs, num_transitions_per_env, actor_obs_shape, privileged_obs_shape, obs_history_shape, action_shape):
         self.storage = RolloutStorage(num_envs, num_transitions_per_env, actor_obs_shape, privileged_obs_shape, obs_history_shape, action_shape, self.device)
+        self.storage.deterministic = self.actor_critic.deterministic
 
     def test_mode(self):
         self.actor_critic.eval()
@@ -134,7 +137,8 @@ class PPO:
             ac.ensure_packed()                                    # the graph reads the packed weight copies, it does not build them
             L = capi.lib()
             n0 = L.go1_kernel_launch_count()
-            with torch.cuda.graph(graph):
+            # deterministic mode: captured on the stream of the warm-up calls, whose workspace (go1_set_deterministic) they have sized
+            with torch.cuda.graph(graph, **({"stream": side} if ac.deterministic else {})):
                 outs = self._act_eager(h_in, p_in)
             n_kernels = L.go1_kernel_launch_count() - n0          # this library's kernels inside the graph
             L.go1_kernel_launch_add(-n_kernels)                   # capture launched nothing
@@ -148,6 +152,7 @@ class PPO:
         ac._mean, ac._logp, ac._last_actions, ac._value, ac._latent = attrs     # the graph's static outputs
         return outs
 
+    @in_mode
     def act(self, obs, privileged_obs, obs_history):
         tr = self.transition
         ac = self.actor_critic
@@ -191,6 +196,7 @@ class PPO:
         tr.clear()
         self.actor_critic.reset(dones)
 
+    @in_mode
     def compute_returns(self, last_critic_obs, last_critic_privileged_obs):
         last_values = self.actor_critic.evaluate(last_critic_obs, last_critic_privileged_obs, tag="last").detach()
         self.storage.compute_returns(last_values, PPO_Args.gamma, PPO_Args.lam)
@@ -200,6 +206,7 @@ class PPO:
             import torch.distributed as dist
             dist.all_reduce(t, group=self.process_group)
 
+    @in_mode
     def update(self):
         ac, L, st = self.actor_critic, capi.lib(), capi.stream_ptr
         world = 1

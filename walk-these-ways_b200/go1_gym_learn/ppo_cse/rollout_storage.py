@@ -3,7 +3,7 @@ GAE through the warp-scan kernel, minibatches through the row-gather kernel."""
 import torch
 
 from go1_b200 import capi
-from .actor_critic import AC_Args, history_kmajor
+from .actor_critic import AC_Args, history_kmajor, in_mode
 
 
 class RolloutStorage:
@@ -137,6 +137,9 @@ class RolloutStorage:
     def clear(self):
         self.step = 0
 
+    deterministic = False       # the learner's mode (AC_Args.deterministic), set by PPO.init_storage
+
+    @in_mode
     def compute_returns(self, last_values, gamma, lam):
         T, N = self.num_transitions_per_env, self.num_envs
         L, st = capi.lib(), capi.stream_ptr()
