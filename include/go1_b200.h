@@ -181,6 +181,22 @@ int go1_sim_update_config(Go1Sim* sim, const Go1SimConfig* cfg, void* stream);
 int go1_sim_step(Go1Sim* sim, const float* actions /*[N][12]*/, const float gravity[3],
                  const float gravity_vec[3], int64_t common_step, int mode, void* stream);
 
+/* Self-collisions between the robot's own links (DESIGN.md §3), the counterpart of Isaac Gym's
+ * asset_options.self_collisions / PhysX's self-collision filter.  Thigh and calf are capsules (thigh joint -> knee, knee -> foot),
+ * the foot a sphere, the trunk the box GO1_BASE_BOX_HALF.  Tested pairs: thigh/calf/foot of one leg against thigh/calf/foot of
+ * every other leg, and each leg's knee, calf midpoint and foot (as spheres of the thigh, calf and foot radius) against the
+ * trunk.  Explicit penalty law: normal force max(k depth - c v_n, 0), friction clamped as for the ground penalty contacts
+ * with the env's robot friction.  The forces are added to the reported thigh, calf, foot and base contact forces. */
+typedef struct Go1SelfCollision {
+    int32_t enabled;                    /* 0 = off (default): the step kernel is the one without self-collisions */
+    float k, c;                         /* N/m, N s/m */
+    float thigh_radius, calf_radius, foot_radius;   /* m */
+} Go1SelfCollision;
+int go1_sizeof_self_collision(void);
+/* Store the self-collision model of `sim`.  Only before the first go1_sim_step: a captured step graph keeps the kernel that
+ * was chosen when it was captured, so a later change fails (and leaves the setting as it was). */
+int go1_sim_set_self_collision(Go1Sim* sim, const Go1SelfCollision* sc);
+
 /* Threads per CTA of the step kernel: 32, 64 or 128; 0 (default) = 32 up to 16384 envs, 128 above (tuning knob). */
 void go1_sim_set_step_block(int threads);
 

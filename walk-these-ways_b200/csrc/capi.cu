@@ -7,7 +7,7 @@
 #include "go1_layout.h"
 #include "go1_model_generated.h"
 
-extern "C" int go1_launch_step(const Go1SimBuffers*, const Go1DevTable*, const float*, const float*, const float*, long long, int, int, cudaStream_t);
+extern "C" int go1_launch_step(const Go1SimBuffers*, const Go1DevTable*, const Go1SelfCollision*, const float*, const float*, const float*, long long, int, int, cudaStream_t);
 extern "C" int go1_launch_reset(const Go1SimBuffers*, const Go1DevTable*, const int*, int, const float*, const float*, int, long long, const float*, int, cudaStream_t);
 extern "C" int go1_launch_set_commands(const Go1SimBuffers*, const int*, int, const float*, int, cudaStream_t);
 extern "C" int go1_launch_reset_dev(const Go1SimBuffers*, const Go1DevTable*, const int*, const int*, const float*, const float*, int, long long, const float*, float*, int, cudaStream_t);
@@ -37,6 +37,8 @@ struct Go1Sim {
     int bound;
     int device;
     float gravity[3];
+    Go1SelfCollision self;   // enabled = 0 unless go1_sim_set_self_collision turned it on
+    int stepped;             // go1_sim_step has been called: the kernel choice is fixed
 };
 
 extern "C" const char* go1_last_error(void) { return g_err.c_str(); }
@@ -49,6 +51,7 @@ extern "C" int go1_device_count(void) {
 
 extern "C" int go1_sizeof_config(void) { return (int)sizeof(Go1SimConfig); }
 extern "C" int go1_sizeof_buffers(void) { return (int)sizeof(Go1SimBuffers); }
+extern "C" int go1_sizeof_self_collision(void) { return (int)sizeof(Go1SelfCollision); }
 
 extern "C" int go1_sim_num_rows(int kind) {
     return kind == 0 ? (int)GO1_ENV_F32_ROWS : (kind == 1 ? (int)GO1_LEG_F32_ROWS : (kind == 2 ? GO1_ENV_I32_ROWS : -1));
@@ -168,6 +171,7 @@ extern "C" int go1_sim_create(const Go1SimConfig* cfg, const float* actuator_wei
     Go1Sim* s = new Go1Sim();
     memset(&s->bufs, 0, sizeof(s->bufs));
     s->cfg = *cfg; s->bound = 0; s->device = device; s->d_tab = nullptr;
+    memset(&s->self, 0, sizeof(s->self)); s->stepped = 0;
     if (int e = build_table(cfg, actuator_weights, &s->h_tab)) { delete s; return e; }
     if ((ce = cudaMalloc(&s->d_tab, sizeof(Go1DevTable))) != cudaSuccess) { delete s; return cuda_fail("cudaMalloc table", ce); }
     if ((ce = cudaMemcpy(s->d_tab, &s->h_tab, sizeof(Go1DevTable), cudaMemcpyHostToDevice)) != cudaSuccess) { cudaFree(s->d_tab); delete s; return cuda_fail("upload table", ce); }
@@ -202,13 +206,23 @@ extern "C" int go1_sim_update_config(Go1Sim* s, const Go1SimConfig* cfg, void* s
     return 0;
 }
 
+extern "C" int go1_sim_set_self_collision(Go1Sim* s, const Go1SelfCollision* sc) {
+    if (!s || !sc) return fail("go1_sim_set_self_collision: null argument");
+    if (s->stepped) return fail("go1_sim_set_self_collision: the self-collision model cannot change after the first go1_sim_step");
+    if (sc->enabled && !(sc->k >= 0.f && sc->c >= 0.f && sc->thigh_radius > 0.f && sc->calf_radius > 0.f && sc->foot_radius > 0.f))
+        return fail("go1_sim_set_self_collision: k and c must be >= 0 and the radii > 0");
+    s->self = *sc;
+    return 0;
+}
+
 extern "C" int go1_sim_step(Go1Sim* s, const float* actions, const float gravity[3], const float gravity_vec[3],
                             int64_t common_step, int mode, void* stream) {
     if (!s || !s->bound) return fail("go1_sim_step: sim not bound");
     if (!actions) return fail("go1_sim_step: null actions");
     if (mode < 0 || mode > 2) return fail("go1_sim_step: bad mode");
     for (int k = 0; k < 3; k++) s->gravity[k] = gravity[k];
-    int e = go1_launch_step(&s->bufs, s->d_tab, actions, gravity, gravity_vec, (long long)common_step, mode, s->cfg.num_envs, (cudaStream_t)stream);
+    s->stepped = 1;
+    int e = go1_launch_step(&s->bufs, s->d_tab, &s->self, actions, gravity, gravity_vec, (long long)common_step, mode, s->cfg.num_envs, (cudaStream_t)stream);
     return e ? cuda_fail("go1_sim_step launch", e) : 0;
 }
 

@@ -118,6 +118,11 @@ class Go1SimBuffers(C.Structure):
         "episode_acc", "noise", "reset_rand", "gravity_dev", "step_dev", "episode_sums_eval")]
 
 
+class Go1SelfCollision(C.Structure):
+    """Self-collision model of a sim (go1_sim_set_self_collision); enabled = 0 keeps the default step kernel."""
+    _fields_ = [("enabled", _i), ("k", _f), ("c", _f), ("thigh_radius", _f), ("calf_radius", _f), ("foot_radius", _f)]
+
+
 CUR_MAX_CATEGORIES = 8
 
 
@@ -218,6 +223,7 @@ def lib():
         "go1_sim_reset_idx": ([vp, vp, ip, vp, vp, ip, i64, vp], ip),
         "go1_sim_set_commands": ([vp, vp, ip, vp, vp], ip),
         "go1_sim_set_step_block": ([ip], None),
+        "go1_sizeof_self_collision": ([], ip), "go1_sim_set_self_collision": ([vp, C.POINTER(Go1SelfCollision)], ip),
         "go1_sizeof_curriculum": ([ip], ip), "go1_curriculum_set_grouped": ([ip], None),
         "go1_set_deterministic": ([ip], None), "go1_deterministic": ([], ip), "go1_deterministic_workspace_bytes": ([], i64),
         "go1_deterministic_reserve": ([vp], ip),
@@ -277,6 +283,8 @@ def lib():
         raise Go1Error(f"Go1SimConfig mirror out of date: C {L.go1_sizeof_config()} vs ctypes {C.sizeof(Go1SimConfig)}")
     if L.go1_sizeof_buffers() != C.sizeof(Go1SimBuffers):
         raise Go1Error("Go1SimBuffers mirror out of date")
+    if L.go1_sizeof_self_collision() != C.sizeof(Go1SelfCollision):
+        raise Go1Error("Go1SelfCollision mirror out of date")
     if L.go1_sizeof_curriculum(0) != C.sizeof(Go1CurriculumConfig) or L.go1_sizeof_curriculum(1) != C.sizeof(Go1CurriculumBuffers):
         raise Go1Error("Go1Curriculum* mirrors out of date")
     _lib = L

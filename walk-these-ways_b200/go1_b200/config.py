@@ -184,6 +184,20 @@ def fill_domain_rand(D, cfg, dt):
     D.x_init_offset, D.y_init_offset = t.x_init_offset, t.y_init_offset
 
 
+SELF_K, SELF_C = 5000.0, 20.0      # self-contact penalty stiffness (N/m) and damping (N s/m), DESIGN.md §3
+
+
+def self_collision_config(cfg, k=SELF_K, c=SELF_C):
+    """Go1SelfCollision of `cfg`: on iff Cfg.asset.model_self_collisions (unset = the GO1_SELF_COLLISIONS=1 environment switch)
+    and bit 0 of Cfg.asset.self_collisions is clear (the reference's "1 to disable, 0 to enable")."""
+    on = getattr(cfg.asset, "model_self_collisions", os.environ.get("GO1_SELF_COLLISIONS") == "1")
+    sc = capi.Go1SelfCollision()
+    sc.enabled = int(bool(on) and (int(getattr(cfg.asset, "self_collisions", 0)) & 1) == 0)
+    sc.k, sc.c = float(k), float(c)
+    sc.thigh_radius, sc.calf_radius, sc.foot_radius = 0.017, 0.008, 0.02
+    return sc
+
+
 def build_sim_config(cfg, num_envs=None, num_train_envs=None, seed=0, physics=None, eval_cfg=None):
     """Resolve `cfg` (a Cfg-like class tree) into a Go1SimConfig.  `physics` overrides solver parameters; `eval_cfg` is the
     second Cfg tree of the train/eval split (its randomisation / reset ranges apply to envs >= num_train_envs)."""
@@ -289,6 +303,8 @@ def build_sim_config(cfg, num_envs=None, num_train_envs=None, seed=0, physics=No
     c.pen_k[:] = [20000., 20000., 5000., 5000.]
     c.pen_c[:] = [150., 150., 30., 30.]
     c.pen_mt, c.limit_k, c.limit_c = 0.2, 300., 3.
+    physics = dict(physics or {})
+    sc = self_collision_config(cfg, physics.pop("self_k", SELF_K), physics.pop("self_c", SELF_C))
     if physics:
         for k, v in physics.items():
             if hasattr(v, "__len__"):
@@ -306,4 +322,4 @@ def build_sim_config(cfg, num_envs=None, num_train_envs=None, seed=0, physics=No
         c.height_points_x[:len(px)] = px
         c.height_points_y[:len(py)] = py
     c.seed = int(seed)
-    return c, dict(active_reward_scales=active, dt=d["dt"], noise_scale_vec=nv)
+    return c, dict(active_reward_scales=active, dt=d["dt"], noise_scale_vec=nv, self_collision=sc)

@@ -15,7 +15,7 @@ from .config import load_actuator_weights
 
 
 class SimCore:
-    def __init__(self, sim_cfg: capi.Go1SimConfig, device="cuda:0", inject_noise=False, inject_reset_rand=False):
+    def __init__(self, sim_cfg: capi.Go1SimConfig, device="cuda:0", inject_noise=False, inject_reset_rand=False, self_collision=None):
         if not torch.cuda.is_available():
             raise capi.Go1Error("SimCore needs a CUDA device: the Go1 step kernel has no CPU fallback")
         self.L = capi.lib()
@@ -70,6 +70,9 @@ class SimCore:
         with torch.cuda.device(self.dev_index):
             capi.check(self.L.go1_sim_create(C.byref(sim_cfg), w.ctypes.data_as(C.c_void_p), self.dev_index, C.byref(self._handle)),
                        "go1_sim_create")
+        self.self_collision = self_collision
+        if self_collision is not None and self_collision.enabled:     # only before the first step (captured graphs keep the kernel)
+            capi.check(self.L.go1_sim_set_self_collision(self._handle, C.byref(self_collision)), "go1_sim_set_self_collision")
         self._bind()
         # DR defaults (legged_robot.py:1260-1278)
         self.env("motor_strengths").fill_(1.0)

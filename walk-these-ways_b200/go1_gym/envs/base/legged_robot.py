@@ -173,7 +173,7 @@ class LeggedRobot(BaseTask):
         self.up_axis_idx = 2
         if mesh_type in ['heightfield', 'trimesh']:
             self._bind_height_field()
-        self.core = SimCore(self.sim_cfg, device=self.device)
+        self.core = SimCore(self.sim_cfg, device=self.device, self_collision=info["self_collision"])
         self.num_dof = self.num_dofs = self.num_actuated_dof = 12
         self.num_bodies = 17
         self.dof_names = [f"{l}_{p}_joint" for l in ("FL", "FR", "RL", "RR") for p in ("hip", "thigh", "calf")]
