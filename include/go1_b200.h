@@ -26,6 +26,12 @@ extern "C" {
 #define GO1_EVENT_STRIDE 6        /* floats per event record */
 #define GO1_RESET_RAND_STRIDE 48  /* injected uniform draws per env (Go1SimBuffers.reset_rand) */
 #define GO1_MAX_LAG_TIMESTEPS 32  /* action FIFO slots reserved per leg in leg_f32 (3 rows each, "lag_buffer") */
+#define GO1_MAX_USER_REWARDS 32   /* user reward terms (go1_gym/envs/rewards) per go1_sim_reward_finish call */
+/* rows of the pre-roll slab of go1_sim_step_deferred: [GO1_PRE_ROLL_ROWS][4N] in leg_f32 layout, 3 rows (joints) per field */
+enum Go1PreRollRow {
+    GO1_PRE_ROLL_LAST_ACTIONS = 0, GO1_PRE_ROLL_LAST_LAST_ACTIONS = 3, GO1_PRE_ROLL_LAST_DOF_VEL = 6,
+    GO1_PRE_ROLL_LAST_JOINT_POS_TARGET = 9, GO1_PRE_ROLL_LAST_LAST_JOINT_POS_TARGET = 12, GO1_PRE_ROLL_ROWS = 15
+};
 
 /* reward term ids: one per CoRLRewards._reward_<name> (go1_gym/envs/rewards/corl_rewards.py:15-201) */
 enum Go1RewardTerm {
@@ -180,6 +186,38 @@ int go1_sim_update_config(Go1Sim* sim, const Go1SimConfig* cfg, void* stream);
  * no dynamics); 2 = post-physics only (test hook: physics outputs already in the buffers). */
 int go1_sim_step(Go1Sim* sim, const float* actions /*[N][12]*/, const float gravity[3],
                  const float gravity_vec[3], int64_t common_step, int mode, void* stream);
+
+/* ---- user reward terms (go1_gym/envs/rewards, DESIGN.md §4) ------------------------------------------------------------
+ * A step with K > 0 user terms is three launches instead of one: go1_sim_step_deferred, the user terms (torch, writing
+ * raw[K][N]), go1_sim_reward_finish.  The reset launches follow as usual, then go1_sim_user_reward_fold.
+ *
+ * go1_sim_step_deferred: go1_sim_step (mode 0) with two differences.  It also writes the values that last_actions,
+ * last_last_actions, last_dof_vel, last_joint_pos_target and last_last_joint_pos_target had before this step's rolls
+ * (legged_robot.py:126-131) to `pre_roll` ([GO1_PRE_ROLL_ROWS][4N]), which is what compute_reward sees.  It leaves rew = the
+ * plain sum of the built-in terms and rew_buf_pos / rew_buf_neg = their split; the combination, the termination term and
+ * the "total" episode sum are left to go1_sim_reward_finish. */
+int go1_sim_step_deferred(Go1Sim* sim, const float* actions /*[N][12]*/, const float gravity[3], const float gravity_vec[3],
+                          int64_t common_step, float* pre_roll, void* stream);
+
+/* Scratch floats go1_sim_reward_finish needs for `num_envs` envs and K user terms. */
+int64_t go1_reward_finish_workspace(int num_envs, int K);
+
+/* Finishes compute_reward (legged_robot.py:263-300) after go1_sim_step_deferred and the user terms.  raw: [K][N] user term
+ * values (before scaling), scales: K host floats (already multiplied by dt).  Each user term r = raw * scale is added to rew
+ * and to user_sums[k] ([K][N] episode sums), and to rew_buf_pos if its sum over all N envs is >= 0, else to rew_buf_neg if
+ * it is <= 0 (neither when the sum is NaN).  That sum is taken in a fixed order (per-CTA partials in `workspace`, summed in
+ * CTA order), so the sign does not depend on scheduling.  Then the combination of the config (only_positive_rewards /
+ * ji22 style / plain), the termination term and the "total" episode sum, as go1_sim_step does them.  Two launches. */
+int go1_sim_reward_finish(Go1Sim* sim, const float* raw, const float* scales, int K, float* user_sums, float* workspace, void* stream);
+
+/* The user-term part of reset_idx's episode bookkeeping (legged_robot.py:181-195) for the reset list `env_ids` (count k, or
+ * *k_dev when k_dev != NULL, as go1_sim_reset_idx_dev): acc[0..K-1] = sum of user_sums[k] over the reset train envs and acc[K] =
+ * their count (written, not added; fixed summation order); for reset eval envs, user_sums_eval[k] ([K][N], -1 = unset) keeps
+ * the first finished episode; the reset envs' user_sums are zeroed.  With acc_hist != NULL the result is also filed in
+ * acc_hist[*slot_dev] ([T][K+1]; a step without a reset train env carries the previous row forward, as go1_rollout_advance
+ * does for the built-in accumulator).  One CTA, no host synchronisation. */
+int go1_sim_user_reward_fold(Go1Sim* sim, const int32_t* env_ids, const int32_t* k_dev, int k, int K, float* user_sums,
+                             float* user_sums_eval, float* acc, float* acc_hist, int T, const int32_t* slot_dev, void* stream);
 
 /* Self-collisions between the robot's own links (DESIGN.md §3), the counterpart of Isaac Gym's
  * asset_options.self_collisions / PhysX's self-collision filter.  Thigh and calf are capsules (thigh joint -> knee, knee -> foot),

@@ -7,7 +7,10 @@
 #include "go1_layout.h"
 #include "go1_model_generated.h"
 
-extern "C" int go1_launch_step(const Go1SimBuffers*, const Go1DevTable*, const Go1SelfCollision*, const float*, const float*, const float*, long long, int, int, cudaStream_t);
+extern "C" int go1_launch_step(const Go1SimBuffers*, const Go1DevTable*, const Go1SelfCollision*, const float*, const float*, const float*, long long, int, int, float*, cudaStream_t);
+extern "C" int go1_launch_reward_finish(const Go1SimBuffers*, const Go1SimConfig*, const float*, const float*, int, float*, float*, int, cudaStream_t);
+extern "C" int go1_launch_user_reward_fold(const int*, const int*, int, int, float*, float*, float*, float*, int, const int*, int, int, cudaStream_t);
+extern "C" long long go1_reward_finish_workspace_floats(int, int);
 extern "C" int go1_launch_reset(const Go1SimBuffers*, const Go1DevTable*, const int*, int, const float*, const float*, int, long long, const float*, int, cudaStream_t);
 extern "C" int go1_launch_set_commands(const Go1SimBuffers*, const int*, int, const float*, int, cudaStream_t);
 extern "C" int go1_launch_reset_dev(const Go1SimBuffers*, const Go1DevTable*, const int*, const int*, const float*, const float*, int, long long, const float*, float*, int, cudaStream_t);
@@ -222,8 +225,41 @@ extern "C" int go1_sim_step(Go1Sim* s, const float* actions, const float gravity
     if (mode < 0 || mode > 2) return fail("go1_sim_step: bad mode");
     for (int k = 0; k < 3; k++) s->gravity[k] = gravity[k];
     s->stepped = 1;
-    int e = go1_launch_step(&s->bufs, s->d_tab, &s->self, actions, gravity, gravity_vec, (long long)common_step, mode, s->cfg.num_envs, (cudaStream_t)stream);
+    int e = go1_launch_step(&s->bufs, s->d_tab, &s->self, actions, gravity, gravity_vec, (long long)common_step, mode, s->cfg.num_envs, nullptr, (cudaStream_t)stream);
     return e ? cuda_fail("go1_sim_step launch", e) : 0;
+}
+
+extern "C" int go1_sim_step_deferred(Go1Sim* s, const float* actions, const float gravity[3], const float gravity_vec[3],
+                                     int64_t common_step, float* pre_roll, void* stream) {
+    if (!s || !s->bound) return fail("go1_sim_step_deferred: sim not bound");
+    if (!actions || !pre_roll) return fail("go1_sim_step_deferred: null actions / pre_roll");
+    for (int k = 0; k < 3; k++) s->gravity[k] = gravity[k];
+    s->stepped = 1;
+    int e = go1_launch_step(&s->bufs, s->d_tab, &s->self, actions, gravity, gravity_vec, (long long)common_step, 0, s->cfg.num_envs, pre_roll, (cudaStream_t)stream);
+    return e ? cuda_fail("go1_sim_step_deferred launch", e) : 0;
+}
+
+extern "C" int64_t go1_reward_finish_workspace(int num_envs, int K) {
+    return (num_envs <= 0 || K < 0) ? 0 : (int64_t)go1_reward_finish_workspace_floats(num_envs, K);
+}
+
+extern "C" int go1_sim_reward_finish(Go1Sim* s, const float* raw, const float* scales, int K, float* user_sums, float* workspace, void* stream) {
+    if (!s || !s->bound) return fail("go1_sim_reward_finish: sim not bound");
+    if (K < 1 || K > GO1_MAX_USER_REWARDS) return fail("go1_sim_reward_finish: K must be in 1..GO1_MAX_USER_REWARDS");
+    if (!raw || !scales || !user_sums || !workspace) return fail("go1_sim_reward_finish: null argument");
+    int e = go1_launch_reward_finish(&s->bufs, &s->cfg, raw, scales, K, user_sums, workspace, s->cfg.num_envs, (cudaStream_t)stream);
+    return e ? cuda_fail("go1_sim_reward_finish launch", e) : 0;
+}
+
+extern "C" int go1_sim_user_reward_fold(Go1Sim* s, const int32_t* env_ids, const int32_t* k_dev, int k, int K, float* user_sums,
+                                        float* user_sums_eval, float* acc, float* acc_hist, int T, const int32_t* slot_dev, void* stream) {
+    if (!s || !s->bound) return fail("go1_sim_user_reward_fold: sim not bound");
+    if (K < 1 || K > GO1_MAX_USER_REWARDS) return fail("go1_sim_user_reward_fold: K must be in 1..GO1_MAX_USER_REWARDS");
+    if (!env_ids || !user_sums || !acc || (!k_dev && (k < 0 || k > s->cfg.num_envs))) return fail("go1_sim_user_reward_fold: bad arguments");
+    if (acc_hist && (T <= 0 || !slot_dev)) return fail("go1_sim_user_reward_fold: acc_hist needs T > 0 and slot_dev");
+    int e = go1_launch_user_reward_fold(env_ids, k_dev, k, K, user_sums, user_sums_eval, acc, acc_hist, T, slot_dev,
+                                        s->cfg.num_train_envs, s->cfg.num_envs, (cudaStream_t)stream);
+    return e ? cuda_fail("go1_sim_user_reward_fold launch", e) : 0;
 }
 
 extern "C" int go1_sim_reset_idx(Go1Sim* s, const int32_t* env_ids, int k, const float* new_commands, const float* actions,

@@ -56,6 +56,9 @@ def bf16_pitch(width):
 
 RESET_RAND_STRIDE = 48
 MAX_LAG_TIMESTEPS = 32
+MAX_USER_REWARDS = 32
+PRE_ROLL_FIELDS = ["last_actions", "last_last_actions", "last_dof_vel", "last_joint_pos_target", "last_last_joint_pos_target"]   # 3 rows each
+PRE_ROLL_ROWS = 3 * len(PRE_ROLL_FIELDS)
 _i, _f = C.c_int32, C.c_float
 
 
@@ -221,6 +224,10 @@ def lib():
         "go1_sim_update_config": ([vp, C.POINTER(Go1SimConfig), vp], ip),
         "go1_sim_step": ([vp, vp, C.POINTER(_f * 3), C.POINTER(_f * 3), i64, ip, vp], ip),
         "go1_sim_reset_idx": ([vp, vp, ip, vp, vp, ip, i64, vp], ip),
+        "go1_sim_step_deferred": ([vp, vp, C.POINTER(_f * 3), C.POINTER(_f * 3), i64, vp, vp], ip),
+        "go1_reward_finish_workspace": ([ip, ip], i64),
+        "go1_sim_reward_finish": ([vp, vp, vp, ip, vp, vp, vp], ip),
+        "go1_sim_user_reward_fold": ([vp, vp, vp, ip, ip, vp, vp, vp, vp, ip, vp, vp], ip),
         "go1_sim_set_commands": ([vp, vp, ip, vp, vp], ip),
         "go1_sim_set_step_block": ([ip], None),
         "go1_sizeof_self_collision": ([], ip), "go1_sim_set_self_collision": ([vp, C.POINTER(Go1SelfCollision)], ip),

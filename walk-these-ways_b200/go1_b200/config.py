@@ -116,8 +116,16 @@ def noise_scale_vec(cfg):
     return np.concatenate(v).astype(np.float32)
 
 
-def reward_tables(cfg, dt):
-    """_prepare_reward_function: drop zero scales, multiply by dt, keep dict order (legged_robot.py:1394-1412)."""
+TASK_TERMS = ("tracking_lin_vel", "tracking_ang_vel", "tracking_contacts_shaped_force", "tracking_contacts_shaped_vel")
+
+
+def reward_tables(cfg, dt, container=None):
+    """_prepare_reward_function: drop zero scales, multiply by dt, keep dict order (legged_robot.py:1394-1412).
+
+    With a reward container class, each nonzero term is built-in when its `_reward_<name>` is the BuiltinReward marker of that
+    name (the kernel table), a user term when it is a plain method (`user`: name -> scale, in order; a built-in of that name is
+    left out of the table), and unknown when there is no such attribute.  Without one, the names of capi.REWARD_TERMS are the
+    built-ins.  Returns (active, order, table, unknown, user)."""
     scales = cfg_dict(cfg.reward_scales)
     order, table = [], np.zeros(capi.NUM_REWARD_TERMS, dtype=np.float32)
     active = {}
@@ -125,16 +133,27 @@ def reward_tables(cfg, dt):
         if sc == 0:
             continue
         active[name] = sc * dt
-    unknown = []
+    unknown, user = [], {}
     for name, sc in active.items():
-        if name not in capi.REWARD_TERMS:
-            unknown.append(name)
+        fn = getattr(container, "_reward_" + name, None) if container is not None else None
+        marker = getattr(fn, "builtin_term", None)
+        if name not in capi.REWARD_TERMS or (container is not None and marker != name):
+            if container is not None and marker is None and callable(fn):
+                if name in TASK_TERMS or name == "termination":
+                    raise ValueError(f"_reward_{name} cannot be overridden: "
+                                     + ("it feeds the command curriculum's command_sums" if name in TASK_TERMS
+                                        else "the termination term is added after the combination of the others"))
+                user[name] = sc
+            else:
+                unknown.append(name)
             continue
         tid = capi.REWARD_TERMS.index(name)
         table[tid] = np.float32(sc)
         if name != "termination":
             order.append(tid)
-    return active, order, table, unknown
+    if len(user) > capi.MAX_USER_REWARDS:
+        raise ValueError(f"{len(user)} user reward terms: at most {capi.MAX_USER_REWARDS}")
+    return active, order, table, unknown, user
 
 
 def _lo_span(rng):
@@ -198,9 +217,10 @@ def self_collision_config(cfg, k=SELF_K, c=SELF_C):
     return sc
 
 
-def build_sim_config(cfg, num_envs=None, num_train_envs=None, seed=0, physics=None, eval_cfg=None):
+def build_sim_config(cfg, num_envs=None, num_train_envs=None, seed=0, physics=None, eval_cfg=None, reward_container=None):
     """Resolve `cfg` (a Cfg-like class tree) into a Go1SimConfig.  `physics` overrides solver parameters; `eval_cfg` is the
-    second Cfg tree of the train/eval split (its randomisation / reset ranges apply to envs >= num_train_envs)."""
+    second Cfg tree of the train/eval split (its randomisation / reset ranges apply to envs >= num_train_envs);
+    `reward_container` is the reward container class whose user terms run beside the kernel (reward_tables)."""
     d = derive(cfg)
     if eval_cfg is not None:
         derive(eval_cfg)
@@ -270,7 +290,7 @@ def build_sim_config(cfg, num_envs=None, num_train_envs=None, seed=0, physics=No
                    ("body_velocity_ss", nm.body_velocity_range), ("gravity_ss", nm.gravity_range)):
         sc, sh = get_scale_shift(rng)
         getattr(c, k)[:] = [sc, sh]
-    active, order, table, unknown = reward_tables(cfg, d["dt"])
+    active, order, table, unknown, user = reward_tables(cfg, d["dt"], reward_container)
     for name in unknown:
         print(f"Warning: reward {'_reward_' + name} has nonzero coefficient but was not found!")   # legged_robot.py:1409
     c.reward_scale[:] = table.tolist()
@@ -322,4 +342,4 @@ def build_sim_config(cfg, num_envs=None, num_train_envs=None, seed=0, physics=No
         c.height_points_x[:len(px)] = px
         c.height_points_y[:len(py)] = py
     c.seed = int(seed)
-    return c, dict(active_reward_scales=active, dt=d["dt"], noise_scale_vec=nv, self_collision=sc)
+    return c, dict(active_reward_scales=active, user_reward_scales=user, dt=d["dt"], noise_scale_vec=nv, self_collision=sc)

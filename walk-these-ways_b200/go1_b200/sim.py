@@ -177,6 +177,27 @@ class SimCore:
         capi.check(self.L.go1_sim_step(self._handle, capi.ptr(actions), C.byref(self.gravity), C.byref(self.gravity_vec),
                                        int(common_step), int(mode), capi.stream_ptr()), "go1_sim_step")
 
+    def step_deferred(self, actions, pre_roll, common_step=0):
+        """step() for a step with user reward terms: the pre-roll last_* values go to `pre_roll` [PRE_ROLL_ROWS][4N], and rew /
+        rew_buf_pos / rew_buf_neg hold the built-in terms only until reward_finish()."""
+        assert actions.is_cuda and actions.dtype == torch.float32 and actions.is_contiguous() and actions.shape == (self.N, 12)
+        assert pre_roll.shape == (capi.PRE_ROLL_ROWS, 4 * self.N) and pre_roll.is_contiguous()
+        capi.check(self.L.go1_sim_step_deferred(self._handle, capi.ptr(actions), C.byref(self.gravity), C.byref(self.gravity_vec),
+                                                int(common_step), capi.ptr(pre_roll), capi.stream_ptr()), "go1_sim_step_deferred")
+
+    def reward_finish(self, raw, scales, user_sums, workspace):
+        """The user terms' values raw [K][N] into rew / rew_buf_pos / rew_buf_neg / the episode sums (go1_sim_reward_finish).
+        scales: ctypes float array of K."""
+        capi.check(self.L.go1_sim_reward_finish(self._handle, capi.ptr(raw), scales, raw.shape[0], capi.ptr(user_sums), capi.ptr(workspace),
+                                                capi.stream_ptr()), "go1_sim_reward_finish")
+
+    def user_reward_fold(self, ids, k_dev, k, user_sums, user_sums_eval, acc, acc_hist=None, slot=None):
+        """User episode sums of the reset envs `ids` (int32; count k or k_dev) -> acc [K+1] (+ acc_hist[slot]), then zeroed."""
+        T = acc_hist.shape[0] if acc_hist is not None else 0
+        capi.check(self.L.go1_sim_user_reward_fold(self._handle, capi.ptr(ids), capi.ptr(k_dev), int(k), user_sums.shape[0], capi.ptr(user_sums),
+                                                   capi.ptr(user_sums_eval), capi.ptr(acc), capi.ptr(acc_hist), T, capi.ptr(slot),
+                                                   capi.stream_ptr()), "go1_sim_user_reward_fold")
+
     EVENT_PREFIX = 48      # records per list copied speculatively together with the counters
 
     def fetch_events(self):

@@ -9,7 +9,12 @@ Per step:   [commands of envs due for the periodic resample -> go1_sim_set_comma
             host curriculum update/sample for the reset envs
             go1_sim_reset_idx (sparse: re-initialise those envs and write their observations)
 
+With user reward terms (go1_gym/envs/rewards) the step launch is go1_sim_step_deferred, the terms (torch) and
+go1_sim_reward_finish, and go1_sim_user_reward_fold follows the reset launch.
+
 Public attributes keep the reference's names and AoS shapes; they are views/copies of the SoA device state."""
+import ctypes
+
 import numpy as np
 import torch
 
@@ -115,6 +120,28 @@ def measured_heights_at(base_quat, base_pos, height_samples, terrain_cfg):
     return h.float() * t.vertical_scale
 
 
+class PreRollEnv:
+    """A reward container's `self.env`: the env, except that the fields the step rolls after compute_reward (legged_robot.py:126-131)
+    read as they were before this step's roll, from the slab go1_sim_step_deferred writes ([N, 12] copies, Isaac DOF order).
+    Those values are the ones of the last step; outside a step's user terms they are stale."""
+
+    _ROWS = {name: 3 * i for i, name in enumerate(capi.PRE_ROLL_FIELDS)}
+
+    def __init__(self, env, slab):
+        object.__setattr__(self, "_env", env)
+        object.__setattr__(self, "_slab", slab)
+
+    def __getattr__(self, name):
+        r = PreRollEnv._ROWS.get(name)
+        if r is None:
+            return getattr(self._env, name)
+        n = self._env.num_envs
+        return self._slab[r:r + 3].view(3, n, 4).permute(1, 2, 0).reshape(n, 12)
+
+    def __setattr__(self, name, value):
+        setattr(self._env, name, value)
+
+
 class LeggedRobot(BaseTask):
     def __init__(self, cfg: Cfg, sim_params, physics_engine, sim_device, headless, eval_cfg=None, initial_dynamics_dict=None):
         self.cfg = cfg
@@ -161,9 +188,13 @@ class LeggedRobot(BaseTask):
                 self.terrain = Terrain(cfg.terrain, self.num_train_envs)
         elif mesh_type not in (None, 'plane'):
             raise ValueError("Terrain mesh type not recognised. Allowed types are [None, plane, heightfield, trimesh]")
-        self.sim_cfg, info = build_sim_config(cfg, num_envs=self.num_envs, num_train_envs=self.num_train_envs, seed=seed, eval_cfg=ecfg)
+        from go1_gym.envs.rewards import REWARD_CONTAINERS
+        self._reward_container_cls = REWARD_CONTAINERS[cfg.rewards.reward_container_name]
+        self.sim_cfg, info = build_sim_config(cfg, num_envs=self.num_envs, num_train_envs=self.num_train_envs, seed=seed, eval_cfg=ecfg,
+                                              reward_container=self._reward_container_cls)
         self.dt = info["dt"]
         self.reward_scales = dict(info["active_reward_scales"])
+        self._user_reward_scales = dict(info["user_reward_scales"])
         self.obs_scales = cfg.obs_scales
         self.curriculum_thresholds = cfg_dict(cfg.curriculum_thresholds)
         cfg.command_ranges = cfg_dict(cfg.commands)
@@ -361,8 +392,59 @@ class LeggedRobot(BaseTask):
         self.lag_timesteps = self.cfg.domain_rand.lag_timesteps
 
     def _prepare_reward_function(self):
-        """legged_robot.py:1385-1429: names of the active terms (the kernel owns the arithmetic)."""
-        self.reward_names = [n for n in self.reward_scales if n != "termination" and n in capi.REWARD_TERMS]
+        """legged_robot.py:1385-1429: the reward container and the names of the active terms.  The kernel owns the arithmetic of the
+        built-in terms; user terms (plain `_reward_<name>` methods of the container, config.reward_tables) run in torch beside it."""
+        user = self._user_reward_scales
+        sc = self.sim_cfg.reward_scale
+        kernel = {n for i, n in enumerate(capi.REWARD_TERMS) if sc[i] != 0}
+        self.reward_names = [n for n in self.reward_scales if n != "termination" and (n in kernel or n in user)]
+        self.user_reward_names = list(user)
+        K, N, dev = len(user), self.num_envs, self.device
+        if K == 0:
+            self.reward_container = self._reward_container_cls(self)
+            return
+        self._pre_roll = torch.zeros(capi.PRE_ROLL_ROWS, 4 * N, device=dev)
+        self.reward_container = self._reward_container_cls(PreRollEnv(self, self._pre_roll))
+        self._user_fns = [getattr(self.reward_container, "_reward_" + n) for n in user]
+        self._user_scales = (ctypes.c_float * K)(*user.values())
+        self._user_raw = torch.zeros(K, N, device=dev)
+        self._user_sums = torch.zeros(K, N, device=dev)
+        self._user_sums_eval = torch.full((K, N), -1.0, device=dev) if self.num_eval_envs > 0 else None
+        self._reward_ws = torch.zeros(max(1, int(capi.lib().go1_reward_finish_workspace(N, K))), device=dev)
+
+    def _eval_user_rewards(self):
+        """compute_reward's loop for the user terms (legged_robot.py:270-279): raw values into _user_raw."""
+        for k, fn in enumerate(self._user_fns):
+            r = fn()
+            if not isinstance(r, torch.Tensor) or r.shape != (self.num_envs,):
+                raise ValueError(f"_reward_{self.user_reward_names[k]} must return a [num_envs] tensor, got "
+                                 f"{tuple(r.shape) if isinstance(r, torch.Tensor) else type(r).__name__}")
+            self._user_raw[k].copy_(r)
+
+    def _sim_step(self, actions, common_step):
+        """The step launch: go1_sim_step, or with user terms the deferred step, the terms and go1_sim_reward_finish."""
+        core = self.core
+        if not self.user_reward_names:
+            core.step(actions, common_step=common_step, mode=0)
+            return
+        core.step_deferred(actions, self._pre_roll, common_step=common_step)
+        self._eval_user_rewards()
+        core.reward_finish(self._user_raw, self._user_scales, self._user_sums, self._reward_ws)
+
+    def _user_rewards_capturable(self):
+        """Whether the user terms can run inside a captured CUDA graph (no host synchronisation, ...): a trial capture of the
+        terms alone, which executes nothing."""
+        g = torch.cuda.CUDAGraph()
+        try:
+            with torch.cuda.graph(g):
+                self._eval_user_rewards()
+            return True
+        except Exception as e:
+            import warnings
+            warnings.warn(f"user reward terms cannot be captured in a CUDA graph ({type(e).__name__}: {e}); the rollout runs "
+                          "launch by launch instead")
+            torch.cuda.synchronize()
+            return False
 
     # ------------------------------------------------------------------ reference attribute surface (views / copies)
     obs_buf = property(lambda s: s.core.obs)
@@ -417,6 +499,8 @@ class LeggedRobot(BaseTask):
     def episode_sums(self):
         es = self.core.env("episode_sums")
         d = {n: es[capi.REWARD_TERMS.index(n)] for n in self.reward_scales if n in capi.REWARD_TERMS}
+        for i, n in enumerate(self.user_reward_names):
+            d[n] = self._user_sums[i]
         d["total"] = es[capi.NUM_REWARD_TERMS]
         return d
 
@@ -427,6 +511,8 @@ class LeggedRobot(BaseTask):
         if ev is None:
             return {}
         d = {n: ev[capi.REWARD_TERMS.index(n)] for n in self.reward_scales if n in capi.REWARD_TERMS}
+        for i, n in enumerate(self.user_reward_names):
+            d[n] = self._user_sums_eval[i]
         d["total"] = ev[capi.NUM_REWARD_TERMS]
         return d
 
@@ -470,7 +556,7 @@ class LeggedRobot(BaseTask):
         if dc is not None:
             return self._step_device(dc, actions)
         self._apply_pending_interval_resample()
-        core.step(actions, common_step=self.common_step_counter, mode=0)
+        self._sim_step(actions, self.common_step_counter)
         rid, rsum, iid, isum = core.fetch_events()
         self._pending_interval = (iid, isum)
         self._post_physics_step_callback_host()
@@ -505,7 +591,7 @@ class LeggedRobot(BaseTask):
             self._sync_interval_events_after_ep_len_write()
         dc.to_device()
         dc.resample(1)
-        core.step(actions, common_step=self.common_step_counter, mode=0)
+        self._sim_step(actions, self.common_step_counter)
         dc.gather()
         self._post_physics_step_callback_host()
         acc = torch.zeros(capi.NUM_EPISODE_SUMS + 1, device=self.device)
@@ -516,8 +602,17 @@ class LeggedRobot(BaseTask):
         if prev is not None:
             torch.where(acc[capi.NUM_EPISODE_SUMS:] > 0, acc, prev, out=acc)
         self._episode_acc_prev = acc
+        user_acc = None
+        if self.user_reward_names:
+            K = len(self.user_reward_names)
+            user_acc = torch.empty(K + 1, device=self.device)
+            core.user_reward_fold(dc.out_ids, dc.out_count, 0, self._user_sums, self._user_sums_eval, user_acc)
+            prev = self.__dict__.get("_user_acc_prev")
+            if prev is not None:
+                torch.where(user_acc[K:] > 0, user_acc, prev, out=user_acc)
+            self._user_acc_prev = user_acc
         ex = self.extras
-        ex["train/episode"] = _LazyDict(self._episode_builder(acc, may_be_empty=True))
+        ex["train/episode"] = _LazyDict(self._episode_builder(acc, may_be_empty=True, user_acc=user_acc))
         if self.cfg.commands.command_curriculum:
             ex["env_bins"] = dc.env_bins_f32
             ex["curriculum/distribution"] = _LazyDict(self._distribution_builder())
@@ -724,13 +819,20 @@ class LeggedRobot(BaseTask):
             cmds = self._resample_commands_host(ids, sums)
         core.episode_acc.zero_()
         core.reset_idx(ids, cmds, actions=actions, post_step=post_step, common_step=self.common_step_counter)
+        self._user_acc = None
+        if self.user_reward_names:
+            self._user_acc = torch.empty(len(self.user_reward_names) + 1, device=self.device)
+            ids_dev = torch.as_tensor(ids, dtype=torch.int32).to(self.device)
+            core.user_reward_fold(ids_dev, None, len(ids), self._user_sums, self._user_sums_eval, self._user_acc)
         self._env_bins_dirty = True
         self._fill_extras(ids)
 
-    def _episode_builder(self, acc, may_be_empty=False):
+    def _episode_builder(self, acc, may_be_empty=False, user_acc=None):
         """extras["train/episode"] of legged_robot.py:180-229 from one snapshot `acc` of the device accumulators
-        (episode sums of the envs reset in that step + their count).  may_be_empty: no env has reset yet -> no entries."""
+        (episode sums of the envs reset in that step + their count; `user_acc` the same for the user terms).  may_be_empty: no env
+        has reset yet -> no entries."""
         core, env = self.core, self
+        user = {n: i for i, n in enumerate(self.user_reward_names)}
 
         def build_episode():
             if may_be_empty and float(acc[capi.NUM_EPISODE_SUMS]) == 0.0:
@@ -740,6 +842,9 @@ class LeggedRobot(BaseTask):
             for name in list(env.reward_scales) + ["total"]:
                 if name == "total":
                     ep["rew_total"] = means[capi.NUM_REWARD_TERMS]
+                elif name in user:
+                    if user_acc is not None:
+                        ep["rew_" + name] = user_acc[user[name]] / user_acc[len(user)].clamp(min=1.0)
                 elif name in capi.REWARD_TERMS:
                     ep["rew_" + name] = means[capi.REWARD_TERMS.index(name)]
             if env.cfg.terrain.curriculum:
@@ -773,7 +878,7 @@ class LeggedRobot(BaseTask):
         accumulators taken here (a clone, no host sync); the dict values are materialised when somebody reads them."""
         core, ex = self.core, self.extras
         if (ids < self.num_train_envs).any():
-            ex["train/episode"] = _LazyDict(self._episode_builder(core.episode_acc.clone()))
+            ex["train/episode"] = _LazyDict(self._episode_builder(core.episode_acc.clone(), user_acc=self.__dict__.get("_user_acc")))
         if (ids >= self.num_train_envs).any():
             ex["eval/episode"] = {}
         if self.cfg.commands.command_curriculum:

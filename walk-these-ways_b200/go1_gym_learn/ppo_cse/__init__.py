@@ -126,7 +126,8 @@ class Runner:
         ok = self.step_graph and os.environ.get("GO1_STEP_GRAPH", "1") != "0" and base is not None and hasattr(env, "_bufs") \
             and hasattr(base, "_device_curriculum") and self.env.num_eval_envs == 0 and self.alg.use_cuda_graph is True \
             and self.alg.actor_critic.injected_eps is None and str(self.device).startswith("cuda")
-        if ok and base._device_curriculum() is not None and base.cfg.commands.command_curriculum:
+        K = len(getattr(base, "user_reward_names", ()))
+        if ok and base._device_curriculum() is not None and base.cfg.commands.command_curriculum and (K == 0 or base._user_rewards_capturable()):
             from go1_b200 import capi
             dev, T = base.core.device, self.num_steps_per_env
             W = capi.NUM_EPISODE_SUMS + 1
@@ -134,6 +135,8 @@ class Runner:
                 st = dict(slot=torch.zeros(1, dtype=torch.int32, device=dev), acc=torch.zeros(W, device=dev),
                           acc_hist=torch.zeros(T, W, device=dev), graphs={}, warm={0: 0, 1: 0}, W=W, T=T,
                           fork=os.environ.get("GO1_STEP_FORK", "1") != "0")
+                if K:       # the user terms' extras["train/episode"] accumulator [K sums + count] and its per-step history
+                    st.update(acc_user=torch.zeros(K + 1, device=dev), acc_user_hist=torch.zeros(T, K + 1, device=dev))
         self._sg = st
         return st
 
@@ -170,11 +173,14 @@ class Runner:
             main.wait_event(e1)
         else:
             dc.resample(1)
-        core.step(actions, common_step=0, mode=0)
+        base._raw_actions = actions           # user reward terms read env.actions: this step's, from the tensor the graph writes
+        base._sim_step(actions, 0)
         dc.gather()
         sg["acc"].zero_()
         dc.resample(0)
         dc.reset_envs(actions, True, 0, sg["acc"])
+        if "acc_user" in sg:
+            core.user_reward_fold(dc.out_ids, dc.out_count, 0, base._user_sums, None, sg["acc_user"], sg["acc_user_hist"], sg["slot"])
         if fork:
             e2 = torch.cuda.Event(); e2.record(main)
         else:
@@ -269,8 +275,11 @@ class Runner:
         # extras / metrics of the whole rollout from ONE snapshot of the per-step accumulators
         acc_hist = sg["acc_hist"].clone()
         base._episode_acc_prev = acc_hist[-1]
+        user_hist = sg["acc_user_hist"].clone() if "acc_user_hist" in sg else [None] * self.num_steps_per_env
+        if "acc_user_hist" in sg:
+            base._user_acc_prev = user_hist[-1]
         ex = base.extras
-        ex["train/episode"] = _LazyDict(base._episode_builder(acc_hist[-1], may_be_empty=True))
+        ex["train/episode"] = _LazyDict(base._episode_builder(acc_hist[-1], may_be_empty=True, user_acc=user_hist[-1]))
         ex["env_bins"] = dc.env_bins_f32
         ex["curriculum/distribution"] = _LazyDict(base._distribution_builder())
         if base.cfg.env.send_timeouts:
@@ -278,7 +287,7 @@ class Runner:
         ex["privileged_obs"] = core.priv_obs
         if hasattr(logger, "store_metrics_lazy"):
             for t in range(self.num_steps_per_env):
-                logger.store_metrics_lazy('train/episode', _LazyDict(base._episode_builder(acc_hist[t], may_be_empty=True)))
+                logger.store_metrics_lazy('train/episode', _LazyDict(base._episode_builder(acc_hist[t], may_be_empty=True, user_acc=user_hist[t])))
         return core.obs, core.priv_obs, env.obs_history, ex
 
     def rollout(self, obs, privileged_obs, obs_history, eval_expert=False):
