@@ -441,9 +441,9 @@ __device__ __forceinline__ bool epilogue_prefetch(const GemmArgs& g, const int r
 // one [64 k][32 n] box, 64B-swizzled), two boxes per 128-wide tile 8 KB apart, and the tensor core reads them in place through its
 // transpose immediates: no shared-to-shared transposition.  ROW16: the epilogue can also store C row-major in BF16 (c16 without ct).
 constexpr int X_BYTES = 65536;
-template <int BN, bool ANYKIND, int CL, bool BF16, int AMN, int BMN, bool ROW16, bool DET = false>
+template <int BN, bool ANYKIND, int CL, bool BF16, int AMN, int BMN, bool ROW16, bool DET>
 __device__ __forceinline__ void gemm_wgmma_body(const GemmMaps& gm, const CUtensorMap& mapC, const CUtensorMap& mapY, const GemmArgs& g,
-                                                const int tiles_m, const int tiles_n, const int total_tiles, const int stages, const DetArgs* det = nullptr) {
+                                                const int tiles_m, const int tiles_n, const int total_tiles, const int stages, const DetArgs* det) {
     static_assert(CL == 1 || (CL == 2 && BN == BM), "CTA pairs share 128-row operand boxes");
     static_assert((AMN == 0 && BMN == 0 && !ROW16) || (BF16 && CL == 1), "MN-major BF16 operands and the row-major BF16 store: one CTA per tile");
     constexpr int G = EPI_G;
@@ -657,31 +657,20 @@ __device__ __forceinline__ void gemm_wgmma_body(const GemmMaps& gm, const CUtens
     if (CL > 1) cluster_sync();
 }
 
-template <int BN, bool ANYKIND, int CL, bool BF16>
+// DET (deterministic mode): the cross-CTA sums go to the workspace regions of det (DetArgs), left to go1_det_sum; the default instantiation
+// receives an empty det and adds into its targets
+template <int BN, bool ANYKIND, int CL, bool BF16, bool DET>
 __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma(const __grid_constant__ GemmMaps gm,
                                                                       const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
-                                                                      const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
-    gemm_wgmma_body<BN, ANYKIND, CL, BF16, 0, 0, false>(gm, mapC, mapY, g, tiles_m, tiles_n, total_tiles, stages);
+                                                                      const int tiles_m, const int tiles_n, const int total_tiles, const int stages, const DetArgs det) {
+    gemm_wgmma_body<BN, ANYKIND, CL, BF16, 0, 0, false, DET>(gm, mapC, mapY, g, tiles_m, tiles_n, total_tiles, stages, &det);
 }
 // BF16 operands in the majors AMN / BMN (1: MN-major), fp32 or row-major BF16 output (go1_gemm_bf16_mn / go1_gemm_bf16_grouped)
-template <int BN, bool ANYKIND, int AMN, int BMN>
+template <int BN, bool ANYKIND, int AMN, int BMN, bool DET>
 __global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_bf16_mn_wgmma(const __grid_constant__ GemmMaps gm,
                                                                          const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
-                                                                         const int tiles_m, const int tiles_n, const int total_tiles, const int stages) {
-    gemm_wgmma_body<BN, ANYKIND, 1, true, AMN, BMN, true>(gm, mapC, mapY, g, tiles_m, tiles_n, total_tiles, stages);
-}
-// the two kernels of the deterministic mode (DetArgs): the same products, their cross-CTA sums left to go1_det_sum
-template <int BN, bool ANYKIND, int CL, bool BF16>
-__global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_tf32_wgmma_det(const __grid_constant__ GemmMaps gm,
-                                                                          const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
-                                                                          const int tiles_m, const int tiles_n, const int total_tiles, const int stages, const DetArgs det) {
-    gemm_wgmma_body<BN, ANYKIND, CL, BF16, 0, 0, false, true>(gm, mapC, mapY, g, tiles_m, tiles_n, total_tiles, stages, &det);
-}
-template <int BN, bool ANYKIND, int AMN, int BMN>
-__global__ void __launch_bounds__(32 * NCONS + 128, 1) gemm_bf16_mn_wgmma_det(const __grid_constant__ GemmMaps gm,
-                                                                             const __grid_constant__ CUtensorMap mapC, const __grid_constant__ CUtensorMap mapY, const GemmArgs g,
-                                                                             const int tiles_m, const int tiles_n, const int total_tiles, const int stages, const DetArgs det) {
-    gemm_wgmma_body<BN, ANYKIND, 1, true, AMN, BMN, true, true>(gm, mapC, mapY, g, tiles_m, tiles_n, total_tiles, stages, &det);
+                                                                         const int tiles_m, const int tiles_n, const int total_tiles, const int stages, const DetArgs det) {
+    gemm_wgmma_body<BN, ANYKIND, 1, true, AMN, BMN, true, DET>(gm, mapC, mapY, g, tiles_m, tiles_n, total_tiles, stages, &det);
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -771,10 +760,9 @@ __global__ void bias_act_strided(float* C, int ldc, const float* bias, int M, in
     *c = v;
 }
 
-// MN < 0: gemm_tf32_wgmma<BN, ANYKIND, CL, BF16>; MN = 0..3: gemm_bf16_mn_wgmma<BN, ANYKIND, MN & 1, MN >> 1> (CL 1, BF16); det: their _det
-// kernels (deterministic mode)
-template <int BN, bool ANYKIND, int CL, bool BF16, int MN = -1, bool DET = false>
-int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st, const DetArgs* det = nullptr) {
+// MN < 0: gemm_tf32_wgmma<BN, ANYKIND, CL, BF16, DET>; MN = 0..3: gemm_bf16_mn_wgmma<BN, ANYKIND, MN & 1, MN >> 1, DET> (CL 1, BF16)
+template <int BN, bool ANYKIND, int CL, bool BF16, int MN, bool DET>
+int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st, const DetArgs& det) {
     constexpr int STAGE_BYTES = (BM + BN) * BK * 4;
     const size_t staging = X_BYTES + (g.tma_aux ? (size_t)NCONS * 4096 : 0);
     const size_t fixed = staging + (2 * 8 + NCONS) * 8 + 16 + 1024;
@@ -785,13 +773,8 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
     const size_t smem = (size_t)stages * STAGE_BYTES + fixed;
     static_assert(MN < 0 || (CL == 1 && BF16), "the MN-major BF16 kernel runs one CTA per tile");
     auto kernel = [] {
-        if constexpr (DET) {
-            if constexpr (MN < 0) return gemm_tf32_wgmma_det<BN, ANYKIND, CL, BF16>;
-            else return gemm_bf16_mn_wgmma_det<BN, ANYKIND, (MN & 1), (MN >> 1)>;
-        } else {
-            if constexpr (MN < 0) return gemm_tf32_wgmma<BN, ANYKIND, CL, BF16>;
-            else return gemm_bf16_mn_wgmma<BN, ANYKIND, (MN & 1), (MN >> 1)>;
-        }
+        if constexpr (MN < 0) return gemm_tf32_wgmma<BN, ANYKIND, CL, BF16, DET>;
+        else return gemm_bf16_mn_wgmma<BN, ANYKIND, (MN & 1), (MN >> 1), DET>;
     }();
     const int tiles_m = (g.M + BM - 1) / BM, tiles_n = (g.N + BN - 1) / BN;
     g.tiles_per_prob = tiles_m * tiles_n * splits;
@@ -821,18 +804,10 @@ int launch_gemm(const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my
     // persistent grid: one CTA per SM (the ring and the staging fill its shared memory), CL x (pair-)tile slots for clusters
     const int units = total / CL;
     cfg.gridDim = dim3(CL * (units < slots ? units : slots));
-    if constexpr (DET) {
-        if (CL == 1) kernel<<<cfg.gridDim, cfg.blockDim, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages, *det);
-        else {
-            cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, gm, mc, my, g, tiles_m, tiles_n, total, stages, *det);
-            if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
-        }
-    } else {
-        if (CL == 1) kernel<<<cfg.gridDim, cfg.blockDim, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages);
-        else {
-            cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, gm, mc, my, g, tiles_m, tiles_n, total, stages);
-            if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
-        }
+    if (CL == 1) kernel<<<cfg.gridDim, cfg.blockDim, smem, st>>>(gm, mc, my, g, tiles_m, tiles_n, total, stages, det);
+    else {
+        cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, gm, mc, my, g, tiles_m, tiles_n, total, stages, det);
+        if (e != cudaSuccess) return go1_set_error(cudaGetErrorString(e));
     }
     go1_count_launch(1);
     return 0;
@@ -1189,7 +1164,7 @@ extern "C" int go1_gemm_timing(int on, double* total_ms, double* total_flop, lon
 
 // the MN-major BF16 kernel of layout mn (bit 0: A MN-major, bit 1: B MN-major)
 template <int BN, bool ANYKIND, bool DET>
-int launch_gemm_mn(int mn, const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st, const DetArgs* det) {
+int launch_gemm_mn(int mn, const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st, const DetArgs& det) {
     switch (mn) {
         case 0: return launch_gemm<BN, ANYKIND, 1, true, 0, DET>(gm, mc, my, g, splits, st, det);
         case 1: return launch_gemm<BN, ANYKIND, 1, true, 1, DET>(gm, mc, my, g, splits, st, det);
@@ -1200,7 +1175,7 @@ int launch_gemm_mn(int mn, const GemmMaps& gm, const CUtensorMap& mc, const CUte
 // the kernel of (mnk, cluster, BN, any) in the default or the deterministic instantiation
 template <bool BF16, bool DET>
 int launch_gemm_any(int mnk, int cluster, int BN, bool any, const GemmMaps& gm, const CUtensorMap& mc, const CUtensorMap& my, GemmArgs& g, int splits, cudaStream_t st,
-                    const DetArgs* det) {
+                    const DetArgs& det) {
     if (mnk >= 0) {
         if constexpr (BF16) {
             if (BN == 128) return any ? launch_gemm_mn<128, true, DET>(mnk, gm, mc, my, g, splits, st, det) : launch_gemm_mn<128, false, DET>(mnk, gm, mc, my, g, splits, st, det);
@@ -1287,7 +1262,7 @@ static int gemm_wgmma_impl(int transA, int transB, int M, int N, int K, int npro
         if (int e = tiles_n % 2 == 0 ? make_map(&gm.half, As[0], M, K, lda, BM / 2, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES)
                                      : make_map(&gm.half, Bs[0], N, K, ldb, BN / 2, KE, CU_TENSOR_MAP_SWIZZLE_128B, ES)) return e;
     }
-    // deterministic mode: the launches whose CTAs add into shared targets run their _det kernels, whose partials go to the stream's workspace
+    // deterministic mode: the launches whose CTAs add into shared targets run their DET kernels, whose partials go to the stream's workspace
     const bool det = go1_det_on() && (splits > 1 || g.colsum || (g.nbx > 0 && (g.gwx || g.dx)));
     DetArgs da = {};
     if (det) {
@@ -1335,8 +1310,8 @@ static int gemm_wgmma_impl(int transA, int transB, int M, int N, int K, int npro
         }
     }
     const bool any = g.act != 0 && g.kind != GO1_ACT_ELU;
-    e = det ? launch_gemm_any<BF16, true>(mnk, cluster, BN, any, gm, mc, my, g, splits, st, &da)
-            : launch_gemm_any<BF16, false>(mnk, cluster, BN, any, gm, mc, my, g, splits, st, nullptr);
+    e = det ? launch_gemm_any<BF16, true>(mnk, cluster, BN, any, gm, mc, my, g, splits, st, da)
+            : launch_gemm_any<BF16, false>(mnk, cluster, BN, any, gm, mc, my, g, splits, st, da);
     if (e) return e;
     if (det) {      // the partials, in a fixed order, into C (split-K: overwriting it unless accumulate) and the epilogue's targets (adding)
         if (splits > 1)

@@ -32,6 +32,8 @@ static int cuda_rc(const char* what) {
 // shared memory so global loads/stores stay coalesced along the env axis.  T <= 32 per pass; longer
 // rollouts chain passes through the carry.
 // ---------------------------------------------------------------------------------------------
+// DET (deterministic mode, go1_set_deterministic): stats is the workspace, and the block's two statistics go to stats[2 blockIdx.x ..]
+template <bool DET>
 __global__ void __launch_bounds__(1024) gae_kernel(const float* __restrict__ rew, const uint8_t* __restrict__ done,
                                                    const float* __restrict__ val, const float* __restrict__ last_val,
                                                    float* __restrict__ ret, float* __restrict__ adv, double* __restrict__ stats,
@@ -92,73 +94,10 @@ __global__ void __launch_bounds__(1024) gae_kernel(const float* __restrict__ rew
     if (w == 0) {
         double a = s_red[0][lane], b = s_red[1][lane];
         for (int d = 16; d > 0; d >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, d); b += __shfl_xor_sync(0xffffffffu, b, d); }
-        if (lane == 0) { atomicAdd(stats, a); atomicAdd(stats + 1, b); }
-    }
-}
-
-// gae_kernel of the deterministic mode (go1_set_deterministic): the block's two statistics go to parts[2 blockIdx.x ..], which go1_det_sum64
-// adds in block order.  (A copy, not a shared template body: the default kernels keep their code generation.)
-__global__ void __launch_bounds__(1024) gae_det_kernel(const float* __restrict__ rew, const uint8_t* __restrict__ done,
-                                                       const float* __restrict__ val, const float* __restrict__ last_val,
-                                                       float* __restrict__ ret, float* __restrict__ adv, double* __restrict__ parts,
-                                                       int T, int n, float gamma, float lam) {
-    __shared__ float s_a[32][33], s_b[32][33], s_v[32][33];
-    __shared__ double s_red[2][32];
-    const int lane = threadIdx.x, w = threadIdx.y;        // block = (32, 32)
-    const int env0 = blockIdx.x * 32;
-    double lsum = 0.0, lsq = 0.0;
-    float carry = 0.f;                                     // A_{t+1} entering the current chunk (per env = per warp)
-    for (int t_hi = T; t_hi > 0; t_hi -= 32) {
-        const int t_lo = max(t_hi - 32, 0), len = t_hi - t_lo;
-        // load: thread (lane = env offset, w = time offset) -> coalesced over envs
-        {
-            const int t = t_lo + w, e = env0 + lane;
-            float a = 0.f, b = 0.f, v = 0.f;
-            if (w < len && e < n) {
-                const size_t i = (size_t)t * n + e;
-                v = val[i];
-                const float nv = (t == T - 1) ? last_val[e] : val[i + n];
-                const float nt = 1.0f - (float)done[i];
-                b = rew[i] + nt * gamma * nv - v;          // delta_t
-                a = nt * gamma * lam;                      // c_t
-            }
-            s_a[w][lane] = a; s_b[w][lane] = b; s_v[w][lane] = v;
+        if (lane == 0) {
+            if constexpr (DET) { stats[2 * blockIdx.x] = a; stats[2 * blockIdx.x + 1] = b; }
+            else { atomicAdd(stats, a); atomicAdd(stats + 1, b); }
         }
-        __syncthreads();
-        // scan: warp w = env offset, lane j = reversed time (j = 0 is the last step of the chunk)
-        {
-            const int tt = len - 1 - lane;
-            float a = (lane < len) ? s_a[tt][w] : 1.f, b = (lane < len) ? s_b[tt][w] : 0.f;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const float ap = __shfl_up_sync(0xffffffffu, a, d), bp = __shfl_up_sync(0xffffffffu, b, d);
-                if (lane >= d) { b = b + a * bp; a = a * ap; }
-            }
-            const float A = b + a * carry;                 // advantage at time t_lo + tt
-            if (lane < len) s_b[tt][w] = A;
-            carry = __shfl_sync(0xffffffffu, A, len - 1);  // A at t_lo feeds the next (earlier) chunk
-        }
-        __syncthreads();
-        {
-            const int t = t_lo + w, e = env0 + lane;
-            if (w < len && e < n) {
-                const size_t i = (size_t)t * n + e;
-                const float A = s_b[w][lane];
-                ret[i] = A + s_v[w][lane];
-                adv[i] = A;                                // == returns - values (rollout_storage.py:87)
-                lsum += (double)A; lsq += (double)A * (double)A;
-            }
-        }
-        __syncthreads();
-    }
-    // block reduce of the statistics
-    for (int d = 16; d > 0; d >>= 1) { lsum += __shfl_xor_sync(0xffffffffu, lsum, d); lsq += __shfl_xor_sync(0xffffffffu, lsq, d); }
-    if (lane == 0) { s_red[0][w] = lsum; s_red[1][w] = lsq; }
-    __syncthreads();
-    if (w == 0) {
-        double a = s_red[0][lane], b = s_red[1][lane];
-        for (int d = 16; d > 0; d >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, d); b += __shfl_xor_sync(0xffffffffu, b, d); }
-        if (lane == 0) { parts[2 * blockIdx.x] = a; parts[2 * blockIdx.x + 1] = b; }
     }
 }
 __global__ void normalize_adv_kernel(float* __restrict__ adv, const double* __restrict__ stats, long long global_count, long long local_count) {
@@ -174,16 +113,14 @@ extern "C" int go1_ppo_gae(const float* rewards, const uint8_t* dones, const flo
     if (!rewards || !dones || !values || !last_values || !returns || !advantages || !stats || T <= 0 || n <= 0) return go1_set_error("go1_ppo_gae: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
     const int nb = (n + 31) / 32;
-    if (go1_det_on()) {
-        double* parts = (double*)go1_det_workspace(st, sizeof(double) * 2 * nb);
-        if (!parts) return 1;
-        gae_det_kernel<<<nb, dim3(32, 32), 0, st>>>(rewards, dones, values, last_values, returns, advantages, parts, T, n, gamma, lam); go1_count_launch(1);
-        if (int e = cuda_rc("go1_ppo_gae")) return e;
-        return go1_det_sum64(parts, nb, 2, stats, 2, 0, st);
-    }
-    cudaMemsetAsync(stats, 0, 2 * sizeof(double), st);
-    gae_kernel<<<nb, dim3(32, 32), 0, st>>>(rewards, dones, values, last_values, returns, advantages, stats, T, n, gamma, lam); go1_count_launch(1);
-    return cuda_rc("go1_ppo_gae");
+    const bool det = go1_det_on();     // deterministic mode: the blocks' statistics meet in stats in block order
+    double* out = go1_det_out(det, st, 2 * (size_t)nb, stats);
+    if (det && !out) return 1;
+    if (!det) cudaMemsetAsync(stats, 0, 2 * sizeof(double), st);
+    (det ? gae_kernel<true> : gae_kernel<false>)<<<nb, dim3(32, 32), 0, st>>>(rewards, dones, values, last_values, returns, advantages, out, T, n, gamma, lam);
+    go1_count_launch(1);
+    if (int e = cuda_rc("go1_ppo_gae")) return e;
+    return det ? go1_det_sum64(out, nb, 2, stats, 2, 0, st) : 0;
 }
 extern "C" int go1_ppo_normalize_advantages(float* advantages, const double* stats, int64_t global_count, int64_t local_count, void* stream) {
     if (!advantages || !stats || global_count < 2 || local_count <= 0) return go1_set_error("go1_ppo_normalize_advantages: bad arguments");
@@ -215,9 +152,9 @@ struct SgemmEp { const float* ex; const float* wex; const float* aux; int ldex, 
 
 // DET: a split's partial tile goes to part[split][M][N] (plain stores; go1_det_sum adds the splits into C)
 template <int TA, int TB, bool DET>
-__device__ __forceinline__ void sgemm_body(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                                           float* __restrict__ Cm, int ldc, const float* __restrict__ bias,
-                                           int M, int N, int K, int act, int kind, int accumulate, int kchunk, const SgemmEp& ep, float* __restrict__ part) {
+__global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
+                                                    float* __restrict__ Cm, int ldc, const float* __restrict__ bias,
+                                                    int M, int N, int K, int act, int kind, int accumulate, int kchunk, const SgemmEp ep, float* __restrict__ part) {
     constexpr int BM = 128, BN = 128, BK = 8;
     __shared__ float As[2][BK][BM + 4], Bs[2][BK][BN + 4];
     const int tid = threadIdx.x;
@@ -315,18 +252,6 @@ __device__ __forceinline__ void sgemm_body(const float* __restrict__ A, int lda,
         }
     }
 }
-template <int TA, int TB>
-__global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                                                    float* __restrict__ Cm, int ldc, const float* __restrict__ bias,
-                                                    int M, int N, int K, int act, int kind, int accumulate, int kchunk, const SgemmEp ep) {
-    sgemm_body<TA, TB, false>(A, lda, B, ldb, Cm, ldc, bias, M, N, K, act, kind, accumulate, kchunk, ep, nullptr);
-}
-template <int TA, int TB>
-__global__ void __launch_bounds__(256) sgemm_det_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb,
-                                                        float* __restrict__ Cm, int ldc, const float* __restrict__ bias,
-                                                        int M, int N, int K, int act, int kind, int accumulate, int kchunk, const SgemmEp ep, float* __restrict__ part) {
-    sgemm_body<TA, TB, true>(A, lda, B, ldb, Cm, ldc, bias, M, N, K, act, kind, accumulate, kchunk, ep, part);
-}
 
 __global__ void bias_act_kernel(float* __restrict__ Cm, int ldc, const float* __restrict__ bias, int M, int N, int act, int kind) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -370,24 +295,20 @@ extern "C" int go1_gemm_ex(int transA, int transB, int M, int N, int K, const fl
     int kchunk = ((K + splitk - 1) / splitk + 7) / 8 * 8;
     splitk = (K + kchunk - 1) / kchunk;
     dim3 grid((N + 127) / 128, (M + 127) / 128, splitk);
-    if (splitk > 1 && go1_det_on()) {      // deterministic mode: the splits' partial tiles meet in C in split order
-        float* part = (float*)go1_det_workspace(st, sizeof(float) * (size_t)splitk * M * N);
-        if (!part) return 1;
-#define LAUNCH(TA, TB) sgemm_det_kernel<TA, TB><<<grid, 256, 0, st>>>(A, lda, B, ldb, Cm, ldc, bias, M, N, K, act, kind, accumulate, kchunk, ep, part)
-        if (!transA && !transB) LAUNCH(0, 0); else if (!transA && transB) LAUNCH(0, 1); else if (transA && !transB) LAUNCH(1, 0); else LAUNCH(1, 1);
-        go1_count_launch(1);
+    const bool det = splitk > 1 && go1_det_on();      // deterministic mode: the splits' partial tiles meet in C in split order
+    float* part = go1_det_out<float>(det, st, (size_t)splitk * M * N, nullptr);
+    if (det && !part) return 1;
+    if (splitk > 1 && !accumulate && !det) {
+        const size_t tot = (size_t)M * N;
+        zero_strided_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cm, ldc, M, N); go1_count_launch(1);
+    }
+#define LAUNCH(TA, TB) (det ? sgemm_kernel<TA, TB, true> : sgemm_kernel<TA, TB, false>)<<<grid, 256, 0, st>>>(A, lda, B, ldb, Cm, ldc, bias, M, N, K, act, kind, accumulate, kchunk, ep, part)
+    if (!transA && !transB) LAUNCH(0, 0); else if (!transA && transB) LAUNCH(0, 1); else if (transA && !transB) LAUNCH(1, 0); else LAUNCH(1, 1);
+    go1_count_launch(1);
 #undef LAUNCH
+    if (det) {
         if (int e = cuda_rc("go1_gemm")) return e;
         if (int e = go1_det_sum(part, splitk, (size_t)M * N, Cm, M, N, ldc, accumulate, st)) return e;
-    } else {
-        if (splitk > 1 && !accumulate) {
-            const size_t tot = (size_t)M * N;
-            zero_strided_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(Cm, ldc, M, N); go1_count_launch(1);
-        }
-#define LAUNCH(TA, TB) sgemm_kernel<TA, TB><<<grid, 256, 0, st>>>(A, lda, B, ldb, Cm, ldc, bias, M, N, K, act, kind, accumulate, kchunk, ep)
-        if (!transA && !transB) LAUNCH(0, 0); else if (!transA && transB) LAUNCH(0, 1); else if (transA && !transB) LAUNCH(1, 0); else LAUNCH(1, 1);
-        go1_count_launch(1);
-#undef LAUNCH
     }
     if (splitk > 1 && (bias || act)) {
         const size_t tot = (size_t)M * N;
@@ -588,8 +509,8 @@ extern "C" int go1_elu_backward(const float* y, int ldy, const float* dy, int ld
 // partial sums in registers over a 64-row slab (x read once, coalesced; dz rows broadcast), then o atomics.
 // DET: the slab's sums go to part[blockIdx.y][o][K] instead of gW (plain stores; go1_det_sum adds the slabs)
 template <int O, bool DET>
-__device__ __forceinline__ void skinny_wgrad_body(const float* __restrict__ dz, int lddz, const float* __restrict__ x, int ldx,
-                                                  float* __restrict__ gW, int ldg, int M, int o, int K, int rows_per_block, float* __restrict__ part) {
+__global__ void __launch_bounds__(128) skinny_wgrad_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ x, int ldx,
+                                                           float* __restrict__ gW, int ldg, int M, int o, int K, int rows_per_block, float* __restrict__ part) {
     const int k = blockIdx.x * 128 + threadIdx.x;
     const int r0 = blockIdx.y * rows_per_block, r1 = min(M, r0 + rows_per_block);
     if (k >= K) return;
@@ -610,22 +531,15 @@ __device__ __forceinline__ void skinny_wgrad_body(const float* __restrict__ dz, 
         }
     }
 }
-template <int O>
-__global__ void __launch_bounds__(128) skinny_wgrad_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ x, int ldx,
-                                                           float* __restrict__ gW, int ldg, int M, int o, int K, int rows_per_block) {
-    skinny_wgrad_body<O, false>(dz, lddz, x, ldx, gW, ldg, M, o, K, rows_per_block, nullptr);
-}
-template <int O>
-__global__ void __launch_bounds__(128) skinny_wgrad_det_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ x, int ldx,
-                                                               int M, int o, int K, int rows_per_block, float* __restrict__ part) {
-    skinny_wgrad_body<O, true>(dz, lddz, x, ldx, nullptr, 0, M, o, K, rows_per_block, part);
-}
 // float4 variant: a warp owns rows (stride 8 inside a row slab), lanes own 4 consecutive input columns; the o gradients of
 // a row are fetched by the first o lanes and shuffle-broadcast.  Per-block partial sums meet in shared memory, then one
 // set of global atomics per block.
-template <int O>
+// DET: the warps add their sums into s_acc one after the other, the bias-gradient sums meet in s_gb in warp order, and the block's
+// results go to part[blockIdx.y][o][K] and (gb: only whether there is one) part_gb[blockIdx.y][o] (plain stores; go1_det_sum adds the slabs)
+template <int O, bool DET>
 __global__ void __launch_bounds__(256) skinny_wgrad4_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ x, int ldx,
-                                                            float* __restrict__ gW, int ldg, float* __restrict__ gb, int M, int o, int K, int rows_per_block) {
+                                                            float* __restrict__ gW, int ldg, float* __restrict__ gb, int M, int o, int K, int rows_per_block,
+                                                            float* __restrict__ part, float* __restrict__ part_gb) {
     __shared__ float s_acc[O][128];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const int k = blockIdx.x * 128 + lane * 4;
@@ -648,65 +562,39 @@ __global__ void __launch_bounds__(256) skinny_wgrad4_kernel(const float* __restr
             acc[j][2] = fmaf(d, xv.z, acc[j][2]); acc[j][3] = fmaf(d, xv.w, acc[j][3]);
         }
     }
+    if constexpr (DET) {
+        __shared__ float s_gb[8][16];
+        for (int ww = 0; ww < 8; ww++) {
+            if (w == ww) {
 #pragma unroll
-    for (int j = 0; j < O; j++)
+                for (int j = 0; j < O; j++)
 #pragma unroll
-        for (int c = 0; c < 4; c++) atomicAdd(&s_acc[j][lane * 4 + c], acc[j][c]);
-    __syncthreads();
-    for (int i = threadIdx.x; i < o * 128; i += 256) {
-        const int j = i >> 7, kk = blockIdx.x * 128 + (i & 127);
-        if (kk < K) atomicAdd(gW + (size_t)j * ldg + kk, s_acc[j][i & 127]);
-    }
-    if (gb && blockIdx.x == 0 && lane < o) atomicAdd(gb + lane, dsum);
-}
-// skinny_wgrad4_kernel of the deterministic mode (a copy, as gae_det_kernel): the warps add their sums into s_acc one after the other, the
-// bias-gradient sums meet in s_gb in warp order, and the block's results go to part[blockIdx.y][o][K] and part_gb[blockIdx.y][o] (gb: only
-// whether there is one), which go1_det_sum adds in slab order
-template <int O>
-__global__ void __launch_bounds__(256) skinny_wgrad4_det_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ x, int ldx, const float* gb,
-                                                                int M, int o, int K, int rows_per_block, float* __restrict__ part, float* __restrict__ part_gb) {
-    __shared__ float s_acc[O][128];
-    __shared__ float s_gb[8][16];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const int k = blockIdx.x * 128 + lane * 4;
-    const int r0 = blockIdx.y * rows_per_block, r1 = min(M, r0 + rows_per_block);
-    for (int i = threadIdx.x; i < O * 128; i += 256) (&s_acc[0][0])[i] = 0.f;
-    __syncthreads();
-    float acc[O][4];
-#pragma unroll
-    for (int j = 0; j < O; j++) { acc[j][0] = 0.f; acc[j][1] = 0.f; acc[j][2] = 0.f; acc[j][3] = 0.f; }
-    float dsum = 0.f;          // lane j < o: sum over this warp's rows of dz[m][j] (the layer's bias gradient, reduced by the column-block-0 CTAs)
-#pragma unroll 2
-    for (int m = r0 + w; m < r1; m += 8) {
-        const float4 xv = k < K ? *reinterpret_cast<const float4*>(x + (size_t)m * ldx + k) : make_float4(0.f, 0.f, 0.f, 0.f);
-        const float dl = lane < o ? __ldg(dz + (size_t)m * lddz + lane) : 0.f;
-        dsum += dl;
-#pragma unroll
-        for (int j = 0; j < O; j++) {
-            const float d = __shfl_sync(0xffffffffu, dl, j);
-            acc[j][0] = fmaf(d, xv.x, acc[j][0]); acc[j][1] = fmaf(d, xv.y, acc[j][1]);
-            acc[j][2] = fmaf(d, xv.z, acc[j][2]); acc[j][3] = fmaf(d, xv.w, acc[j][3]);
+                    for (int c = 0; c < 4; c++) s_acc[j][lane * 4 + c] += acc[j][c];
+            }
+            __syncthreads();
         }
-    }
-    for (int ww = 0; ww < 8; ww++) {
-        if (w == ww) {
-#pragma unroll
-            for (int j = 0; j < O; j++)
-#pragma unroll
-                for (int c = 0; c < 4; c++) s_acc[j][lane * 4 + c] += acc[j][c];
-        }
+        if (lane < 16) s_gb[w][lane] = dsum;
         __syncthreads();
-    }
-    if (lane < 16) s_gb[w][lane] = dsum;
-    __syncthreads();
-    for (int i = threadIdx.x; i < o * 128; i += 256) {
-        const int j = i >> 7, kk = blockIdx.x * 128 + (i & 127);
-        if (kk < K) part[((size_t)blockIdx.y * o + j) * K + kk] = s_acc[j][i & 127];
-    }
-    if (gb && blockIdx.x == 0 && threadIdx.x < o) {
-        float t = s_gb[0][threadIdx.x];
-        for (int k = 1; k < 8; k++) t += s_gb[k][threadIdx.x];
-        part_gb[(size_t)blockIdx.y * o + threadIdx.x] = t;
+        for (int i = threadIdx.x; i < o * 128; i += 256) {
+            const int j = i >> 7, kk = blockIdx.x * 128 + (i & 127);
+            if (kk < K) part[((size_t)blockIdx.y * o + j) * K + kk] = s_acc[j][i & 127];
+        }
+        if (gb && blockIdx.x == 0 && threadIdx.x < o) {
+            float t = s_gb[0][threadIdx.x];
+            for (int k = 1; k < 8; k++) t += s_gb[k][threadIdx.x];
+            part_gb[(size_t)blockIdx.y * o + threadIdx.x] = t;
+        }
+    } else {
+#pragma unroll
+        for (int j = 0; j < O; j++)
+#pragma unroll
+            for (int c = 0; c < 4; c++) atomicAdd(&s_acc[j][lane * 4 + c], acc[j][c]);
+        __syncthreads();
+        for (int i = threadIdx.x; i < o * 128; i += 256) {
+            const int j = i >> 7, kk = blockIdx.x * 128 + (i & 127);
+            if (kk < K) atomicAdd(gW + (size_t)j * ldg + kk, s_acc[j][i & 127]);
+        }
+        if (gb && blockIdx.x == 0 && lane < o) atomicAdd(gb + lane, dsum);
     }
 }
 extern "C" int go1_skinny_wgrad_ex(const float* dz, int lddz, const float* x, int ldx, float* gW, int ldg, float* gb, int M, int o, int K, int accumulate, void* stream) {
@@ -718,48 +606,28 @@ extern "C" int go1_skinny_wgrad_ex(const float* dz, int lddz, const float* x, in
         else cudaMemset2DAsync(gW, sizeof(float) * ldg, 0, sizeof(float) * K, o, st);
         if (gb) cudaMemsetAsync(gb, 0, sizeof(float) * (size_t)o, st);
     }
-    const bool det = go1_det_on();
-    if ((K & 3) == 0 && (ldx & 3) == 0 && (((uintptr_t)x) & 15) == 0) {
-        const int kb = (K + 127) / 128;
-        int rpb4 = (M * kb + 131) / 132;                 // about one block per SM (the per-block reduction and atomics dominate with more)
-        rpb4 = (rpb4 + 7) / 8 * 8; if (rpb4 < 8) rpb4 = 8;
-        dim3 grid4(kb, (M + rpb4 - 1) / rpb4);
-        if (det) {      // deterministic mode: the row slabs' sums meet in gW / gb in slab order
-            const size_t nw = (size_t)grid4.y * o * K;
-            float* part = (float*)go1_det_workspace(st, sizeof(float) * (nw + (size_t)grid4.y * o));
-            if (!part) return 1;
-            float* part_gb = part + nw;
-            if (o <= 2) skinny_wgrad4_det_kernel<2><<<grid4, 256, 0, st>>>(dz, lddz, x, ldx, gb, M, o, K, rpb4, part, part_gb);
-            else if (o <= 4) skinny_wgrad4_det_kernel<4><<<grid4, 256, 0, st>>>(dz, lddz, x, ldx, gb, M, o, K, rpb4, part, part_gb);
-            else skinny_wgrad4_det_kernel<16><<<grid4, 256, 0, st>>>(dz, lddz, x, ldx, gb, M, o, K, rpb4, part, part_gb);
-            go1_count_launch(1);
-            if (int e = cuda_rc("go1_skinny_wgrad")) return e;
-            if (int e = go1_det_sum(part, grid4.y, (size_t)o * K, gW, o, K, ldg, 1, st)) return e;
-            return gb ? go1_det_sum(part_gb, grid4.y, o, gb, 1, o, o, 1, st) : 0;
-        }
-        if (o <= 2) skinny_wgrad4_kernel<2><<<grid4, 256, 0, st>>>(dz, lddz, x, ldx, gW, ldg, gb, M, o, K, rpb4);
-        else if (o <= 4) skinny_wgrad4_kernel<4><<<grid4, 256, 0, st>>>(dz, lddz, x, ldx, gW, ldg, gb, M, o, K, rpb4);
-        else skinny_wgrad4_kernel<16><<<grid4, 256, 0, st>>>(dz, lddz, x, ldx, gW, ldg, gb, M, o, K, rpb4);
-        go1_count_launch(1);
-        return cuda_rc("go1_skinny_wgrad");
+    const bool det = go1_det_on();     // deterministic mode: the row slabs' sums meet in gW / gb in slab order
+    const bool vec = (K & 3) == 0 && (ldx & 3) == 0 && (((uintptr_t)x) & 15) == 0;
+    int rpb = 64;
+    if (vec) {
+        rpb = (M * ((K + 127) / 128) + 131) / 132;       // about one block per SM (the per-block reduction and atomics dominate with more)
+        rpb = (rpb + 7) / 8 * 8; if (rpb < 8) rpb = 8;
     }
-    const int rpb = 64;
-    dim3 grid((K + 127) / 128, (M + rpb - 1) / rpb);
-    if (det) {
-        float* part = (float*)go1_det_workspace(st, sizeof(float) * (size_t)grid.y * o * K);
-        if (!part) return 1;
-        if (o <= 2) skinny_wgrad_det_kernel<2><<<grid, 128, 0, st>>>(dz, lddz, x, ldx, M, o, K, rpb, part);
-        else if (o <= 4) skinny_wgrad_det_kernel<4><<<grid, 128, 0, st>>>(dz, lddz, x, ldx, M, o, K, rpb, part);
-        else skinny_wgrad_det_kernel<16><<<grid, 128, 0, st>>>(dz, lddz, x, ldx, M, o, K, rpb, part);
-        go1_count_launch(1);
-        if (int e = cuda_rc("go1_skinny_wgrad")) return e;
-        return go1_det_sum(part, grid.y, (size_t)o * K, gW, o, K, ldg, 1, st);
-    }
-    if (o <= 2) skinny_wgrad_kernel<2><<<grid, 128, 0, st>>>(dz, lddz, x, ldx, gW, ldg, M, o, K, rpb);
-    else if (o <= 4) skinny_wgrad_kernel<4><<<grid, 128, 0, st>>>(dz, lddz, x, ldx, gW, ldg, M, o, K, rpb);
-    else skinny_wgrad_kernel<16><<<grid, 128, 0, st>>>(dz, lddz, x, ldx, gW, ldg, M, o, K, rpb);
+    const dim3 grid((K + 127) / 128, (M + rpb - 1) / rpb);
+    const size_t nw = (size_t)grid.y * o * K;
+    float* part = go1_det_out<float>(det, st, nw + (vec ? (size_t)grid.y * o : 0), nullptr);
+    if (det && !part) return 1;
+    float* const part_gb = det ? part + nw : nullptr;
+#define LAUNCH(O)                                                                                                                                      \
+    if (vec) (det ? skinny_wgrad4_kernel<O, true> : skinny_wgrad4_kernel<O, false>)<<<grid, 256, 0, st>>>(dz, lddz, x, ldx, gW, ldg, gb, M, o, K, rpb, part, part_gb); \
+    else (det ? skinny_wgrad_kernel<O, true> : skinny_wgrad_kernel<O, false>)<<<grid, 128, 0, st>>>(dz, lddz, x, ldx, gW, ldg, M, o, K, rpb, part)
+    if (o <= 2) { LAUNCH(2); } else if (o <= 4) { LAUNCH(4); } else { LAUNCH(16); }
+#undef LAUNCH
     go1_count_launch(1);
-    return cuda_rc("go1_skinny_wgrad");
+    if (int e = cuda_rc("go1_skinny_wgrad")) return e;
+    if (!det) return 0;
+    if (int e = go1_det_sum(part, grid.y, (size_t)o * K, gW, o, K, ldg, 1, st)) return e;
+    return gb ? go1_det_sum(part_gb, grid.y, o, gb, 1, o, o, 1, st) : 0;
 }
 
 extern "C" int go1_skinny_wgrad(const float* dz, int lddz, const float* x, int ldx, float* gW, int ldg, int M, int o, int K, int accumulate, void* stream) {
@@ -810,7 +678,7 @@ extern "C" int go1_copy_segments(const Go1CopySeg* segs, int n, void* stream) {
 
 // out[n] (+)= sum_m x[m][n]   (bias gradients).  DET (both variants): the slab's sums go to out[blockIdx.y][N] (plain stores, partials for go1_det_sum)
 template <bool DET>
-__device__ __forceinline__ void colsum_body(const float* __restrict__ x, int ldx, float* __restrict__ out, int M, int N, int rows_per_block) {
+__global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x, int ldx, float* __restrict__ out, int M, int N, int rows_per_block) {
     __shared__ float s[8][33];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const int n = blockIdx.x * 32 + lane;
@@ -827,15 +695,9 @@ __device__ __forceinline__ void colsum_body(const float* __restrict__ x, int ldx
         else atomicAdd(out + n, t);
     }
 }
-__global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x, int ldx, float* __restrict__ out, int M, int N, int rows_per_block) {
-    colsum_body<false>(x, ldx, out, M, N, rows_per_block);
-}
-__global__ void __launch_bounds__(256) colsum_det_kernel(const float* __restrict__ x, int ldx, float* __restrict__ part, int M, int N, int rows_per_block) {
-    colsum_body<true>(x, ldx, part, M, N, rows_per_block);
-}
 // wide variant: one float4 column group per lane (128 columns per warp row), 4 independent rows in flight per thread
 template <bool DET>
-__device__ __forceinline__ void colsum4_body(const float* __restrict__ x, int ldx, float* __restrict__ out, int M, int N, int rows_per_block) {
+__global__ void __launch_bounds__(256) colsum4_kernel(const float* __restrict__ x, int ldx, float* __restrict__ out, int M, int N, int rows_per_block) {
     __shared__ float4 s[8][32];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     const int n = blockIdx.x * 128 + lane * 4;
@@ -866,38 +728,21 @@ __device__ __forceinline__ void colsum4_body(const float* __restrict__ x, int ld
         else { atomicAdd(out + n, t.x); atomicAdd(out + n + 1, t.y); atomicAdd(out + n + 2, t.z); atomicAdd(out + n + 3, t.w); }
     }
 }
-__global__ void __launch_bounds__(256) colsum4_kernel(const float* __restrict__ x, int ldx, float* __restrict__ out, int M, int N, int rows_per_block) {
-    colsum4_body<false>(x, ldx, out, M, N, rows_per_block);
-}
-__global__ void __launch_bounds__(256) colsum4_det_kernel(const float* __restrict__ x, int ldx, float* __restrict__ part, int M, int N, int rows_per_block) {
-    colsum4_body<true>(x, ldx, part, M, N, rows_per_block);
-}
 extern "C" int go1_colsum(const float* x, int ldx, float* out, int M, int N, int accumulate, void* stream) {
     if (!x || !out || M <= 0 || N <= 0) return go1_set_error("go1_colsum: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
     const bool vec = N >= 64 && (N & 3) == 0 && (ldx & 3) == 0 && (((uintptr_t)x) & 15) == 0;
-    if (go1_det_on()) {     // deterministic mode: the row slabs' sums meet in out in slab order
-        const int rpb = vec ? 128 : 512;
-        const dim3 grid(vec ? (N + 127) / 128 : (N + 31) / 32, (M + rpb - 1) / rpb);
-        float* part = (float*)go1_det_workspace(st, sizeof(float) * (size_t)grid.y * N);
-        if (!part) return 1;
-        if (vec) colsum4_det_kernel<<<grid, 256, 0, st>>>(x, ldx, part, M, N, rpb);
-        else colsum_det_kernel<<<grid, 256, 0, st>>>(x, ldx, part, M, N, rpb);
-        go1_count_launch(1);
-        if (int e = cuda_rc("go1_colsum")) return e;
-        return go1_det_sum(part, grid.y, N, out, 1, N, N, accumulate, st);
-    }
-    if (!accumulate) cudaMemsetAsync(out, 0, sizeof(float) * N, st);
-    if (vec) {
-        const int rpb4 = 128;
-        dim3 grid4((N + 127) / 128, (M + rpb4 - 1) / rpb4);
-        colsum4_kernel<<<grid4, 256, 0, st>>>(x, ldx, out, M, N, rpb4); go1_count_launch(1);
-        return cuda_rc("go1_colsum");
-    }
-    const int rpb = 512;
-    dim3 grid((N + 31) / 32, (M + rpb - 1) / rpb);
-    colsum_kernel<<<grid, 256, 0, st>>>(x, ldx, out, M, N, rpb); go1_count_launch(1);
-    return cuda_rc("go1_colsum");
+    const bool det = go1_det_on();     // deterministic mode: the row slabs' sums meet in out in slab order
+    const int rpb = vec ? 128 : 512;
+    const dim3 grid(vec ? (N + 127) / 128 : (N + 31) / 32, (M + rpb - 1) / rpb);
+    float* dst = go1_det_out(det, st, (size_t)grid.y * N, out);
+    if (det && !dst) return 1;
+    if (!accumulate && !det) cudaMemsetAsync(out, 0, sizeof(float) * N, st);
+    if (vec) (det ? colsum4_kernel<true> : colsum4_kernel<false>)<<<grid, 256, 0, st>>>(x, ldx, dst, M, N, rpb);
+    else (det ? colsum_kernel<true> : colsum_kernel<false>)<<<grid, 256, 0, st>>>(x, ldx, dst, M, N, rpb);
+    go1_count_launch(1);
+    if (int e = cuda_rc("go1_colsum")) return e;
+    return det ? go1_det_sum(dst, grid.y, N, out, 1, N, N, accumulate, st) : 0;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -941,7 +786,7 @@ extern "C" int go1_ppo_sample_actions(const float* mean, int ldm, const float* s
 #define PPO_MAX_ACT 16
 // DET: the block's PPO_MAX_ACT dstd sums and three scalars go to part[blockIdx.x][PPO_MAX_ACT + 3] (partials for go1_det_sum)
 template <bool DET>
-__device__ __forceinline__ void ppo_loss_body(const float* __restrict__ mean, int ldm, const float* __restrict__ std, const float* __restrict__ value,
+__global__ void __launch_bounds__(256) ppo_loss_kernel(const float* __restrict__ mean, int ldm, const float* __restrict__ std, const float* __restrict__ value,
         const float* __restrict__ actions, const float* __restrict__ old_logp, const float* __restrict__ old_mean, const float* __restrict__ old_std,
         const float* __restrict__ adv, const float* __restrict__ returns, const float* __restrict__ old_values,
         float* __restrict__ dmean, int lddm, float* __restrict__ dvalue, float* __restrict__ dstd, float* __restrict__ scalars,
@@ -1010,22 +855,6 @@ __device__ __forceinline__ void ppo_loss_body(const float* __restrict__ mean, in
         else atomicAdd(scalars + (j == PPO_MAX_ACT ? 0 : (j == PPO_MAX_ACT + 1 ? 1 : 3)), t * inv_count);
     }
 }
-__global__ void __launch_bounds__(256) ppo_loss_kernel(const float* __restrict__ mean, int ldm, const float* __restrict__ std, const float* __restrict__ value,
-        const float* __restrict__ actions, const float* __restrict__ old_logp, const float* __restrict__ old_mean, const float* __restrict__ old_std,
-        const float* __restrict__ adv, const float* __restrict__ returns, const float* __restrict__ old_values,
-        float* __restrict__ dmean, int lddm, float* __restrict__ dvalue, float* __restrict__ dstd, float* __restrict__ scalars,
-        int n, int na, float clip, float vcoef, float ecoef, int clipped_v, float inv_count) {
-    ppo_loss_body<false>(mean, ldm, std, value, actions, old_logp, old_mean, old_std, adv, returns, old_values, dmean, lddm, dvalue, dstd, scalars,
-                         n, na, clip, vcoef, ecoef, clipped_v, inv_count, nullptr);
-}
-__global__ void __launch_bounds__(256) ppo_loss_det_kernel(const float* __restrict__ mean, int ldm, const float* __restrict__ std, const float* __restrict__ value,
-        const float* __restrict__ actions, const float* __restrict__ old_logp, const float* __restrict__ old_mean, const float* __restrict__ old_std,
-        const float* __restrict__ adv, const float* __restrict__ returns, const float* __restrict__ old_values,
-        float* __restrict__ dmean, int lddm, float* __restrict__ dvalue, int n, int na, float clip, float vcoef, float ecoef, int clipped_v, float inv_count,
-        float* __restrict__ part) {
-    ppo_loss_body<true>(mean, ldm, std, value, actions, old_logp, old_mean, old_std, adv, returns, old_values, dmean, lddm, dvalue, nullptr, nullptr,
-                        n, na, clip, vcoef, ecoef, clipped_v, inv_count, part);
-}
 __global__ void ppo_entropy_kernel(const float* __restrict__ std, float* __restrict__ dstd, float* __restrict__ scalars, int na, float ecoef, float local_frac) {
     // entropy of Normal(mean, std) summed over actions is the same for every sample: sum_j 0.5 + 0.5 log(2 pi) + log std_j
     const int j = threadIdx.x;
@@ -1045,29 +874,28 @@ extern "C" int go1_ppo_loss(const float* mean, int ldm, const float* std, const 
     cudaStream_t st = (cudaStream_t)stream;
     cudaMemsetAsync(dstd, 0, sizeof(float) * num_actions, st);
     cudaMemsetAsync(scalars, 0, sizeof(float) * 8, st);
-    if (go1_det_on()) {     // deterministic mode: the blocks' sums meet in dstd / scalars in block order, then the entropy kernel adds its terms
-        const int nb = (n + 255) / 256;
-        constexpr int W = PPO_MAX_ACT + 3;
-        float* part = (float*)go1_det_workspace(st, sizeof(float) * (size_t)nb * W);
-        if (!part) return 1;
-        ppo_loss_det_kernel<<<nb, 256, 0, st>>>(mean, ldm, std, value, actions, old_logp, old_mean, old_std, advantages, returns, old_values,
-                                                dmean, lddm, dvalue, n, num_actions, clip_param, value_loss_coef, entropy_coef,
-                                                use_clipped_value_loss, inv_count, part); go1_count_launch(1);
+    const bool det = go1_det_on();     // deterministic mode: the blocks' sums meet in dstd / scalars in block order, then the entropy kernel adds its terms
+    const int nb = (n + 255) / 256;
+    constexpr int W = PPO_MAX_ACT + 3;
+    float* part = go1_det_out<float>(det, st, (size_t)nb * W, nullptr);
+    if (det && !part) return 1;
+    (det ? ppo_loss_kernel<true> : ppo_loss_kernel<false>)<<<nb, 256, 0, st>>>(mean, ldm, std, value, actions, old_logp, old_mean, old_std, advantages, returns,
+                                                                               old_values, dmean, lddm, dvalue, dstd, scalars, n, num_actions, clip_param,
+                                                                               value_loss_coef, entropy_coef, use_clipped_value_loss, inv_count, part);
+    go1_count_launch(1);
+    if (det) {
         if (int e = cuda_rc("go1_ppo_loss")) return e;
         if (int e = go1_det_sum(part, nb, W, dstd, 1, num_actions, num_actions, 0, st)) return e;
         if (int e = go1_det_sum(part + PPO_MAX_ACT, nb, W, scalars, 1, 2, 2, 0, st)) return e;         // surrogate, value loss
         if (int e = go1_det_sum(part + PPO_MAX_ACT + 2, nb, W, scalars + 3, 1, 1, 1, 0, st)) return e;  // kl
-        ppo_entropy_kernel<<<1, 32, 0, st>>>(std, dstd, scalars, num_actions, entropy_coef, (float)n * inv_count); go1_count_launch(1);
-        return cuda_rc("go1_ppo_loss");
     }
-    ppo_loss_kernel<<<(n + 255) / 256, 256, 0, st>>>(mean, ldm, std, value, actions, old_logp, old_mean, old_std, advantages, returns, old_values,
-                                                    dmean, lddm, dvalue, dstd, scalars, n, num_actions, clip_param, value_loss_coef, entropy_coef,
-                                                    use_clipped_value_loss, inv_count); go1_count_launch(1);
     ppo_entropy_kernel<<<1, 32, 0, st>>>(std, dstd, scalars, num_actions, entropy_coef, (float)n * inv_count); go1_count_launch(1);
     return cuda_rc("go1_ppo_loss");
 }
 
-// MSE (ppo.py:168-186): train split [0, num_train) gets loss + gradient, the rest only the test loss
+// MSE (ppo.py:168-186): train split [0, num_train) gets loss + gradient, the rest only the test loss.  DET: scalars is the workspace, and
+// the block's two losses go to scalars[2 blockIdx.x ..]
+template <bool DET>
 __global__ void __launch_bounds__(256) mse_kernel(const float* __restrict__ pred, int ldp, const float* __restrict__ tgt, int ldt, float* __restrict__ dpred, int lddp,
                                                   float* __restrict__ scalars, int n, int num_train, int dim) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1090,51 +918,22 @@ __global__ void __launch_bounds__(256) mse_kernel(const float* __restrict__ pred
         float t = 0.f;
         for (int k = 0; k < 8; k++) t += s[threadIdx.x][k];
         const float cnt = threadIdx.x == 0 ? (float)num_train * dim : (float)(n - num_train) * dim;
-        if (cnt > 0.f) atomicAdd(scalars + threadIdx.x, t / cnt);
-    }
-}
-// mse_kernel of the deterministic mode: the block's two losses go to part[2 blockIdx.x ..], which go1_det_sum adds in block order (a copy, as
-// gae_det_kernel)
-__global__ void __launch_bounds__(256) mse_det_kernel(const float* __restrict__ pred, int ldp, const float* __restrict__ tgt, int ldt, float* __restrict__ dpred, int lddp,
-                                                      float* __restrict__ part, int n, int num_train, int dim) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    float ltr = 0.f, lte = 0.f;
-    if (i < n) {
-        const bool train = i < num_train;
-        const float inv_tr = 1.0f / ((float)num_train * dim);
-        for (int j = 0; j < dim; j++) {
-            const float d = pred[(size_t)i * ldp + j] - tgt[(size_t)i * ldt + j];
-            if (train) { ltr += d * d; dpred[(size_t)i * lddp + j] = 2.0f * d * inv_tr; }
-            else { lte += d * d; dpred[(size_t)i * lddp + j] = 0.f; }
-        }
-    }
-    __shared__ float s[2][8];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    for (int d = 16; d > 0; d >>= 1) { ltr += __shfl_xor_sync(0xffffffffu, ltr, d); lte += __shfl_xor_sync(0xffffffffu, lte, d); }
-    if (lane == 0) { s[0][w] = ltr; s[1][w] = lte; }
-    __syncthreads();
-    if (threadIdx.x < 2) {
-        float t = 0.f;
-        for (int k = 0; k < 8; k++) t += s[threadIdx.x][k];
-        const float cnt = threadIdx.x == 0 ? (float)num_train * dim : (float)(n - num_train) * dim;
-        part[2 * blockIdx.x + threadIdx.x] = cnt > 0.f ? t / cnt : 0.f;
+        if constexpr (DET) scalars[2 * blockIdx.x + threadIdx.x] = cnt > 0.f ? t / cnt : 0.f;
+        else if (cnt > 0.f) atomicAdd(scalars + threadIdx.x, t / cnt);
     }
 }
 extern "C" int go1_ppo_mse(const float* pred, int ldp, const float* target, int ldt, float* dpred, int lddp, float* scalars,
                            int n, int num_train, int dim, void* stream) {
     if (!pred || !target || !dpred || !scalars || n <= 0 || dim <= 0 || num_train < 0 || num_train > n) return go1_set_error("go1_ppo_mse: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
-    if (go1_det_on()) {     // deterministic mode: the blocks' losses meet in scalars in block order
-        const int nb = (n + 255) / 256;
-        float* part = (float*)go1_det_workspace(st, sizeof(float) * 2 * (size_t)nb);
-        if (!part) return 1;
-        mse_det_kernel<<<nb, 256, 0, st>>>(pred, ldp, target, ldt, dpred, lddp, part, n, num_train, dim); go1_count_launch(1);
-        if (int e = cuda_rc("go1_ppo_mse")) return e;
-        return go1_det_sum(part, nb, 2, scalars, 1, 2, 2, 0, st);
-    }
-    cudaMemsetAsync(scalars, 0, sizeof(float) * 2, st);
-    mse_kernel<<<(n + 255) / 256, 256, 0, st>>>(pred, ldp, target, ldt, dpred, lddp, scalars, n, num_train, dim); go1_count_launch(1);
-    return cuda_rc("go1_ppo_mse");
+    const bool det = go1_det_on();     // deterministic mode: the blocks' losses meet in scalars in block order
+    const int nb = (n + 255) / 256;
+    float* out = go1_det_out(det, st, 2 * (size_t)nb, scalars);
+    if (det && !out) return 1;
+    if (!det) cudaMemsetAsync(scalars, 0, sizeof(float) * 2, st);
+    (det ? mse_kernel<true> : mse_kernel<false>)<<<nb, 256, 0, st>>>(pred, ldp, target, ldt, dpred, lddp, out, n, num_train, dim); go1_count_launch(1);
+    if (int e = cuda_rc("go1_ppo_mse")) return e;
+    return det ? go1_det_sum(out, nb, 2, scalars, 1, 2, 2, 0, st) : 0;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1142,7 +941,7 @@ extern "C" int go1_ppo_mse(const float* pred, int ldp, const float* target, int 
 // ---------------------------------------------------------------------------------------------
 // DET: the block's sum goes to out[blockIdx.x] (partials for go1_det_sum64)
 template <bool DET>
-__device__ __forceinline__ void sqnorm_body(const float* __restrict__ g, long long count, double* __restrict__ out) {
+__global__ void __launch_bounds__(256) sqnorm_kernel(const float* __restrict__ g, long long count, double* __restrict__ out) {
     double acc = 0.0;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x) { const float v = g[i]; acc += (double)v * (double)v; }
     __shared__ double s[8];
@@ -1156,21 +955,16 @@ __device__ __forceinline__ void sqnorm_body(const float* __restrict__ g, long lo
         else atomicAdd(out, t);
     }
 }
-__global__ void __launch_bounds__(256) sqnorm_kernel(const float* __restrict__ g, long long count, double* __restrict__ out) { sqnorm_body<false>(g, count, out); }
-__global__ void __launch_bounds__(256) sqnorm_det_kernel(const float* __restrict__ g, long long count, double* __restrict__ part) { sqnorm_body<true>(g, count, part); }
 extern "C" int go1_ppo_grad_sqnorm(const float* grad, int64_t count, double* grad_sq, void* stream) {
     if (!grad || !grad_sq || count <= 0) return go1_set_error("go1_ppo_grad_sqnorm: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
-    if (go1_det_on()) {     // deterministic mode: the 296 blocks' sums meet in grad_sq in block order
-        double* part = (double*)go1_det_workspace(st, sizeof(double) * 296);
-        if (!part) return 1;
-        sqnorm_det_kernel<<<296, 256, 0, st>>>(grad, count, part); go1_count_launch(1);
-        if (int e = cuda_rc("go1_ppo_grad_sqnorm")) return e;
-        return go1_det_sum64(part, 296, 1, grad_sq, 1, 0, st);
-    }
-    cudaMemsetAsync(grad_sq, 0, sizeof(double), st);
-    sqnorm_kernel<<<296, 256, 0, st>>>(grad, count, grad_sq); go1_count_launch(1);
-    return cuda_rc("go1_ppo_grad_sqnorm");
+    const bool det = go1_det_on();     // deterministic mode: the 296 blocks' sums meet in grad_sq in block order
+    double* out = go1_det_out(det, st, 296, grad_sq);
+    if (det && !out) return 1;
+    if (!det) cudaMemsetAsync(grad_sq, 0, sizeof(double), st);
+    (det ? sqnorm_kernel<true> : sqnorm_kernel<false>)<<<296, 256, 0, st>>>(grad, count, out); go1_count_launch(1);
+    if (int e = cuda_rc("go1_ppo_grad_sqnorm")) return e;
+    return det ? go1_det_sum64(out, 296, 1, grad_sq, 1, 0, st) : 0;
 }
 __global__ void __launch_bounds__(256) adam_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, long long count,
                                                    const double* __restrict__ grad_sq, float max_norm, float lr, const float* __restrict__ lr_dev, float b1, float b2, float eps, float bc1, float bc2_sqrt) {
@@ -1285,8 +1079,8 @@ __global__ void __launch_bounds__(256) extra_dinput_kernel(const float* __restri
 }
 // DET (this kernel and extra_wgrad_wide): the slab's sums go to part[blockIdx.y][o][E] (plain stores; go1_det_sum adds the slabs into gWe)
 template <bool DET>
-__device__ __forceinline__ void extra_wgrad_body(const float* __restrict__ dz, int lddz, const float* __restrict__ extra, int ldex,
-                                                 float* __restrict__ gWe, int ldgw, int M, int o, int E, int rows_per_block, float* __restrict__ part) {
+__global__ void __launch_bounds__(256) extra_wgrad_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ extra, int ldex,
+                                                          float* __restrict__ gWe, int ldgw, int M, int o, int E, int rows_per_block, float* __restrict__ part) {
     const int r0 = blockIdx.y * rows_per_block, r1 = min(M, r0 + rows_per_block);
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
     if (j >= o) return;
@@ -1304,14 +1098,6 @@ __device__ __forceinline__ void extra_wgrad_body(const float* __restrict__ dz, i
             else atomicAdd(gWe + (size_t)j * ldgw + t, acc[t]);
         }
     }
-}
-__global__ void __launch_bounds__(256) extra_wgrad_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ extra, int ldex,
-                                                          float* __restrict__ gWe, int ldgw, int M, int o, int E, int rows_per_block) {
-    extra_wgrad_body<false>(dz, lddz, extra, ldex, gWe, ldgw, M, o, E, rows_per_block, nullptr);
-}
-__global__ void __launch_bounds__(256) extra_wgrad_det_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ extra, int ldex,
-                                                              int M, int o, int E, int rows_per_block, float* __restrict__ part) {
-    extra_wgrad_body<true>(dz, lddz, extra, ldex, nullptr, 0, M, o, E, rows_per_block, part);
 }
 __global__ void zero_small_kernel(float* p, int ld, int rows, int cols) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1356,8 +1142,8 @@ __global__ void __launch_bounds__(128) extra_dinput_wide_kernel(const float* __r
 // weight gradient: one thread per column j with its EB sums in registers over the CTA's row slab; the slab's extra rows are staged in
 // shared memory 32 at a time (zero beyond E) and read as broadcasts; E atomics per thread at the end.
 template <int EB, bool DET>
-__device__ __forceinline__ void extra_wgrad_wide_body(const float* __restrict__ dz, int lddz, const float* __restrict__ extra, int ldex,
-                                                      float* __restrict__ gWe, int ldgw, int M, int o, int E, int rows_per_block, float* __restrict__ part) {
+__global__ void __launch_bounds__(128) extra_wgrad_wide_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ extra, int ldex,
+                                                               float* __restrict__ gWe, int ldgw, int M, int o, int E, int rows_per_block, float* __restrict__ part) {
     __shared__ __align__(16) float xs[32][EB];
     const int r0 = blockIdx.y * rows_per_block, r1 = min(M, r0 + rows_per_block);
     const int j = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1392,16 +1178,6 @@ __device__ __forceinline__ void extra_wgrad_wide_body(const float* __restrict__ 
         }
     }
 }
-template <int EB>
-__global__ void __launch_bounds__(128) extra_wgrad_wide_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ extra, int ldex,
-                                                               float* __restrict__ gWe, int ldgw, int M, int o, int E, int rows_per_block) {
-    extra_wgrad_wide_body<EB, false>(dz, lddz, extra, ldex, gWe, ldgw, M, o, E, rows_per_block, nullptr);
-}
-template <int EB>
-__global__ void __launch_bounds__(128) extra_wgrad_wide_det_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ extra, int ldex,
-                                                                   int M, int o, int E, int rows_per_block, float* __restrict__ part) {
-    extra_wgrad_wide_body<EB, true>(dz, lddz, extra, ldex, nullptr, 0, M, o, E, rows_per_block, part);
-}
 #define XWIDE_EB_SWITCH(E, EBV, ...)                                                   \
     if ((E) <= 8) { constexpr int EBV = 8; __VA_ARGS__ }                               \
     else if ((E) <= 16) { constexpr int EBV = 16; __VA_ARGS__ }                        \
@@ -1417,47 +1193,36 @@ extern "C" int go1_mlp_extra_backward(const float* dz, int lddz, int dz_transpos
     if (g_w_extra && dz_transposed) return go1_set_error("go1_mlp_extra_backward: the weight gradient takes dz as [M][o] (dz_transposed 0)");
     if (lddz < (dz_transposed ? M : o)) return go1_set_error("go1_mlp_extra_backward: lddz must be >= o ([M][o] dz) or >= M ([o][M] dz)");
     cudaStream_t st = (cudaStream_t)stream;
-    const bool det = go1_det_on();
-    if (E <= 4 && !dz_transposed) {
-        if (dextra) { extra_dinput_kernel<<<(M * 32 + 255) / 256, 256, 0, st>>>(dz, lddz, w_extra, ldw, dextra, ldde, M, o, E); go1_count_launch(1); }
-        if (g_w_extra) {
-            if (!accumulate) { zero_small_kernel<<<(o * E + 255) / 256, 256, 0, st>>>(g_w_extra, ldgw, o, E); go1_count_launch(1); }
-            const int rpb = 64;
-            dim3 grid((o + 255) / 256, (M + rpb - 1) / rpb);
-            if (det) {      // deterministic mode: the row slabs' sums meet in g_w_extra in slab order
-                float* part = (float*)go1_det_workspace(st, sizeof(float) * (size_t)grid.y * o * E);
-                if (!part) return 1;
-                extra_wgrad_det_kernel<<<grid, 256, 0, st>>>(dz, lddz, extra, ldex, M, o, E, rpb, part); go1_count_launch(1);
-                if (int e = cuda_rc("go1_mlp_extra_backward")) return e;
-                if (int e = go1_det_sum(part, grid.y, (size_t)o * E, g_w_extra, o, E, ldgw, 1, st)) return e;
-            } else {
-                extra_wgrad_kernel<<<grid, 256, 0, st>>>(dz, lddz, extra, ldex, g_w_extra, ldgw, M, o, E, rpb); go1_count_launch(1);
-            }
-        }
-        return cuda_rc("go1_mlp_extra_backward");
-    }
+    const bool narrow = E <= 4 && !dz_transposed;      // the E <= 4 kernels, else the wide ones
     if (dextra) {
-        const unsigned grid = (unsigned)((M + 127) / 128);
-        if (dz_transposed) { XWIDE_EB_SWITCH(E, EB, extra_dinput_wide_kernel<EB, true><<<grid, 128, 0, st>>>(dz, lddz, w_extra, ldw, dextra, ldde, M, o, E);) }
-        else { XWIDE_EB_SWITCH(E, EB, extra_dinput_wide_kernel<EB, false><<<grid, 128, 0, st>>>(dz, lddz, w_extra, ldw, dextra, ldde, M, o, E);) }
+        if (narrow) extra_dinput_kernel<<<(M * 32 + 255) / 256, 256, 0, st>>>(dz, lddz, w_extra, ldw, dextra, ldde, M, o, E);
+        else {
+            const unsigned grid = (unsigned)((M + 127) / 128);
+            if (dz_transposed) { XWIDE_EB_SWITCH(E, EB, extra_dinput_wide_kernel<EB, true><<<grid, 128, 0, st>>>(dz, lddz, w_extra, ldw, dextra, ldde, M, o, E);) }
+            else { XWIDE_EB_SWITCH(E, EB, extra_dinput_wide_kernel<EB, false><<<grid, 128, 0, st>>>(dz, lddz, w_extra, ldw, dextra, ldde, M, o, E);) }
+        }
         go1_count_launch(1);
     }
     if (g_w_extra) {
         if (!accumulate) { zero_small_kernel<<<(o * E + 255) / 256, 256, 0, st>>>(g_w_extra, ldgw, o, E); go1_count_launch(1); }
-        const int gx = (o + 127) / 128;
-        const int gy = min((M + 31) / 32, max(1, (132 * 4 + gx - 1) / gx));     // ~4 CTAs per SM; fewer slabs, fewer atomics
-        const int rpb = ((M + gy - 1) / gy + 31) / 32 * 32;
-        const dim3 grid(gx, (M + rpb - 1) / rpb);
-        if (det) {      // deterministic mode: the row slabs' sums meet in g_w_extra in slab order
-            float* part = (float*)go1_det_workspace(st, sizeof(float) * (size_t)grid.y * o * E);
-            if (!part) return 1;
-            XWIDE_EB_SWITCH(E, EB, extra_wgrad_wide_det_kernel<EB><<<grid, 128, 0, st>>>(dz, lddz, extra, ldex, M, o, E, rpb, part);)
-            go1_count_launch(1);
-            if (int e = cuda_rc("go1_mlp_extra_backward")) return e;
-            return go1_det_sum(part, grid.y, (size_t)o * E, g_w_extra, o, E, ldgw, 1, st);
+        int rpb = 64;
+        dim3 grid((o + 255) / 256, (M + rpb - 1) / rpb);
+        if (!narrow) {
+            const int gx = (o + 127) / 128;
+            const int gy = min((M + 31) / 32, max(1, (132 * 4 + gx - 1) / gx));     // ~4 CTAs per SM; fewer slabs, fewer atomics
+            rpb = ((M + gy - 1) / gy + 31) / 32 * 32;
+            grid = dim3(gx, (M + rpb - 1) / rpb);
         }
-        XWIDE_EB_SWITCH(E, EB, extra_wgrad_wide_kernel<EB><<<grid, 128, 0, st>>>(dz, lddz, extra, ldex, g_w_extra, ldgw, M, o, E, rpb);)
+        const bool det = go1_det_on();     // deterministic mode: the row slabs' sums meet in g_w_extra in slab order
+        float* part = go1_det_out<float>(det, st, (size_t)grid.y * o * E, nullptr);
+        if (det && !part) return 1;
+        if (narrow) (det ? extra_wgrad_kernel<true> : extra_wgrad_kernel<false>)<<<grid, 256, 0, st>>>(dz, lddz, extra, ldex, g_w_extra, ldgw, M, o, E, rpb, part);
+        else { XWIDE_EB_SWITCH(E, EB, (det ? extra_wgrad_wide_kernel<EB, true> : extra_wgrad_wide_kernel<EB, false>)<<<grid, 128, 0, st>>>(dz, lddz, extra, ldex, g_w_extra, ldgw, M, o, E, rpb, part);) }
         go1_count_launch(1);
+        if (det) {
+            if (int e = cuda_rc("go1_mlp_extra_backward")) return e;
+            if (int e = go1_det_sum(part, grid.y, (size_t)o * E, g_w_extra, o, E, ldgw, 1, st)) return e;
+        }
     }
     return cuda_rc("go1_mlp_extra_backward");
 }
@@ -1476,8 +1241,9 @@ __global__ void skinny_dgrad_kernel(const float* __restrict__ dz, int lddz, cons
 // its O x 4 weights in registers; the row's o output gradients are fetched by the first o lanes and shuffle-broadcast.  Optionally the
 // column sums of the values written (= the bias gradient of the layer below) are reduced here as well: per-lane partial sums, one
 // shared-memory reduction per block, one set of atomics per block.  OUT16: dprev is a BF16 matrix (uint16_t, lddp elements) that gets the
-// values rounded to nearest even; the column sums see the fp32 values (go1_skinny_dgrad_act_bf16).
-template <int O, int KIND, bool OUT16 = false>
+// values rounded to nearest even; the column sums see the fp32 values (go1_skinny_dgrad_act_bf16).  DET: colsum is the workspace, and the
+// block's column sums go to colsum[blockIdx.y][n] (plain stores; go1_det_sum adds the slabs)
+template <int O, int KIND, bool OUT16, bool DET>
 __global__ void __launch_bounds__(256) skinny_dgrad4_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ W, int ldw, const float* __restrict__ y, int ldy,
                                                             float* __restrict__ dprev, int lddp, float* __restrict__ colsum, int M, int o, int n, int rows_per_block) {
     __shared__ float4 s_sum[8][32];
@@ -1513,63 +1279,15 @@ __global__ void __launch_bounds__(256) skinny_dgrad4_kernel(const float* __restr
         } else if (col_ok) *reinterpret_cast<float4*>(dprev + (size_t)m * lddp + c) = make_float4(v0, v1, v2, v3);
         cs.x += v0; cs.y += v1; cs.z += v2; cs.w += v3;
     }
-    if (colsum) {
+    if (DET || colsum) {
         s_sum[w][lane] = cs;
         __syncthreads();
         if (w == 0 && col_ok) {
             float4 t = s_sum[0][lane];
 #pragma unroll
             for (int k = 1; k < 8; k++) { t.x += s_sum[k][lane].x; t.y += s_sum[k][lane].y; t.z += s_sum[k][lane].z; t.w += s_sum[k][lane].w; }
-            atomicAdd(colsum + c, t.x); atomicAdd(colsum + c + 1, t.y); atomicAdd(colsum + c + 2, t.z); atomicAdd(colsum + c + 3, t.w);
-        }
-    }
-}
-// skinny_dgrad4_kernel with column sums, of the deterministic mode (a copy, as gae_det_kernel): the block's column sums go to
-// part[blockIdx.y][n], which go1_det_sum adds in slab order
-template <int O, int KIND, bool OUT16>
-__global__ void __launch_bounds__(256) skinny_dgrad4_det_kernel(const float* __restrict__ dz, int lddz, const float* __restrict__ W, int ldw, const float* __restrict__ y, int ldy,
-                                                                float* __restrict__ dprev, int lddp, float* __restrict__ part, int M, int o, int n, int rows_per_block) {
-    __shared__ float4 s_sum[8][32];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    const int c = blockIdx.x * 128 + lane * 4;
-    const bool col_ok = c < n;
-    float wr[O][4];
-#pragma unroll
-    for (int t = 0; t < O; t++) {
-        const float4 ww = (t < o && col_ok) ? __ldg(reinterpret_cast<const float4*>(W + (size_t)t * ldw + c)) : make_float4(0.f, 0.f, 0.f, 0.f);
-        wr[t][0] = ww.x; wr[t][1] = ww.y; wr[t][2] = ww.z; wr[t][3] = ww.w;
-    }
-    const int r0 = blockIdx.y * rows_per_block, r1 = min(M, r0 + rows_per_block);
-    float4 cs = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 2
-    for (int m = r0 + w; m < r1; m += 8) {
-        const float dl = lane < o ? __ldg(dz + (size_t)m * lddz + lane) : 0.f;
-        float4 yy = make_float4(1.f, 1.f, 1.f, 1.f);
-        if (y && col_ok) yy = __ldg(reinterpret_cast<const float4*>(y + (size_t)m * ldy + c));
-        float v0 = 0.f, v1 = 0.f, v2 = 0.f, v3 = 0.f;
-#pragma unroll
-        for (int t = 0; t < O; t++) {
-            const float d = __shfl_sync(0xffffffffu, dl, t);
-            v0 = fmaf(d, wr[t][0], v0); v1 = fmaf(d, wr[t][1], v1); v2 = fmaf(d, wr[t][2], v2); v3 = fmaf(d, wr[t][3], v3);
-        }
-        if (y) { v0 *= act_deriv<KIND>(yy.x); v1 *= act_deriv<KIND>(yy.y); v2 *= act_deriv<KIND>(yy.z); v3 *= act_deriv<KIND>(yy.w); }
-        if (OUT16) {
-            if (col_ok) {
-                uint16_t* d16 = reinterpret_cast<uint16_t*>(dprev) + (size_t)m * lddp + c;
-                *reinterpret_cast<uint2*>(d16) = make_uint2((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v0)) | ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v1)) << 16),
-                                                            (uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v2)) | ((uint32_t)__bfloat16_as_ushort(__float2bfloat16_rn(v3)) << 16));
-            }
-        } else if (col_ok) *reinterpret_cast<float4*>(dprev + (size_t)m * lddp + c) = make_float4(v0, v1, v2, v3);
-        cs.x += v0; cs.y += v1; cs.z += v2; cs.w += v3;
-    }
-    {
-        s_sum[w][lane] = cs;
-        __syncthreads();
-        if (w == 0 && col_ok) {
-            float4 t = s_sum[0][lane];
-#pragma unroll
-            for (int k = 1; k < 8; k++) { t.x += s_sum[k][lane].x; t.y += s_sum[k][lane].y; t.z += s_sum[k][lane].z; t.w += s_sum[k][lane].w; }
-            *reinterpret_cast<float4*>(part + (size_t)blockIdx.y * n + c) = t;
+            if constexpr (DET) *reinterpret_cast<float4*>(colsum + (size_t)blockIdx.y * n + c) = t;
+            else { atomicAdd(colsum + c, t.x); atomicAdd(colsum + c + 1, t.y); atomicAdd(colsum + c + 2, t.z); atomicAdd(colsum + c + 3, t.w); }
         }
     }
 }
@@ -1582,21 +1300,15 @@ static int launch_skinny_dgrad4(const float* dz, int lddz, const float* W, int l
     int rpb = (M * cb + 2 * 132 - 1) / (2 * 132);           // about two blocks per SM
     rpb = (rpb + 7) / 8 * 8; if (rpb < 8) rpb = 8;
     dim3 grid(cb, (M + rpb - 1) / rpb);
-    if (colsum && go1_det_on()) {
-        float* part = (float*)go1_det_workspace(st, sizeof(float) * (size_t)grid.y * n);
-        if (!part) return 1;
-#define LAUNCH(O, KD) skinny_dgrad4_det_kernel<O, KD, OUT16><<<grid, 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, part, M, o, n, rpb)
-        GO1_ACT_SWITCH(kind, KD, if (o <= 2) LAUNCH(2, KD); else if (o <= 4) LAUNCH(4, KD); else LAUNCH(16, KD);)
-#undef LAUNCH
-        go1_count_launch(1);
-        if (int e = cuda_rc(what)) return e;
-        return go1_det_sum(part, grid.y, n, colsum, 1, n, n, 1, st);
-    }
-#define LAUNCH(O, KD) skinny_dgrad4_kernel<O, KD, OUT16><<<grid, 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, colsum, M, o, n, rpb)
+    const bool det = colsum && go1_det_on();
+    float* cs = go1_det_out(det, st, (size_t)grid.y * n, colsum);
+    if (det && !cs) return 1;
+#define LAUNCH(O, KD) (det ? skinny_dgrad4_kernel<O, KD, OUT16, true> : skinny_dgrad4_kernel<O, KD, OUT16, false>)<<<grid, 256, 0, st>>>(dz, lddz, W, ldw, y_prev, ldy, dprev, lddp, cs, M, o, n, rpb)
     GO1_ACT_SWITCH(kind, KD, if (o <= 2) LAUNCH(2, KD); else if (o <= 4) LAUNCH(4, KD); else LAUNCH(16, KD);)
 #undef LAUNCH
     go1_count_launch(1);
-    return cuda_rc(what);
+    if (int e = cuda_rc(what)) return e;
+    return det ? go1_det_sum(cs, grid.y, n, colsum, 1, n, n, 1, st) : 0;
 }
 extern "C" int go1_skinny_dgrad_act(const float* dz, int lddz, const float* W, int ldw, const float* y_prev, int ldy, float* dprev, int lddp,
                                     float* colsum, int M, int o, int n, int kind, void* stream) {
