@@ -235,6 +235,22 @@ int go1_sizeof_self_collision(void);
  * was chosen when it was captured, so a later change fails (and leaves the setting as it was). */
 int go1_sim_set_self_collision(Go1Sim* sim, const Go1SelfCollision* sc);
 
+/* Asset options of the simulated Go1 (Cfg.asset, DESIGN.md §3).  Bodies are numbered in Isaac Gym order:
+ * 0 base, then hip, thigh, calf, foot of FL (1-4), FR (5-8), RL (9-12), RR (13-16). */
+#define GO1_NUM_BODIES 17
+typedef struct Go1AssetOptions {
+    float penalty_weight[GO1_NUM_BODIES]; /* collision term: sum_b penalty_weight[b] * (|F_b| > 0.1); Go1: 1 on thighs and calves */
+    uint32_t termination_mask;          /* bit b: |F_b| > 1 ends the episode; Go1: 1 (the base) */
+    int32_t fix_base;                   /* 1: the base is welded to the world (root pose held, root twist zero) */
+    int32_t disable_gravity;            /* 1: no gravity acceleration on any body */
+    float armature;                     /* kg m^2 added to every joint's diagonal of the joint-space inertia; >= 0 */
+} Go1AssetOptions;
+int go1_sizeof_asset_options(void);
+/* Store the asset options of `sim` (go1_sim_create sets the Go1 values above).  Weights must be finite and >= 0, the mask
+ * below 2^17, armature finite and >= 0.  Only before the first go1_sim_step: captured step graphs keep their kernel
+ * arguments, so a later call fails (and leaves the options as they were). */
+int go1_sim_set_asset_options(Go1Sim* sim, const Go1AssetOptions* opt);
+
 /* Threads per CTA of the step kernel: 32, 64 or 128; 0 (default) = 32 up to 16384 envs, 128 above (tuning knob). */
 void go1_sim_set_step_block(int threads);
 

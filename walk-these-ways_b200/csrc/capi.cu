@@ -1,19 +1,20 @@
 // capi.cu — C-ABI of libgo1b200.so (declared in include/go1_b200.h): handle management, table upload,
 // error reporting.  No torch types, no hidden allocations after create, no CPU fallback.
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdio.h>
 #include <string.h>
 #include <string>
 #include "go1_layout.h"
 #include "go1_model_generated.h"
 
-extern "C" int go1_launch_step(const Go1SimBuffers*, const Go1DevTable*, const Go1SelfCollision*, const float*, const float*, const float*, long long, int, int, float*, cudaStream_t);
+extern "C" int go1_launch_step(const Go1SimBuffers*, const Go1DevTable*, const Go1SelfCollision*, const Go1AssetOptions*, const float*, const float*, const float*, long long, int, int, float*, cudaStream_t);
 extern "C" int go1_launch_reward_finish(const Go1SimBuffers*, const Go1SimConfig*, const float*, const float*, int, float*, float*, int, cudaStream_t);
 extern "C" int go1_launch_user_reward_fold(const int*, const int*, int, int, float*, float*, float*, float*, int, const int*, int, int, cudaStream_t);
 extern "C" long long go1_reward_finish_workspace_floats(int, int);
-extern "C" int go1_launch_reset(const Go1SimBuffers*, const Go1DevTable*, const int*, int, const float*, const float*, int, long long, const float*, int, cudaStream_t);
+extern "C" int go1_launch_reset(const Go1SimBuffers*, const Go1DevTable*, const int*, int, const float*, const float*, int, long long, const float*, int, int, cudaStream_t);
 extern "C" int go1_launch_set_commands(const Go1SimBuffers*, const int*, int, const float*, int, cudaStream_t);
-extern "C" int go1_launch_reset_dev(const Go1SimBuffers*, const Go1DevTable*, const int*, const int*, const float*, const float*, int, long long, const float*, float*, int, cudaStream_t);
+extern "C" int go1_launch_reset_dev(const Go1SimBuffers*, const Go1DevTable*, const int*, const int*, const float*, const float*, int, long long, const float*, float*, int, int, cudaStream_t);
 extern "C" int go1_launch_curriculum(const Go1SimBuffers*, const Go1CurriculumConfig*, const Go1CurriculumBuffers*, int, int, cudaStream_t);
 extern "C" int go1_launch_curriculum_pack(const Go1SimBuffers*, const Go1CurriculumConfig*, const Go1CurriculumBuffers*, int, cudaStream_t);
 extern "C" int go1_launch_history_roll(const float*, const float*, float*, int, int, int, cudaStream_t);
@@ -41,6 +42,7 @@ struct Go1Sim {
     int device;
     float gravity[3];
     Go1SelfCollision self;   // enabled = 0 unless go1_sim_set_self_collision turned it on
+    Go1AssetOptions asset;   // the Go1 values (go1_asset_defaults) unless go1_sim_set_asset_options replaced them
     int stepped;             // go1_sim_step has been called: the kernel choice is fixed
 };
 
@@ -55,6 +57,15 @@ extern "C" int go1_device_count(void) {
 extern "C" int go1_sizeof_config(void) { return (int)sizeof(Go1SimConfig); }
 extern "C" int go1_sizeof_buffers(void) { return (int)sizeof(Go1SimBuffers); }
 extern "C" int go1_sizeof_self_collision(void) { return (int)sizeof(Go1SelfCollision); }
+extern "C" int go1_sizeof_asset_options(void) { return (int)sizeof(Go1AssetOptions); }
+
+// config_go1's asset section (go1_gym/envs/go1/go1_config.py): penalize_contacts_on = ["thigh", "calf"],
+// terminate_after_contacts_on = ["base"], a floating base under gravity, no armature
+static void go1_asset_defaults(Go1AssetOptions* o) {
+    memset(o, 0, sizeof(*o));
+    for (int leg = 0; leg < 4; leg++) { o->penalty_weight[1 + 4 * leg + 1] = 1.f; o->penalty_weight[1 + 4 * leg + 2] = 1.f; }
+    o->termination_mask = 1u;
+}
 
 extern "C" int go1_sim_num_rows(int kind) {
     return kind == 0 ? (int)GO1_ENV_F32_ROWS : (kind == 1 ? (int)GO1_LEG_F32_ROWS : (kind == 2 ? GO1_ENV_I32_ROWS : -1));
@@ -175,6 +186,7 @@ extern "C" int go1_sim_create(const Go1SimConfig* cfg, const float* actuator_wei
     memset(&s->bufs, 0, sizeof(s->bufs));
     s->cfg = *cfg; s->bound = 0; s->device = device; s->d_tab = nullptr;
     memset(&s->self, 0, sizeof(s->self)); s->stepped = 0;
+    go1_asset_defaults(&s->asset);
     if (int e = build_table(cfg, actuator_weights, &s->h_tab)) { delete s; return e; }
     if ((ce = cudaMalloc(&s->d_tab, sizeof(Go1DevTable))) != cudaSuccess) { delete s; return cuda_fail("cudaMalloc table", ce); }
     if ((ce = cudaMemcpy(s->d_tab, &s->h_tab, sizeof(Go1DevTable), cudaMemcpyHostToDevice)) != cudaSuccess) { cudaFree(s->d_tab); delete s; return cuda_fail("upload table", ce); }
@@ -218,6 +230,18 @@ extern "C" int go1_sim_set_self_collision(Go1Sim* s, const Go1SelfCollision* sc)
     return 0;
 }
 
+extern "C" int go1_sim_set_asset_options(Go1Sim* s, const Go1AssetOptions* o) {
+    if (!s || !o) return fail("go1_sim_set_asset_options: null argument");
+    if (s->stepped) return fail("go1_sim_set_asset_options: the asset options cannot change after the first go1_sim_step");
+    for (int b = 0; b < GO1_NUM_BODIES; b++)
+        if (!(isfinite(o->penalty_weight[b]) && o->penalty_weight[b] >= 0.f)) return fail("go1_sim_set_asset_options: penalty weights must be finite and >= 0");
+    if (o->termination_mask >> GO1_NUM_BODIES) return fail("go1_sim_set_asset_options: termination_mask has bits above body 16");
+    if (!(isfinite(o->armature) && o->armature >= 0.f)) return fail("go1_sim_set_asset_options: armature must be finite and >= 0");
+    s->asset = *o;
+    s->asset.fix_base = o->fix_base ? 1 : 0; s->asset.disable_gravity = o->disable_gravity ? 1 : 0;
+    return 0;
+}
+
 extern "C" int go1_sim_step(Go1Sim* s, const float* actions, const float gravity[3], const float gravity_vec[3],
                             int64_t common_step, int mode, void* stream) {
     if (!s || !s->bound) return fail("go1_sim_step: sim not bound");
@@ -225,7 +249,7 @@ extern "C" int go1_sim_step(Go1Sim* s, const float* actions, const float gravity
     if (mode < 0 || mode > 2) return fail("go1_sim_step: bad mode");
     for (int k = 0; k < 3; k++) s->gravity[k] = gravity[k];
     s->stepped = 1;
-    int e = go1_launch_step(&s->bufs, s->d_tab, &s->self, actions, gravity, gravity_vec, (long long)common_step, mode, s->cfg.num_envs, nullptr, (cudaStream_t)stream);
+    int e = go1_launch_step(&s->bufs, s->d_tab, &s->self, &s->asset, actions, gravity, gravity_vec, (long long)common_step, mode, s->cfg.num_envs, nullptr, (cudaStream_t)stream);
     return e ? cuda_fail("go1_sim_step launch", e) : 0;
 }
 
@@ -235,7 +259,7 @@ extern "C" int go1_sim_step_deferred(Go1Sim* s, const float* actions, const floa
     if (!actions || !pre_roll) return fail("go1_sim_step_deferred: null actions / pre_roll");
     for (int k = 0; k < 3; k++) s->gravity[k] = gravity[k];
     s->stepped = 1;
-    int e = go1_launch_step(&s->bufs, s->d_tab, &s->self, actions, gravity, gravity_vec, (long long)common_step, 0, s->cfg.num_envs, pre_roll, (cudaStream_t)stream);
+    int e = go1_launch_step(&s->bufs, s->d_tab, &s->self, &s->asset, actions, gravity, gravity_vec, (long long)common_step, 0, s->cfg.num_envs, pre_roll, (cudaStream_t)stream);
     return e ? cuda_fail("go1_sim_step_deferred launch", e) : 0;
 }
 
@@ -268,7 +292,7 @@ extern "C" int go1_sim_reset_idx(Go1Sim* s, const int32_t* env_ids, int k, const
     if (k < 0 || k > s->cfg.num_envs) return fail("go1_sim_reset_idx: bad k");
     if (k == 0) return 0;
     if (!env_ids || !new_commands) return fail("go1_sim_reset_idx: null ids/commands");
-    int e = go1_launch_reset(&s->bufs, s->d_tab, env_ids, k, new_commands, actions, post_step, (long long)common_step, s->gravity, s->cfg.num_envs, (cudaStream_t)stream);
+    int e = go1_launch_reset(&s->bufs, s->d_tab, env_ids, k, new_commands, actions, post_step, (long long)common_step, s->gravity, s->asset.fix_base, s->cfg.num_envs, (cudaStream_t)stream);
     return e ? cuda_fail("go1_sim_reset_idx launch", e) : 0;
 }
 
@@ -314,7 +338,7 @@ extern "C" int go1_sim_reset_idx_dev(Go1Sim* s, const int32_t* env_ids, const in
     if (!s || !s->bound) return fail("go1_sim_reset_idx_dev: sim not bound");
     if (!env_ids || !k_dev || !new_commands) return fail("go1_sim_reset_idx_dev: null ids/count/commands");
     int e = go1_launch_reset_dev(&s->bufs, s->d_tab, env_ids, k_dev, new_commands, actions, post_step, (long long)common_step, s->gravity,
-                                 episode_acc, s->cfg.num_envs, (cudaStream_t)stream);
+                                 episode_acc, s->asset.fix_base, s->cfg.num_envs, (cudaStream_t)stream);
     return e ? cuda_fail("go1_sim_reset_idx_dev launch", e) : 0;
 }
 

@@ -126,6 +126,16 @@ class Go1SelfCollision(C.Structure):
     _fields_ = [("enabled", _i), ("k", _f), ("c", _f), ("thigh_radius", _f), ("calf_radius", _f), ("foot_radius", _f)]
 
 
+NUM_BODIES = 17
+
+
+class Go1AssetOptions(C.Structure):
+    """Asset options of a sim (go1_sim_set_asset_options): per-body collision-penalty weights and termination bits in Isaac Gym body
+    order (config.BODY_NAMES), a welded base, the gravity switch and the joint armature."""
+    _fields_ = [("penalty_weight", _f * NUM_BODIES), ("termination_mask", C.c_uint32), ("fix_base", _i), ("disable_gravity", _i),
+                ("armature", _f)]
+
+
 CUR_MAX_CATEGORIES = 8
 
 
@@ -231,6 +241,7 @@ def lib():
         "go1_sim_set_commands": ([vp, vp, ip, vp, vp], ip),
         "go1_sim_set_step_block": ([ip], None),
         "go1_sizeof_self_collision": ([], ip), "go1_sim_set_self_collision": ([vp, C.POINTER(Go1SelfCollision)], ip),
+        "go1_sizeof_asset_options": ([], ip), "go1_sim_set_asset_options": ([vp, C.POINTER(Go1AssetOptions)], ip),
         "go1_sizeof_curriculum": ([ip], ip), "go1_curriculum_set_grouped": ([ip], None),
         "go1_set_deterministic": ([ip], None), "go1_deterministic": ([], ip), "go1_deterministic_workspace_bytes": ([], i64),
         "go1_deterministic_reserve": ([vp], ip),
@@ -292,6 +303,8 @@ def lib():
         raise Go1Error("Go1SimBuffers mirror out of date")
     if L.go1_sizeof_self_collision() != C.sizeof(Go1SelfCollision):
         raise Go1Error("Go1SelfCollision mirror out of date")
+    if L.go1_sizeof_asset_options() != C.sizeof(Go1AssetOptions):
+        raise Go1Error("Go1AssetOptions mirror out of date")
     if L.go1_sizeof_curriculum(0) != C.sizeof(Go1CurriculumConfig) or L.go1_sizeof_curriculum(1) != C.sizeof(Go1CurriculumBuffers):
         raise Go1Error("Go1Curriculum* mirrors out of date")
     _lib = L

@@ -14,6 +14,9 @@ from . import capi
 
 _PKG = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 DOF_NAMES = [f"{leg}_{part}_joint" for leg in ("FL", "FR", "RL", "RR") for part in ("hip", "thigh", "calf")]
+# The 17 rigid bodies in Isaac Gym order (go1.urdf with collapse_fixed_joints: trunk and imu_link merge into base, each
+# *_thigh_shoulder into its hip): the body axis of LeggedRobot.contact_forces, of the contact-index sets and of Go1AssetOptions.
+BODY_NAMES = ["base"] + [f"{leg}_{part}" for leg in ("FL", "FR", "RL", "RR") for part in ("hip", "thigh", "calf", "foot")]
 
 
 def load_model():
@@ -217,6 +220,70 @@ def self_collision_config(cfg, k=SELF_K, c=SELF_C):
     return sc
 
 
+# Cfg.asset options that the compiled Go1 model does not simulate, with the base Cfg's values (legged_robot_config.py): a
+# different value is reported once per build_sim_config.  density, thickness, flip_visual_attachments and
+# replace_cylinder_with_capsule change nothing for this model (its masses and inertias are compiled in, its collision shapes are
+# spheres, capsules and a box, meshes are never loaded), so they are accepted silently.
+_WARN_ONLY = dict(linear_damping=0., angular_damping=0., max_linear_velocity=1000., max_angular_velocity=1000.,
+                  default_dof_drive_mode=3, collapse_fixed_joints=True)
+
+
+def _asset_get(asset, key, default):
+    """An attribute of Cfg.asset, which is a config class or, restored from parameters.pkl, possibly a plain dict."""
+    return asset.get(key, default) if isinstance(asset, dict) else getattr(asset, key, default)
+
+
+def contact_bodies(cfg):
+    """Body indices (BODY_NAMES) that Cfg.asset selects, as the reference builds them (legged_robot.py:1521-1527, 1580-1590):
+    every body whose name contains an entry, entry by entry, so a body that several entries select is listed once per entry.
+    Returns dict(penalised=[...], termination=[...], feet=[...]); feet must be exactly the four *_foot bodies."""
+    a = cfg.asset
+    pick = lambda names: [i for n in names for i, b in enumerate(BODY_NAMES) if str(n) in b]
+    foot = str(_asset_get(a, "foot_name", "None"))
+    feet = pick([foot])
+    want = [i for i, b in enumerate(BODY_NAMES) if b.endswith("_foot")]
+    if feet != want:
+        raise ValueError(f"Cfg.asset.foot_name = {foot!r} selects {[BODY_NAMES[i] for i in feet]}: the simulated Go1's feet terms and "
+                         f"contact states are defined over exactly {[BODY_NAMES[i] for i in want]}")
+    return dict(penalised=pick(_asset_get(a, "penalize_contacts_on", [])),
+                termination=pick(_asset_get(a, "terminate_after_contacts_on", [])), feet=feet)
+
+
+def asset_config(cfg, warn=True, bodies=None):
+    """Go1AssetOptions of Cfg.asset: collision-penalty weight per body (the number of penalize_contacts_on entries its name
+    contains), termination bits (terminate_after_contacts_on), fix_base_link, disable_gravity and armature.  With `warn`, prints
+    one warning per option the compiled Go1 model does not simulate (_WARN_ONLY, or a `file` other than go1.urdf).  `bodies`:
+    contact_bodies(cfg) when the caller has resolved it already."""
+    a = cfg.asset
+    bodies = contact_bodies(cfg) if bodies is None else bodies
+    o = capi.Go1AssetOptions()
+    for i in bodies["penalised"]:
+        o.penalty_weight[i] += 1.0
+    mask = 0
+    for i in bodies["termination"]:
+        mask |= 1 << i
+    o.termination_mask = mask
+    o.fix_base = int(bool(_asset_get(a, "fix_base_link", False)))
+    o.disable_gravity = int(bool(_asset_get(a, "disable_gravity", False)))
+    arm = _asset_get(a, "armature", 0.)
+    try:
+        armf = float(arm)
+    except (TypeError, ValueError):
+        armf = float("nan")
+    if not (np.isfinite(armf) and armf >= 0.):
+        raise ValueError(f"Cfg.asset.armature = {arm!r}: must be a finite float >= 0 (kg m^2 added to every joint's inertia)")
+    o.armature = armf
+    if warn:
+        f = str(_asset_get(a, "file", ""))
+        if not f.endswith("go1.urdf"):
+            print(f"Warning: Cfg.asset.file = {f!r} is not go1.urdf: the compiled Go1 model is simulated")
+        for k, default in _WARN_ONLY.items():
+            v = _asset_get(a, k, default)
+            if v != default:
+                print(f"Warning: Cfg.asset.{k} = {v!r} differs from {default!r} and is not simulated: the compiled Go1 model ignores it")
+    return o
+
+
 def build_sim_config(cfg, num_envs=None, num_train_envs=None, seed=0, physics=None, eval_cfg=None, reward_container=None):
     """Resolve `cfg` (a Cfg-like class tree) into a Go1SimConfig.  `physics` overrides solver parameters; `eval_cfg` is the
     second Cfg tree of the train/eval split (its randomisation / reset ranges apply to envs >= num_train_envs);
@@ -325,6 +392,8 @@ def build_sim_config(cfg, num_envs=None, num_train_envs=None, seed=0, physics=No
     c.pen_mt, c.limit_k, c.limit_c = 0.2, 300., 3.
     physics = dict(physics or {})
     sc = self_collision_config(cfg, physics.pop("self_k", SELF_K), physics.pop("self_c", SELF_C))
+    bodies = contact_bodies(cfg)
+    asset = asset_config(cfg, bodies=bodies)
     if physics:
         for k, v in physics.items():
             if hasattr(v, "__len__"):
@@ -342,4 +411,5 @@ def build_sim_config(cfg, num_envs=None, num_train_envs=None, seed=0, physics=No
         c.height_points_x[:len(px)] = px
         c.height_points_y[:len(py)] = py
     c.seed = int(seed)
-    return c, dict(active_reward_scales=active, user_reward_scales=user, dt=d["dt"], noise_scale_vec=nv, self_collision=sc)
+    return c, dict(active_reward_scales=active, user_reward_scales=user, dt=d["dt"], noise_scale_vec=nv, self_collision=sc,
+                   asset=asset, contact_bodies=bodies)

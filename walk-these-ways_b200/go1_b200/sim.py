@@ -15,7 +15,8 @@ from .config import load_actuator_weights
 
 
 class SimCore:
-    def __init__(self, sim_cfg: capi.Go1SimConfig, device="cuda:0", inject_noise=False, inject_reset_rand=False, self_collision=None):
+    def __init__(self, sim_cfg: capi.Go1SimConfig, device="cuda:0", inject_noise=False, inject_reset_rand=False, self_collision=None,
+                 asset=None):
         if not torch.cuda.is_available():
             raise capi.Go1Error("SimCore needs a CUDA device: the Go1 step kernel has no CPU fallback")
         self.L = capi.lib()
@@ -73,6 +74,9 @@ class SimCore:
         self.self_collision = self_collision
         if self_collision is not None and self_collision.enabled:     # only before the first step (captured graphs keep the kernel)
             capi.check(self.L.go1_sim_set_self_collision(self._handle, C.byref(self_collision)), "go1_sim_set_self_collision")
+        self.asset = asset                                             # Go1AssetOptions; None keeps the Go1 values of go1_sim_create
+        if asset is not None:                                          # also only before the first step (graphs keep kernel arguments)
+            capi.check(self.L.go1_sim_set_asset_options(self._handle, C.byref(asset)), "go1_sim_set_asset_options")
         self._bind()
         # DR defaults (legged_robot.py:1260-1278)
         self.env("motor_strengths").fill_(1.0)

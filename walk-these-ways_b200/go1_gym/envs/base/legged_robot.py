@@ -19,7 +19,7 @@ import numpy as np
 import torch
 
 from go1_b200 import capi
-from go1_b200.config import build_sim_config, cfg_dict
+from go1_b200.config import BODY_NAMES, build_sim_config, cfg_dict
 from go1_b200.sim import SimCore
 from go1_gym.envs.base.base_task import BaseTask
 from go1_gym.utils.terrain import Terrain
@@ -204,13 +204,14 @@ class LeggedRobot(BaseTask):
         self.up_axis_idx = 2
         if mesh_type in ['heightfield', 'trimesh']:
             self._bind_height_field()
-        self.core = SimCore(self.sim_cfg, device=self.device, self_collision=info["self_collision"])
+        self.core = SimCore(self.sim_cfg, device=self.device, self_collision=info["self_collision"], asset=info["asset"])
         self.num_dof = self.num_dofs = self.num_actuated_dof = 12
-        self.num_bodies = 17
+        self.num_bodies = len(BODY_NAMES)
         self.dof_names = [f"{l}_{p}_joint" for l in ("FL", "FR", "RL", "RR") for p in ("hip", "thigh", "calf")]
-        self.feet_indices = torch.tensor([4, 8, 12, 16], device=self.device)
-        self.penalised_contact_indices = torch.tensor([2, 6, 10, 14, 3, 7, 11, 15], device=self.device)
-        self.termination_contact_indices = torch.tensor([0], device=self.device)
+        bodies = info["contact_bodies"]            # Cfg.asset's sets (legged_robot.py:1521-1527, 1580-1590), as the kernel applies them
+        self.feet_indices = torch.tensor(bodies["feet"], device=self.device)
+        self.penalised_contact_indices = torch.tensor(bodies["penalised"], dtype=torch.long, device=self.device)
+        self.termination_contact_indices = torch.tensor(bodies["termination"], dtype=torch.long, device=self.device)
         self.env_origins = torch.zeros(self.num_envs, 3, device=self.device)
         self.terrain_levels = torch.zeros(self.num_envs, device=self.device, dtype=torch.long)
         self.terrain_types = torch.zeros(self.num_envs, device=self.device, dtype=torch.long)
@@ -487,12 +488,12 @@ class LeggedRobot(BaseTask):
 
     @property
     def contact_forces(self):
-        """[N, 17, 3] in Isaac Gym body order (base; per leg hip, thigh, calf, foot)."""
+        """[N, 17, 3] in Isaac Gym body order (BODY_NAMES: base; per leg hip, thigh, calf, foot)."""
         c = self.core
-        out = torch.zeros(self.num_envs, 17, 3, device=self.device)
-        out[:, 0] = c.foot_aos("base_contact_forces_part").sum(1)
-        for k, name in enumerate(("hip_contact_forces", "thigh_contact_forces", "calf_contact_forces", "foot_contact_forces")):
-            out[:, [1 + k, 5 + k, 9 + k, 13 + k]] = c.foot_aos(name)
+        out = torch.zeros(self.num_envs, len(BODY_NAMES), 3, device=self.device)
+        out[:, BODY_NAMES.index("base")] = c.foot_aos("base_contact_forces_part").sum(1)
+        for part in ("hip", "thigh", "calf", "foot"):
+            out[:, [BODY_NAMES.index(f"{leg}_{part}") for leg in ("FL", "FR", "RL", "RR")]] = c.foot_aos(f"{part}_contact_forces")
         return out
 
     @property
